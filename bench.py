@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Benchmark of the MaskDiT hot path on B200 (contract: see the task statement; one JSON line on rank 0).
+"""Benchmark of the MaskDiT hot path on H100 (one JSON line on rank 0).
 
-  python bench.py --gpus N --steps K --warmup W                 # B200 arm: MaskDiT-XL/2 ImageNet-256 train step
-  python bench.py --impl reference --gpus N --steps K --warmup W  # reference arm: the CPU path of the same workload
+  python bench.py --gpus N --steps K --warmup W                 # GPU arm: MaskDiT-XL/2 ImageNet-256 train step
+  python bench.py --impl reference --gpus N --steps K --warmup W  # reference arm: the CPU oracle port of the same workload
   python bench.py --workload sampler                            # EDM sampler, 18 steps, CFG 1.5, batch 64
 
 A "step" = EDMLoss forward + hand-written backward + (N>1: one NCCL all-reduce of the flat fp32 gradient) +
@@ -10,6 +10,9 @@ fused AdamW + EMA, on synthetic latents of BASELINE.json's shape with random-ini
 zero-initialised tensors are randomised, SURVEY.md §3.3 — otherwise the net is the identity).
 `value`  : samples/s, inputs resident in HBM.      `e2e.value`: same, inputs copied from pinned host memory
 every step and the loss read back to the host every step.
+`--dump-outputs DIR`: after the timed steps, what the last timed step computed is written as DIR/<name>.npy, so that
+two builds can be compared output for output on identical inputs: for training the per-sample loss and a fixed, seeded
+sample of the trained and EMA weights it left behind (float32); for `--workload sampler` the sampled latents (float64).
 """
 from __future__ import annotations
 
@@ -35,7 +38,8 @@ def peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return dict(burst=p["bf16_tflops"], sustained=p["bf16_tflops_sustained"], hbm=p["hbm_gbs"], src="measured")
     except Exception:
-        return dict(burst=1590.0, sustained=1400.0, hbm=6650.0, src="fallback")
+        # H100 SXM data sheet (dense bf16, HBM3 at 700 W): a reference point, not a measured rate
+        return dict(burst=989.0, sustained=989.0, hbm=3350.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -176,68 +180,9 @@ def cpu_reference_eval(R=32):
     return fwd, B / (35 * per_eval)
 
 
-REF_DIR = os.path.join(ROOT, "baseline", "_ref")
-
-
-def have_unmodified_reference():
-    return os.path.exists(os.path.join(REF_DIR, "models", "maskdit.py"))
-
-
-def cpu_reference_train_unmodified(B, steps, warmup, R=32):
-    """The UNMODIFIED reference (`models/maskdit.py` + `train_utils/loss.py`, staged from /root/reference into the
-    git-ignored baseline/_ref/ by `__graft_entry__.build()`), imported through the timm stand-in, fp32, PyTorch CPU backend,
-    `torch.optim.AdamW(weight_decay=0)` in place of apex FusedAdam, the net wrapped to expose `.module` as the loss
-    expects (loss.py:47) - BASELINE.md section 3.  Zero-initialised tensors randomised N(0, 0.02) like the GPU run."""
-    from oracle import timm_standin
-    timm_standin.install()
-    if REF_DIR not in sys.path:
-        sys.path.insert(0, REF_DIR)
-    import models.maskdit as rm
-    import train_utils.loss as rl
-    torch.manual_seed(0)
-    net = rm.Precond_models["edm"](img_resolution=R, img_channels=4, num_classes=1000, model_type="DiT-XL/2",
-                                   use_decoder=True, mae_loss_coef=0.1, pad_cls_token=False).train()
-    randomise_zero_init(net)
-
-    class Wrap:
-        def __init__(self, m):
-            self.module, self.model, self.training = m, m.model, True
-
-        def __call__(self, *a, **k):
-            return self.module(*a, **k)
-
-    wrap, loss_fn = Wrap(net), rl.Losses["edm"]()
-    opt = torch.optim.AdamW([p for p in net.parameters() if p.requires_grad], lr=1e-4, weight_decay=0)
-    g = torch.Generator().manual_seed(0)
-    times = []
-    for it in range(warmup + steps):
-        x = torch.randn(B, 4, R, R, generator=g) * 0.5
-        y = torch.nn.functional.one_hot(torch.randint(0, 1000, (B,), generator=g), 1000).float()
-        t0 = time.perf_counter()
-        opt.zero_grad(set_to_none=True)
-        loss = loss_fn(net=wrap, images=x, labels=y, mask_ratio=0.5, mae_loss_coef=0.1)
-        loss.mean().backward()
-        opt.step()
-        if it >= warmup:
-            times.append(time.perf_counter() - t0)
-    return B * len(times) / sum(times), sum(times)
-
-
-def cpu_baseline_record(steps, warmup, R=32, B=8, extras=False, prefer_unmodified=False):
+def cpu_baseline_record(steps, warmup, R=32, B=8, extras=False):
+    """CPU arm: the oracle port (oracle/maskdit_oracle.py, pinned to the unmodified reference by tests/golden)."""
     threads, how = pin_to_one_socket()
-    if prefer_unmodified and have_unmodified_reference():
-        sps, secs = cpu_reference_train_unmodified(B, steps, warmup, R=R)
-        extra = {}
-        if extras:
-            fwd, ips = cpu_reference_eval(R)
-            extra = {"c1_forward_b2": {"value": fwd, "unit": "samples/s", "kind": "port"},
-                     "c5_sampler_b2_scaled": {"value": ips, "unit": "img/s", "kind": "port",
-                                              "how": "3 CFG network evaluations at B=2 timed, scaled to the 35 of an 18-step run"}}
-        return sps, secs, {**extra, "value": sps, "unit": "samples/s", "cores": threads, "kind": "reference", "same_config": False,
-                           "sample": f"{steps} timed steps (+{warmup} warm-up) of batch {B} (SURVEY 8d): the UNMODIFIED "
-                                     f"reference modules (models/maskdit.py + train_utils/loss.py staged in baseline/_ref, "
-                                     f"timm stand-in), EDM loss fwd + bwd + torch AdamW(wd=0), torch CPU fp32, {threads} "
-                                     f"threads {how}; host has {os.cpu_count()} logical CPUs; {secs:.1f} s timed"}
     sps, secs = cpu_reference_train(B, steps, warmup, R=R)
     extra = {}
     if extras:
@@ -248,8 +193,8 @@ def cpu_baseline_record(steps, warmup, R=32, B=8, extras=False, prefer_unmodifie
     return sps, secs, {**extra, "value": sps, "unit": "samples/s", "cores": threads, "kind": "port", "same_config": False,
                        "sample": f"{steps} timed steps (+{warmup} warm-up) of batch {B} (SURVEY 8d), EDM loss fwd + bwd + "
                                  f"AdamW, torch CPU fp32, {threads} threads {how}; host has {os.cpu_count()} logical "
-                                 f"CPUs; {secs:.1f} s timed.  /root/reference is not on the GPU box: the oracle port "
-                                 "(pinned to the unmodified reference by tests/golden) is what runs"}
+                                 f"CPUs; {secs:.1f} s timed; the oracle port, pinned to the unmodified reference by "
+                                 "tests/golden"}
 
 
 def run_reference_arm(args, rank):
@@ -257,7 +202,7 @@ def run_reference_arm(args, rank):
         return
     R = 64 if args.workload == "train512" else 32
     B = 8 if R == 32 else 2
-    sps, secs, rec = cpu_baseline_record(args.steps, max(1, min(args.warmup, 2)), R=R, B=B, prefer_unmodified=True)
+    sps, secs, rec = cpu_baseline_record(args.steps, max(1, min(args.warmup, 2)), R=R, B=B)
     line = {"impl": "reference", "metric": "train_samples_per_sec", "value": sps, "unit": "samples/s",
             "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup, "ms_per_step": 1e3 * secs / args.steps,
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
@@ -266,22 +211,6 @@ def run_reference_arm(args, rank):
             "cpu_baseline": rec,
             "e2e": {"value": sps, "unit": "samples/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     print(json.dumps(line), flush=True)
-
-
-def gemm_traffic():
-    """DRAM read+write bytes per GEMM launch from the committed `ncu --set full` capture (never a constant in code)."""
-    for name in ("r02_gemm_ncu_full_v2.json", "r02_gemm_ncu_full.json", "r01_gemm_ncu_full_v3.json"):
-        f = os.path.join(ROOT, "profiles", name)
-        try:
-            d = json.load(open(f))
-            rows = d["launches"] if isinstance(d, dict) else d
-            vals = [r["dram_bytes"] if "dram_bytes" in r else 1e6 * (r["dram_read_MB"] + r["dram_write_MB"])
-                    for r in rows if "dram_bytes" in r or "dram_read_MB" in r]
-            if vals:
-                return sum(vals) / len(vals), f"profiles/{name} (mean of {len(vals)} launches inside a step)"
-        except Exception:
-            continue
-    return None, "no ncu --set full capture found under profiles/"
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -334,6 +263,8 @@ def main():
     ap.add_argument("--workload", default="train256", choices=["train256", "train512", "sampler"])
     ap.add_argument("--batch-per-gpu", type=int, default=None)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs as DIR/<name>.npy (training: float32; sampler: float64 latents)")
     ap.add_argument("--no-sub", action="store_true",
                     help="skip the sub-records (BASELINE configs 3-5: 128/GPU, 64x64x4 latents, sampler)")
     args = ap.parse_args()
@@ -358,7 +289,7 @@ def main():
     if args.workload == "sampler":
         line = bench_sampler(args, net, env, PK)
     else:
-        line = bench_train(args, net, env, R, PK, args.batch_per_gpu or (256 if R == 32 else 128), args.steps,
+        line = bench_train(args, net, env, R, PK, args.batch_per_gpu or (256 if R == 32 else 64), args.steps,
                            args.warmup, full=True)
         if args.workload == "train256" and not args.no_sub and args.batch_per_gpu is None:
             # BASELINE.json configs 3, 4, 5 next to the headline (config 2), same process, same box, same clocks
@@ -382,7 +313,8 @@ def main():
                 net64 = None
                 try:
                     net64 = build_xl2(64, dev)
-                    return bench_train(args, net64, env, 64, PK, 128, max(4, args.steps // 4), 3, full=False)
+                    # batch 64: the largest the 80 GB of an H100 holds at 512 px (batch 128 needs a 108 GB workspace)
+                    return bench_train(args, net64, env, 64, PK, 64, max(4, args.steps // 4), 3, full=False)
                 finally:
                     net64 = None
                     torch.cuda.empty_cache()
@@ -402,8 +334,7 @@ def main():
             del os.environ["MDT_GRAD_AR"]
             torch.cuda.empty_cache()
         if rank == 0 and world == 1 and not args.no_cpu_baseline:
-            _, _, line["cpu_baseline"] = cpu_baseline_record(3, 1, R=R, B=8 if R == 32 else 2, extras=(R == 32),
-                                                             prefer_unmodified=True)
+            _, _, line["cpu_baseline"] = cpu_baseline_record(3, 1, R=R, B=8 if R == 32 else 2, extras=(R == 32))
     if rank == 0:
         print(json.dumps(line), flush=True)
     if world > 1:
@@ -427,9 +358,12 @@ def bench_train(args, net, env, R, PK, B, steps, warmup, full):
     h2d = pool[0][0].numel() * 4 + pool[0][1].numel() * 4
     loss_host = torch.zeros(1).pin_memory()
 
+    last = {}
+
     def step_resident(i):
         x, y = resident[i % len(resident)]
-        return ts.step(x, y, 0.5, 0.1)
+        last["loss"] = ts.step(x, y, 0.5, 0.1)
+        return last["loss"]
 
     def step_e2e(i):
         xh, yh = pool[i % len(pool)]
@@ -446,6 +380,8 @@ def bench_train(args, net, env, R, PK, B, steps, warmup, full):
     ms = env.timed(step_resident, steps)
     launches = _lib.LAUNCHES - n0
     clk = clocks.stop() if (rank == 0 and full) else None
+    if full and rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, last["loss"], ts)
     ms_step = ms / steps
     sps = B * world * steps / (ms / 1e3)
     flop = FLOP_PER_SAMPLE[256 if R == 32 else 512]
@@ -468,7 +404,7 @@ def bench_train(args, net, env, R, PK, B, steps, warmup, full):
     ms_e2e = env.timed(step_e2e, steps)
     final_loss = float(loss_host.item())
 
-    # dominant kernel (the tcgen05 GEMM family) timed per launch with CUDA events inside real steps: the library brackets
+    # dominant kernel (the wgmma GEMM family) timed per launch with CUDA events inside real steps: the library brackets
     # every mdt_gemm_bf16 launch - the C++ step driver's own - with an event pair on the launching stream
     # (mdt_gemm_profile_enable); three steps, per launch the median of the three.
     import ctypes
@@ -489,22 +425,21 @@ def bench_train(args, net, env, R, PK, B, steps, warmup, full):
     gemm_flops = sum(f for f, _ in prof)
     sps_e2e = B * world * steps / (ms_e2e / 1e3)
     achieved = gemm_flops / (gemm_ms * 1e-3) / 1e12 if gemm_ms > 0 else 0.0
-    traffic, traffic_src = gemm_traffic() if (R == 32 and B == 256) else (None, "no capture for this configuration")
     line = {
         "metric": "train_samples_per_sec", "value": sps, "unit": "samples/s", "n_gpus": world, "steps": steps,
         "warmup": warmup, "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak",
         "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
         "config": {"workload": workload, "batch_per_gpu": B, "global_batch": B * world, "parallelism": f"dp{world}",
                    "grad_allreduce": ts.describe_collective(),
-                   "l2_policy": "per-step working set (activations > 40 GB) far exceeds the 126 MB L2; no flush needed",
+                   "l2_policy": "per-step working set (activations > 40 GB) far exceeds the 50 MB L2; no flush needed",
                    "final_loss": final_loss},
         "clocks": clk,
         "e2e": {"value": sps_e2e, "unit": "samples/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4},
         "gpu_launches": launches,
-        "roofline": {"bound": "tensor", "kernel": "gemm_tcgen05_kernel (all GEMM launches of one step)",
+        "roofline": {"bound": "tensor", "kernel": "gemm_wgmma_kernel (all GEMM launches of one step)",
                      "achieved": achieved, "peak": PK["sustained"], "unit": "TFLOP/s",
                      "frac": achieved / PK["sustained"], "peak_source": f"{PK['src']} sustained bf16",
-                     "traffic": traffic, "traffic_source": traffic_src,
+                     "traffic": None, "traffic_source": "not measured on this GPU",
                      "launches_per_step": len(prof), "share_of_step": gemm_ms / ms_step,
                      "step_achieved": step_tf, "step_frac": step_tf / PK["sustained"]},
     }
@@ -512,6 +447,21 @@ def bench_train(args, net, env, R, PK, B, steps, warmup, full):
     del ts, ema, resident
     torch.cuda.empty_cache()
     return line
+
+
+def dump_outputs(out_dir, loss, ts, n_sample=1 << 20, seed=0):
+    """What the timed training step hands back: the per-sample loss, plus the weights and EMA weights it updated
+    (a fixed seeded sample of n_sample entries of each flat fp32 store; 8 MB in all at the default)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    np.save(os.path.join(out_dir, "loss.npy"), loss.float().cpu().numpy())
+    n = ts.st.n_train
+    g = torch.Generator().manual_seed(seed)
+    idx = torch.randint(0, n, (min(n_sample, n),), generator=g).to(ts.st.w32.device)
+    np.save(os.path.join(out_dir, "weights_sample.npy"), ts.st.w32[:n][idx].float().cpu().numpy())
+    if ts.ema_st is not None:
+        np.save(os.path.join(out_dir, "ema_weights_sample.npy"), ts.ema_st.w32[:n][idx].float().cpu().numpy())
 
 
 def bench_sampler(args, net, env, PK, iters=None, warm=None):
@@ -540,6 +490,11 @@ def bench_sampler(args, net, env, PK, iters=None, warm=None):
         clocks.start()
     n0 = _lib.LAUNCHES
     ms = env.timed(run, K)
+    if args.dump_outputs and args.workload == "sampler" and rank == 0:  # the sampled latents of the last timed run
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        torch.cuda.synchronize()
+        np.save(os.path.join(args.dump_outputs, "latents.npy"), out_h.numpy())
     ips = B * world * K / (ms / 1e3)
     ach = ips / world * SAMPLER_FLOP_PER_IMAGE / 1e12
     return {"metric": "edm_sampler_imgs_per_sec", "value": ips, "unit": "img/s", "n_gpus": world, "steps": K,

@@ -2,7 +2,7 @@
 """Sampling entry point with the reference's CLI / YAML surface (generate.py:54-87, configs/test/*.yaml).
 
 Builds `Precond_models[config.model.precond]` from the YAML, loads `ckpt['ema']` (reference checkpoints load
-unchanged: same state-dict keys), and runs `edm_sampler` on the B200 engine for the requested seeds with
+unchanged: same state-dict keys), and runs `edm_sampler` on the H100 engine for the requested seeds with
 per-sample generators (utils.StackedRandomGenerator, utils.py:119-133).  Under torchrun the seed batches are dealt
 to the ranks exactly as generate_with_net does (sample.py:232-235: rank-strided, one barrier per batch); giving any of
 --solver / --discretization / --schedule / --scaling selects `ablation_sampler` (sample.py:243-245).  The SD-VAE

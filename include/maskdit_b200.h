@@ -1,4 +1,4 @@
-/* maskdit_b200 — C ABI of the B200 (sm_100a) MaskDiT hot path.
+/* maskdit_b200 — C ABI of the H100 (sm_90a) MaskDiT hot path.
  *
  * The reference (Anima-Lab/MaskDiT) is pure Python/PyTorch and has no FFI layer; its seam for this path is the
  * Python registries `Precond_models`, `DiT_models` (models/maskdit.py:709-715,779-781), `Losses`
@@ -27,14 +27,14 @@ extern "C" {
 
 const char* mdt_status_string(int status);
 int mdt_abi_version(void);
-/* BLOCK_N * 10 + CTAs-per-tile (1 or 2 = tcgen05 cta_group::2 SM pair) of the last mdt_gemm_bf16 launch (tests). */
+/* BLOCK_N * 10 + CTAs-per-tile (always 1) of the last mdt_gemm_bf16 launch (tests). */
 int mdt_gemm_last_config(void);
 /* Bit set of the GEMM instances launched since the last reset: bit (BLOCK_N/64 - 2) * 2 + (CTAs - 1), i.e. 128/1 = 0,
  * 128/2 = 1, 192/1 = 2, 192/2 = 3, 256/1 = 4, 256/2 = 5.  reset != 0 clears it after reading.                        */
 int mdt_gemm_configs_seen(int reset);
 
 /* ------------------------------------------------------------------------------------------------------------
- * bf16 tensor-core GEMM (tcgen05 / TMEM / TMA):  out[M,N] (+)= sum_k A[m,k] * B[n,k], fp32 accumulate.
+ * bf16 tensor-core GEMM (wgmma / TMA):  out[M,N] (+)= sum_k A[m,k] * B[n,k], fp32 accumulate.
  * Replaces every nn.Linear forward and its autograd dgrad/wgrad: timm Attention.qkv/proj and Mlp.fc1/fc2
  * (ctor sites models/maskdit.py:178,182), adaLN_modulation (:185,206,227), DecoderLayer.linear (:203),
  * FinalLayer.linear (:224), TimestepEmbedder.mlp (:34-38), LabelEmbedder.embedding_table (:75).
@@ -75,7 +75,7 @@ typedef struct mdt_gemm_args {
 int mdt_gemm_bf16(const mdt_gemm_args* args, void* stream);
 /* The host-side decisions mdt_gemm_bf16 would take for `args`, without launching anything (needs no device: host
  * tests pin the dispatch with it; pointers in `args` are only checked for alignment, never dereferenced):
- * out10 = {BLOCK_N, CTAs per tile (2 = cta_group::2 SM pair), k-slices, paired half-tile order (0/1), half-width last
+ * out10 = {BLOCK_N, CTAs per tile (always 1), k-slices, paired half-tile order (0/1), half-width last
  * column tile (0/1), row tiles, column tiles, k-blocks of 64, work units, grid size in CTAs}.                        */
 int mdt_gemm_plan(const mdt_gemm_args* args, long long* out10);
 /* Measurement aid (bench.py roofline): while enabled, every mdt_gemm_bf16 launch of this process - also the step
@@ -158,10 +158,7 @@ int mdt_attention_bwd(const void* qkv, const void* out, const void* dout, const 
                       int H, int dh, void* stream);
 /* Introspection for the parity tests (host-side, no launch): which kernel family served the last successful
  * mdt_attention_fwd (which = 0) / mdt_attention_bwd (which = 1) call of this process:
- *   0 mma.sync fallback (odd sequence lengths), 1 split-tile TMA tcgen05 (T = 128/256), 2 no-swizzle tcgen05,
- *   3 blocked split-tile tcgen05 (T = 512/1024, T = 256 backward), 4 blocked no-swizzle tcgen05; -1 = none yet.
- * With MDT_ATTN_STRICT=1 in the environment a shape no tcgen05 kernel accepts returns MDT_ERR_UNSUPPORTED instead
- * of running the mma.sync kernels.                                                                             */
+ *   0 mma.sync kernels (T not a multiple of 64, other head_dims), 1 wgmma + TMA kernels; -1 = none yet.          */
 int mdt_attention_last_impl(int which);
 /* Log of every attention call since the last reset, 4 ints per call: (which, T, head_dim, kernel family).  Returns
  * the number of entries copied (<= cap); out4 == NULL resets the log.  The step driver's internal calls are logged too. */
@@ -242,7 +239,7 @@ int mdt_adamw_ema_g16(float* w, const void* g_bf16, float* m, float* v, float* e
                       float lr, float beta1, float beta2, float eps, float weight_decay, int step, float ema_decay,
                       float grad_scale, int max_blocks, void* stream);
 
-/* Cap on the SMs the persistent kernels (tcgen05 GEMM, persistent attention backward) occupy: n > 0 sizes their grids
+/* Cap on the SMs the persistent kernels (the wgmma GEMM) occupy: n > 0 sizes their grids
  * for n SMs instead of the device's count, leaving the rest to a concurrently running collective (the gradient
  * all-reduce overlapped with the backward); 0 = whole device.  Host-side setting, read at launch.                  */
 int mdt_set_sm_budget(int n);

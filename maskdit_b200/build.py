@@ -1,4 +1,4 @@
-"""Build the in-tree CUDA library (`maskdit_b200/libmaskdit_b200.so`) for sm_100a with nvcc.
+"""Build the in-tree CUDA library (`maskdit_b200/libmaskdit_b200.so`) for sm_90a (H100) with nvcc.
 
 nvcc cross-compiles without a GPU, so this runs in the CPU container; the .so then travels to the GPU box with
 the repo snapshot.  Objects are rebuilt only when a source or header is newer than the object.
@@ -16,7 +16,7 @@ BUILD = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libmaskdit_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC",
 ]
 

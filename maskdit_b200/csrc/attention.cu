@@ -3,9 +3,10 @@
 //
 //   qkv [B, T, 3, H, dh] bf16  ->  out [B, T, H*dh] bf16,  lse [B, H, T] fp32 (natural-log-sum-exp of scaled scores)
 //
-// Round-1 implementation: flash-style tiles on the warp-level tensor-core path (mma.sync m16n8k16 bf16, ldmatrix),
-// fp32 online softmax.  Attention is 2.4 % of the step's FLOPs (SURVEY.md §8); the tcgen05/TMEM version (S tile in
-// TMEM, head_dim 72 padded to 80 in smem) is the planned replacement once the GEMM path is at roofline.
+// The production shapes (T a multiple of 64, head_dim 32 / 64 / 72) run on the wgmma + TMA kernels of
+// attention_wgmma.cu.  This file holds the dispatch and the general kernels for every other shape (odd token counts of
+// class-unconditional or differently masked inputs): flash-style tiles on the warp-level tensor-core path (mma.sync
+// m16n8k16 bf16, ldmatrix), fp32 online softmax.
 // head_dim is zero-padded to DP (multiple of 16) in shared memory; rows are padded by 8 elements so that ldmatrix
 // is bank-conflict free.
 //
@@ -357,45 +358,13 @@ attn_bwd_dkv_kernel(const __nv_bfloat16* __restrict__ qkv, const __nv_bfloat16* 
 }  // namespace mdt
 
 namespace mdt {
-// tcgen05 kernels (attention_tc.cu); MDT_ERR_UNSUPPORTED = shape outside their range -> mma.sync kernels below
-int attention_tc_fwd(const void* qkv, void* out, float* lse, int B, int T, int H, int dh, float scale, cudaStream_t st);
-int attention_tc_bwd(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, int B, int T,
-                     int H, int dh, float scale, cudaStream_t st);
-// attention_sw.cu: head_dim 64 / 72 with TMA-friendly split tiles (T = 128 / 256)
-int attention_sw_fwd(const void* qkv, void* out, float* lse, int B, int T, int H, int dh, float scale, cudaStream_t st);
-int attention_sw_bwd(const void* qkv, const void* out, const void* dout, const float* lse, void* dqkv, int B, int T,
-                     int H, int dh, float scale, cudaStream_t st);
-// attention_sw_long.cu: the blocked kernels on split TMA tiles (default; MDT_ATTN_SWL=0 = attention_tc_long.cu)
-int attention_sw_long_fwd(const void* qkv, void* out, float* lse, int B, int T, int H, int dh, float scale,
-                          cudaStream_t st);
-int attention_sw_long_bwd(const void* qkv, const void* out, const void* dout, const float* lse, float* delta,
-                          void* dqkv, int B, int T, int H, int dh, float scale, cudaStream_t st);
-// attention_tc_long.cu: T = 512 / 1024 (and the T = 256 backward the persistent kernel does not cover)
-int attention_tc_long_fwd(const void* qkv, void* out, float* lse, int B, int T, int H, int dh, float scale,
-                          cudaStream_t st);
-int attention_tc_long_bwd(const void* qkv, const void* out, const void* dout, const float* lse, float* delta,
-                          void* dqkv, int B, int T, int H, int dh, float scale, cudaStream_t st);
+// attention_wgmma.cu: T a multiple of 64, head_dim 32 / 64 / 72; MDT_ERR_UNSUPPORTED otherwise -> the kernels above
+int attention_wg_fwd(const void* qkv, void* out, float* lse, int B, int T, int H, int dh, float scale, cudaStream_t st);
+int attention_wg_bwd(const void* qkv, const void* out, const void* dout, const float* lse, float* delta, void* dqkv,
+                     int B, int T, int H, int dh, float scale, cudaStream_t st);
 }  // namespace mdt
 
 using namespace mdt;
-
-static bool use_tc() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MDT_ATTN_TC");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
-
-static bool use_tc_long() {  // MDT_ATTN_LONG=0: T >= 512 stays on the mma.sync kernels (A/B switch)
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MDT_ATTN_LONG");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v == 1;
-}
 
 static int dp_of(int dh) {
   if (dh % 8) return 0;
@@ -414,9 +383,8 @@ static int dp_of(int dh) {
   }
 
 // Which implementation served the last call (tests assert the production kernels ran instead of trusting the
-// fallthrough chain): 0 = mma.sync (attention.cu), 1 = split-tile TMA tcgen05 (attention_sw.cu), 2 = no-swizzle
-// tcgen05 (attention_tc.cu), 3 = blocked split-tile tcgen05 (attention_sw_long.cu), 4 = blocked no-swizzle tcgen05
-// (attention_tc_long.cu).  MDT_ATTN_STRICT=1: a shape none of the tcgen05 paths accepts is an error, not a fallback.
+// fallthrough): 0 = mma.sync (this file: sequence lengths that are not a multiple of 64, other head_dims), 1 = wgmma +
+// TMA (attention_wgmma.cu).
 static int g_attn_last_impl[2] = {-1, -1};
 constexpr int kAttnLogCap = 1024;
 static int g_attn_log[kAttnLogCap][4];  // (which, T, head_dim, impl) of every call since the last reset
@@ -428,18 +396,6 @@ static void attn_log(int which, int T, int dh, int impl) {
     e[0] = which, e[1] = T, e[2] = dh, e[3] = impl;
   }
 }
-static bool attn_strict() {
-  static const bool on = [] { const char* e = getenv("MDT_ATTN_STRICT"); return e && e[0] == '1'; }();
-  return on;
-}
-#define MDT_ATTN_TRY(WHICH, IMPL, CALL)                                  \
-  {                                                                      \
-    const int rc_ = (CALL);                                              \
-    if (rc_ != MDT_ERR_UNSUPPORTED) {                                    \
-      if (rc_ == MDT_OK) attn_log(WHICH, T, dh, IMPL);                   \
-      return rc_;                                                        \
-    }                                                                    \
-  }
 
 extern "C" {
 
@@ -463,15 +419,12 @@ int mdt_attention_fwd(const void* qkv, void* out, float* lse, int B, int T, int 
   if ((reinterpret_cast<uintptr_t>(qkv) & 15) || (reinterpret_cast<uintptr_t>(out) & 15)) return MDT_ERR_ARG;
   dim3 grid((T + kTile - 1) / kTile, B * H);
   const float scale = 1.f / sqrtf(static_cast<float>(dh));
-  if (use_tc()) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    MDT_ATTN_TRY(0, 1, attention_sw_fwd(qkv, out, lse, B, T, H, dh, scale, st));
-    MDT_ATTN_TRY(0, 2, attention_tc_fwd(qkv, out, lse, B, T, H, dh, scale, st));
-    if (use_tc_long()) {
-      MDT_ATTN_TRY(0, 3, attention_sw_long_fwd(qkv, out, lse, B, T, H, dh, scale, st));
-      MDT_ATTN_TRY(0, 4, attention_tc_long_fwd(qkv, out, lse, B, T, H, dh, scale, st));
+  {
+    const int rc = attention_wg_fwd(qkv, out, lse, B, T, H, dh, scale, static_cast<cudaStream_t>(stream));
+    if (rc != MDT_ERR_UNSUPPORTED) {
+      if (rc == MDT_OK) attn_log(0, T, dh, 1);
+      return rc;
     }
-    if (attn_strict()) return MDT_ERR_UNSUPPORTED;
   }
   attn_log(0, T, dh, 0);
   MDT_DP_DISPATCH(dp, attn_fwd_kernel<kDP><<<grid, 128, 0, static_cast<cudaStream_t>(stream)>>>(
@@ -490,14 +443,12 @@ int mdt_attention_bwd(const void* qkv, const void* out, const void* dout, const 
   const float scale = 1.f / sqrtf(static_cast<float>(dh));
   float* delta = const_cast<float*>(lse) + static_cast<size_t>(B) * H * T;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (use_tc()) {
-    MDT_ATTN_TRY(1, 1, attention_sw_bwd(qkv, out, dout, lse, dqkv, B, T, H, dh, scale, st));
-    MDT_ATTN_TRY(1, 2, attention_tc_bwd(qkv, out, dout, lse, dqkv, B, T, H, dh, scale, st));
-    if (use_tc_long()) {
-      MDT_ATTN_TRY(1, 3, attention_sw_long_bwd(qkv, out, dout, lse, delta, dqkv, B, T, H, dh, scale, st));
-      MDT_ATTN_TRY(1, 4, attention_tc_long_bwd(qkv, out, dout, lse, delta, dqkv, B, T, H, dh, scale, st));
+  {
+    const int rc = attention_wg_bwd(qkv, out, dout, lse, delta, dqkv, B, T, H, dh, scale, st);
+    if (rc != MDT_ERR_UNSUPPORTED) {
+      if (rc == MDT_OK) attn_log(1, T, dh, 1);
+      return rc;
     }
-    if (attn_strict()) return MDT_ERR_UNSUPPORTED;
   }
   attn_log(1, T, dh, 0);
   MDT_DP_DISPATCH(dp, {

@@ -618,7 +618,7 @@ int mdt_timestep_freq(const float* sigma, int B, int dim, void* out_bf16, void* 
 static int ew_grid(long long n, int per_thread = 1) {
   long long blocks = (n / per_thread + 255) / 256;
   if (blocks < 1) blocks = 1;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > kNumSMsDefault * 16) blocks = kNumSMsDefault * 16;
   return static_cast<int>(blocks);
 }
 

@@ -1,4 +1,4 @@
-// Internal declarations shared by gemm_tcgen05.cu and api.cu.
+// Internal declarations shared by gemm_wgmma.cu and api.cu.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -39,15 +39,10 @@ struct GemmPlan {
 };
 int gemm_plan(const mdt_gemm_args& a, GemmPlan* out);
 
-// Tensor map that makes TMA write attention token tiles directly in the UMMA no-swizzle core-matrix layout
-// (attention_tc.cuh): a row-major bf16 matrix [rows, row_elems] is described as the 4-D tensor
-// {8 elements (16 B), 8 rows, row_elems/8 chunks, rows/8 row blocks}; a box {8, 8, chunks, row_blocks} lands in smem as
-// [row block][chunk][row % 8][16 B].  `m` is a CUtensorMap (opaque here to keep cuda.h out of this header).
-int make_token_tile_tmap(void* m, const void* ptr, unsigned long long rows, unsigned long long row_elems,
-                         unsigned box_chunks, unsigned box_row_blocks);
-// 2-D bf16 tensor map of a row-major matrix [rows, row_elems], box {box_cols, box_rows}: SWIZZLE_128B for
-// box_cols = 64, SWIZZLE_64B for box_cols = 32.
-int make_row_tile_tmap(void* m, const void* ptr, unsigned long long rows, unsigned long long row_elems,
-                       unsigned box_cols, unsigned box_rows);
+// Tensor map of one head's columns in a token-major bf16 matrix [rows, heads * dh]: the 3-D tensor {dh, heads, rows};
+// a box {64, 1, 64} lands in smem as 64 rows x 128 B, SWIZZLE_128B, columns >= dh zero-filled.  `m` is a CUtensorMap
+// (opaque here to keep cuda.h out of this header).
+int make_head_tile_tmap(void* m, const void* ptr, unsigned long long dh, unsigned long long heads,
+                        unsigned long long rows);
 
 }  // namespace mdt

@@ -358,7 +358,7 @@ static int adamw_launch(bool g16, float* w, const void* g, float* m, float* v, f
   const float inv_bc1 = static_cast<float>(1.0 / (1.0 - pow(static_cast<double>(beta1), step)));
   const float inv_bc2 = static_cast<float>(1.0 / (1.0 - pow(static_cast<double>(beta2), step)));
   long long blocks = (n / 4 + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > kNumSMsDefault * 8) blocks = kNumSMsDefault * 8;
   if (max_blocks > 0 && blocks > max_blocks) blocks = max_blocks;
   auto kern = g16 ? adamw_ema_kernel<true> : adamw_ema_kernel<false>;
   kern<<<static_cast<int>(blocks), 256, 0, S(stream)>>>(w, g, m, v, ema, static_cast<__nv_bfloat16*>(w_bf16), n, lr,
@@ -392,7 +392,7 @@ int mdt_step_front(const float* moments, const float* eps, const float* rnd_norm
     return MDT_ERR_ARG;
   const long long total = static_cast<long long>(B) * C * (R * R / 4);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > kNumSMsDefault * 8) blocks = kNumSMsDefault * 8;
   step_front_kernel<<<static_cast<int>(blocks), 256, 0, S(stream)>>>(moments, eps, rnd_normal, noise_unit, drop_u,
                                                                      drop_prob, scale_factor, P_mean, P_std, y, yn,
                                                                      sigma, labels, B, C, R * R / 4, num_classes);

@@ -1,4 +1,4 @@
-// Work-unit order of the persistent GEMM (gemm_tcgen05.cu).  Plain C++ so that the host-side test
+// Work-unit order of the persistent GEMM (gemm_wgmma.cu).  Plain C++ so that the host-side test
 // (tests/test_unit_sched.py) compiles the very same code with g++ and checks coverage and balance.
 #pragma once
 #include "gemm.h"
@@ -32,7 +32,7 @@ struct UnitSched {
   // fc2 263 us vs 240 us for the same-flop fc1 dgrad); now it is 8.0.
   // Paired order (p.pair_halves, used for the non-accumulating epilogues): LPT leaves ALL half-width tiles for the end
   // of the launch, when the A panels they need (the whole activation matrix: 226-302 MB for the K = 3456 / 4608
-  // GEMMs) have long left the 126 MB L2 - ncu r02: fc2 forward reads 1054 MB from DRAM against 690 MB algorithmic, and
+  // GEMMs) have long left the L2 (the fc2 forward then reads its A panels from DRAM more than once), and
   // the tail (74 pairs, each streaming a private 256-row A panel for half a tile-time of MMAs) is DRAM-bound.  Here
   // the tiles stay in m-major order and the two half tiles of an m-panel PAIR form one unit (walked back to back by the
   // same CTA group): every unit costs one full tile-time again (makespan 8.0 for N = 1152, as with LPT) and a panel's

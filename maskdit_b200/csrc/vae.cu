@@ -3,7 +3,7 @@
 // one single-head AttnBlock, nearest-2x Upsample + conv, norm_out + conv_out).
 //
 // Layout: activations are pixel-major ("NHWC") fp32 row matrices [B*H*W, C], so every convolution is a GEMM on the
-// tcgen05 kernel of gemm_tcgen05.cu: a 3x3 convolution reads an im2col operand A[(b,y,x), (ky,kx,c)] (bf16) that ONE
+// wgmma kernel of gemm_wgmma.cu: a 3x3 convolution reads an im2col operand A[(b,y,x), (ky,kx,c)] (bf16) that ONE
 // kernel builds with the GroupNorm affine, the swish and the nearest-2x upsample of the source fused in (the normalised
 // tensor is never materialised), weights are pre-flattened to [C_out, (ky,kx,c)]; bias and the residual add ride in the
 // GEMM epilogue.  The kernels here are the HBM-bound glue: statistics, im2col, row softmax, layout conversion.
@@ -189,7 +189,7 @@ int mdt_vae_im2col(const float* src, const double* sums, const float* gamma, con
   const int tx = C / 4, ty = tx >= 256 ? 1 : 256 / tx;
   const long long npix = static_cast<long long>(B) * H * W;
   long long blocks = (npix + ty - 1) / ty;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > kNumSMsDefault * 16) blocks = kNumSMsDefault * 16;
   vae_im2col_kernel<<<static_cast<int>(blocks), dim3(tx, ty), 0, VS(stream)>>>(
       src, sums, gamma, beta, silu, ks, up, static_cast<__nv_bfloat16*>(A_bf16), B, H, W, C, Kp, 1e-6f);
   return vae_status();

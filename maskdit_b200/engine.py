@@ -1,4 +1,4 @@
-"""Forward / backward orchestration of the MaskDiT network over the sm_100a kernels.
+"""Forward / backward orchestration of the MaskDiT network over the sm_90a kernels.
 
 This is the arithmetic of `DiT.forward` + `forward_encoder` (models/maskdit.py:467-557) and of its autograd
 backward, expressed as a fixed sequence of C-ABI kernel launches on the current CUDA stream:
@@ -10,7 +10,7 @@ backward, expressed as a fixed sequence of C-ABI kernel launches on the current 
       gate-bwd -> dgrad GEMM (GELU' fused) / wgrad GEMM (stream-K) -> LN-modulate-bwd -> attention-bwd ...
 
 Residual stream, LayerNorm statistics, softmax, modulation vectors, loss and all gradients w.r.t. parameters are
-fp32; GEMM operands are bf16 with fp32 accumulation in TMEM.  Nothing here falls back to PyTorch math.
+fp32; GEMM operands are bf16 with fp32 accumulation in registers.  Nothing here falls back to PyTorch math.
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""Flat parameter storage for the B200 engine.
+"""Flat parameter storage for the H100 engine.
 
 All parameters of an `EDMPrecond` live in ONE contiguous fp32 device buffer (trainable first, frozen pos-embeds
 last); the module's `nn.Parameter`s are views into it, so `state_dict()/load_state_dict()/deepcopy/.parameters()`

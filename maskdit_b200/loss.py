@@ -1,4 +1,4 @@
-"""EDM training loss (reference: train_utils/loss.py) on the B200 engine.
+"""EDM training loss (reference: train_utils/loss.py) on the H100 engine.
 
 `Losses['edm']` has the reference's constructor and call signature.  When `net` is a `maskdit_b200.EDMPrecond`
 (bare, or wrapped in anything exposing `.module` like DDP / `DataParallelB200`), the loss runs fused:

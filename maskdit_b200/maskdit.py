@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference model interface (models/maskdit.py) over the B200 engine.
+"""Host-side mirror of the reference model interface (models/maskdit.py) over the H100 engine.
 
 Exports the same registries the reference's entry points consume (SURVEY.md §8b):
     DiT_models      name -> constructor            (models/maskdit.py:709-715)
@@ -138,7 +138,7 @@ class DiT(nn.Module):
                 nn.init.xavier_uniform_(prm.view(prm.shape[0], -1))
 
     def forward(self, *a, **k):
-        raise RuntimeError("call the EDMPrecond wrapper: the B200 engine fuses the EDM scalings into the network "
+        raise RuntimeError("call the EDMPrecond wrapper: the H100 engine fuses the EDM scalings into the network "
                            "kernels, the bare DiT is a parameter holder")
 
 
@@ -169,7 +169,7 @@ class _NetFn(torch.autograd.Function):
 
 
 class EDMPrecond(nn.Module):
-    """EDM preconditioning wrapper (reference: models/maskdit.py:722-776) running on the sm_100a engine."""
+    """EDM preconditioning wrapper (reference: models/maskdit.py:722-776) running on the sm_90a engine."""
 
     def __init__(self, img_resolution, img_channels, num_classes=0, sigma_min=0, sigma_max=float("inf"),
                  sigma_data=0.5, model_type="DiT-B/2", **model_kwargs):
@@ -202,7 +202,7 @@ class EDMPrecond(nn.Module):
         """Flatten parameters on `device` (once / after .to()) and refresh the bf16 weight shadow when any
         parameter was modified through PyTorch (optimizer step, load_state_dict, EMA copy...)."""
         if device.type != "cuda":
-            raise ops.L.MdtError("maskdit_b200 runs on CUDA (sm_100a) only — there is no CPU fallback")
+            raise ops.L.MdtError("maskdit_b200 runs on CUDA (sm_90a) only — there is no CPU fallback")
         params = self._params()
         if self._store is None:
             self._store = FlatStore()

@@ -1,4 +1,4 @@
-"""EDM Heun sampler (reference: sample.py:30-66) driving the B200 engine.
+"""EDM Heun sampler (reference: sample.py:30-66) driving the H100 engine.
 
 Same signature and semantics as the reference `edm_sampler` (fp64 state, 2N-1 network evaluations, `randn_like`
 consumed once per step even when S_churn = 0).  With a `maskdit_b200.EDMPrecond` network each evaluation is one

@@ -1,4 +1,4 @@
-"""Data-parallel training step on the B200 engine (reference: train.py:200-230 inner step, :178 DDP, :141 optimizer,
+"""Data-parallel training step on the H100 engine (reference: train.py:200-230 inner step, :178 DDP, :141 optimizer,
 train_utils/helper.py:47-58 EMA).
 
 One process per GPU.  A step is:
@@ -111,13 +111,12 @@ class TrainStep:
           collective  'mdt' (default with an NCCL process group): our own communicator behind the C ABI (`GradComm`);
                       'torch': `torch.distributed.all_reduce` on the process group (gloo tests, A/B).
           grad_dtype  'bf16' (default, SURVEY 8e): the fp32 gradient buffer is cast to a bf16 exchange buffer, 1.46 GB cross
-                      the links (3.5 ms at 8 x B200 instead of 6.2) and the optimizer kernel reads the bf16 sums; local
+                      the links instead of 2.92 GB and the optimizer kernel reads the bf16 sums; local
                       accumulation, moments and master weights stay fp32.  2-rank vs 1-GPU gradient rel-L2 2.3e-3.
                       'fp32': the 2.92 GB buffer is reduced as is (DDP's arithmetic; rel-L2 1e-5, order noise).
           overlap     the exchange of a block's gradients starts as soon as its backward is enqueued, on a side stream,
                       through a communicator confined to `comm_ctas` CTAs while the persistent GEMM / attention grids
-                      are sized for (SMs - comm_ctas) (`mdt_set_sm_budget`).  Measured SLOWER than the default on B200
-                      (133.1 vs 130.2 ms at 2 GPUs, profiles/r02_experiments.md section 5): off by default, kept for A/B.
+                      are sized for (SMs - comm_ctas) (`mdt_set_sm_budget`).  Off by default, kept for A/B.
         Environment overrides: MDT_COLLECTIVE, MDT_GRAD_AR, MDT_OVERLAP, MDT_COMM_CTAS."""
         self.net, self.ema = net, ema
         self.lr, self.betas, self.eps, self.wd, self.ema_decay = lr, betas, eps, weight_decay, ema_decay
@@ -168,15 +167,11 @@ class TrainStep:
         self.graph = (os.environ.get("MDT_TRAIN_GRAPH", "0") == "1") if graph is None else bool(graph)
         self._graphs = {}
         # gradient all-reduce in this many chunks on a side stream, the fused AdamW/EMA pass of chunk k running while
-        # chunk k+1 is on the wire.  Measured on 4 x B200 (profiles/r02_experiments.md): 131.65 ms/step flat, 130.71 with
-        # 4 chunks (fp32); 129.16 -> 128.31 (bf16 buffer); 8 chunks 128.79.  (At 2 GPUs in round 1: neutral.)
+        # chunk k+1 is on the wire.
         self.ar_chunks = int(os.environ.get("MDT_AR_CHUNKS", "4"))
         self.side = torch.cuda.Stream(device=dev, priority=-1) if self.overlap else None
         self._done = []          # [lo, hi) ranges already handled in the current step
         self._lr_now = lr
-        # (A background optimizer pass per block on the side stream was measured too, B200, 1 GPU, 4 / 2 SMs reserved:
-        # 129.0 / 130.5 ms per step against 121.8 ms - every SM taken from the persistent GEMM grids costs a whole tile
-        # wave, profiles/README.md - and removed.)
         net._grad_ready_hook = self._on_grads_ready if (self.overlap and self.world > 1) else None
 
     # -- optimizer state for checkpoints (reference: train.py:259-270 stores optimizer.state_dict() under 'opt') ------
@@ -292,8 +287,8 @@ class TrainStep:
     def _fwd_bwd_graphed(self, images, labels, mask_ratio, mae_loss_coef, loss_call, moments=False):
         """Gradient zeroing + loss forward + engine backward (~770 launches, 70 ms of host time) replayed from a CUDA
         graph captured once per (shapes, mask_ratio, mae_loss_coef); the all-reduce and the optimizer pass stay eager
-        (their scalars change every step).  Opt-in (`TrainStep(graph=True)` / MDT_TRAIN_GRAPH=1): written at the end of
-        round 1; run on B200 in round 2 (tests/test_model_gpu_extra.py::test_train_step_cuda_graph_matches_eager)."""
+        (their scalars change every step).  Opt-in (`TrainStep(graph=True)` / MDT_TRAIN_GRAPH=1): checked by
+        tests/test_model_gpu_extra.py::test_train_step_cuda_graph_matches_eager."""
         # keyed on the kept-token count (what shapes the launches), not on the float ratio: a schedule such as cos4
         # (configs/finetune/imagenet256-latent-cos.yaml) revisits few distinct T; at most 2 graphs are kept.
         L = self.net.model.num_patches

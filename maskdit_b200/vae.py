@@ -1,9 +1,9 @@
-"""SD-VAE decode on the B200 kernels — the sampler tail of the reference (sample.py:275 `images = vae.decode(z)`,
+"""SD-VAE decode on the H100 kernels — the sampler tail of the reference (sample.py:275 `images = vae.decode(z)`,
 autoencoder.py:306-453), so that `generate.py` ends in images as `generate_with_net` does.
 
 `AutoencoderKLDecoder` holds `post_quant_conv.*` and `decoder.*` under the reference's state-dict keys (an
 `autoencoder_kl.pth` written for `FrozenAutoencoderKL` loads with `strict=False`: the encoder half is ignored) and
-`decode(z)` returns the `[B, 3, 8h, 8w]` image the reference's `decode` returns.  Every convolution is the tcgen05 GEMM on
+`decode(z)` returns the `[B, 3, 8h, 8w]` image the reference's `decode` returns.  Every convolution is the wgmma GEMM on
 an im2col operand with GroupNorm + swish + nearest upsample fused into its construction (csrc/vae.cu); activations are
 pixel-major fp32 row matrices.  No PyTorch arithmetic on the path (torch only lays out the weights once).
 """
@@ -101,7 +101,7 @@ class AutoencoderKLDecoder(nn.Module):
         for k in self._keys:
             w = self._p(k)
             if not w.is_cuda:
-                raise ops.L.MdtError("maskdit_b200 runs on CUDA (sm_100a) only — there is no CPU fallback")
+                raise ops.L.MdtError("maskdit_b200 runs on CUDA (sm_90a) only — there is no CPU fallback")
             if k.endswith(".weight") and w.ndim == 4 and not k.startswith("post_quant_conv"):
                 co, ci, kh, kw = w.shape
                 K = kh * kw * ci

@@ -247,36 +247,36 @@ def test_c_driver_layout_equals_flat_store(mt, R, ncls):
 
 def test_gemm_dispatch_plan_for_the_xl2_step():
     """`mdt_gemm_plan` (no device needed): the host-side decisions of the GEMM launches of one XL/2 training step at
-    B = 256 (M_e = 32768 kept-token rows, M_d = 65536 decoder rows, SURVEY 8) - tile width, SM pairs, grid, the paired
-    half-tile order for N = 1152 / 3456 and the k-slice counts of the wgrad GEMMs (profiles/r02_experiments.md 11, 13)."""
+    B = 256 (M_e = 32768 kept-token rows, M_d = 65536 decoder rows, SURVEY 8) on an H100 (132 SMs) - tile width, grid,
+    the paired half-tile order for N = 1152 / 3456 and the k-slice counts of the wgrad GEMMs."""
     from maskdit_b200 import _lib
     P = _lib.gemm_plan
     Me, Md, D, H4, Dd, H4d = 32768, 65536, 1152, 4608, 512, 2048
-    # forward / dgrad: 256-wide tiles on SM pairs, one persistent CTA per SM
+    # forward / dgrad: 128 x 256 tiles, one persistent CTA per SM
     for (M, N, K, kw) in ((Me, 3 * D, D, {}), (Me, D, D, {"epi": _lib.EPI_GATE_RESID}), (Me, H4, D, {"epi": _lib.EPI_GELU}),
                           (Me, D, H4, {"epi": _lib.EPI_GATE_RESID}), (Me, D, H4, {"b_mn": True}),
                           (Me, H4, D, {"b_mn": True, "epi": _lib.EPI_DGELU}), (Md, 3 * Dd, Dd, {}), (Md, Dd, H4d, {})):
         p = P(M, N, K, **kw)
-        assert (p["block_n"], p["cg"], p["splits"], p["grid"]) == (256, 2, 1, 148), (M, N, K, p)
+        assert (p["block_n"], p["cg"], p["splits"], p["grid"]) == (256, 1, 1, 132), (M, N, K, p)
         narrow = N % 256 != 0 and N % 256 <= 128
         assert p["narrow_last"] == int(narrow) and p["pair_halves"] == int(narrow)
-        mt, nt = M // 256, -(-N // 256)
+        mt, nt = M // 128, -(-N // 256)
         units = mt * nt if not narrow else (mt // 2) * (2 * (nt - 1) + 1)
         assert (p["num_m_tiles"], p["num_n_tiles"], p["num_kb"], p["units"]) == (mt, nt, K // 64, units)
     # wgrad (accumulating epilogue): LPT inside the k-slices, slice count from the wave-time model
-    for (M, N, want) in ((D, H4, 4), (H4, D, 4), (3 * D, D, 1), (D, D, 11)):
+    for (M, N, want) in ((D, H4, 4), (H4, D, 5), (3 * D, D, 9), (D, D, 11)):
         p = P(M, N, Me, a_mn=True, b_mn=True, epi=_lib.EPI_ATOMIC)
-        assert (p["block_n"], p["cg"], p["pair_halves"], p["splits"]) == (256, 2, 0, want), (M, N, p)
-        assert p["units"] == p["num_m_tiles"] * p["num_n_tiles"] * want and p["grid"] == min(148, 2 * p["units"])
-    for (M, N, want) in ((Dd, H4d, 9), (H4d, Dd, 9), (3 * Dd, Dd, 6)):
+        assert (p["block_n"], p["cg"], p["pair_halves"], p["splits"]) == (256, 1, 0, want), (M, N, p)
+        assert p["units"] == p["num_m_tiles"] * p["num_n_tiles"] * want and p["grid"] == min(132, p["units"])
+    for (M, N, want) in ((Dd, H4d, 4), (H4d, Dd, 4), (3 * Dd, Dd, 11)):
         assert P(M, N, Md, a_mn=True, b_mn=True, epi=_lib.EPI_ATOMIC)["splits"] == want, (M, N)
-    # skinny problems: single CTAs, narrow tiles, never more CTAs than units
+    # skinny problems: narrow tiles, never more CTAs than units
     p = P(2, 1152, 256)
     assert (p["cg"], p["block_n"], p["grid"]) == (1, 256, 5)
     p = P(1024, 16, 512)
-    assert (p["cg"], p["block_n"], p["units"], p["grid"]) == (2, 128, 4, 8)
+    assert (p["cg"], p["block_n"], p["units"], p["grid"]) == (1, 128, 8, 8)
     p = P(256, 160, 64)
-    assert (p["cg"], p["block_n"]) == (2, 192)
+    assert (p["cg"], p["block_n"]) == (1, 192)
     # argument errors surface as a status, not a crash
     with pytest.raises(_lib.MdtError):
         P(0, 16, 16)

@@ -51,7 +51,7 @@ def test_sampler_with_churn_vs_reference_golden():
     assert z.dtype == torch.float64 and rel_l2(z, g["z"]) <= 2e-2
 
 
-# ---- round 2: reference goldens that reach the PRODUCTION kernels (2-CTA GEMM tiles, split-tile tcgen05 attention) ------
+# ---- reference goldens that reach the production kernels (256-wide wgmma GEMM tiles, flash attention) -----------------
 def _train_case(name, R, mask_ratio=0.5):
     g = load(name)
     net, cfg, _ = build("DiT-XL/2", R, 1000)
@@ -71,20 +71,20 @@ def _train_case(name, R, mask_ratio=0.5):
 
 def test_xl2_r32_loss_and_all_grads_vs_reference_golden():
     """BASELINE config 1/2 geometry (XL/2, 32x32x4, mask 0.5) at batch 2 WITH gradients: 256 encoder token rows ->
-    the 2-CTA (cta_group::2) GEMM instances incl. wgrad/dgrad, attn_sw_fwd/bwd<80> (T=128, head_dim 72) and the
-    SWIZZLE_64B decoder attention (T=256, head_dim 32) — end to end against the unmodified reference's autograd."""
+    the 256-wide GEMM instances incl. wgrad/dgrad, the encoder attention (T=128, head_dim 72) and the decoder
+    attention (T=256, head_dim 32) — end to end against the unmodified reference's autograd."""
     rec = _train_case("xl2_c1_grads", 32)
-    assert 2562 in rec.gemm_cfgs, rec.gemm_cfgs                     # BLOCK_N 256, SM pair
+    assert 2561 in rec.gemm_cfgs, rec.gemm_cfgs                     # BLOCK_N 256
     assert rec.attn_fwd == {(128, 72, 1), (256, 32, 1)}, rec.attn_fwd
     assert rec.attn_bwd == {(128, 72, 1), (256, 32, 1)}, rec.attn_bwd
 
 
 def test_xl2_r64_loss_and_all_grads_vs_reference_golden():
     """BASELINE config 4 geometry (XL/2, 64x64x4 latents: T=512 kept tokens of head_dim 72, L=1024 decoder tokens of
-    head_dim 32): the blocked split-tile attention kernels forward + backward, end to end against the reference."""
+    head_dim 32): the attention kernels forward + backward at the long sequences, end to end against the reference."""
     rec = _train_case("xl2_r64_grads", 64)
-    assert rec.attn_fwd == {(512, 72, 3), (1024, 32, 3)}, rec.attn_fwd
-    assert rec.attn_bwd == {(512, 72, 3), (1024, 32, 3)}, rec.attn_bwd
+    assert rec.attn_fwd == {(512, 72, 1), (1024, 32, 1)}, rec.attn_fwd
+    assert rec.attn_bwd == {(512, 72, 1), (1024, 32, 1)}, rec.attn_bwd
 
 
 def test_xl2_eval_cfg_forward_and_short_sampler_vs_reference_golden():
@@ -357,7 +357,7 @@ def test_c_driver_matches_python_engine(case):
                                      torch.cuda.current_stream().cuda_stream), "mdt_forward", 0)
 
 
-# ---- round 2: the sampler tail — SD-VAE decode on the tcgen05 GEMM + fused im2col (sample.py:275,287) ----------------
+# ---- the sampler tail — SD-VAE decode on the wgmma GEMM + fused im2col (sample.py:275,287) ----------------
 def test_vae_decode_vs_reference_golden():
     """`AutoencoderKLDecoder.decode` vs the unmodified reference Decoder + post_quant_conv (autoencoder.py:306-453) on the
     stand-in weights: 8x8 latents -> 64x64 images (every layer type: conv_in, ResnetBlocks with and without nin_shortcut,
@@ -404,22 +404,22 @@ def test_unconditional_odd_token_count_vs_reference_golden():
     assert torch.allclose(loss.cpu(), g["loss"], rtol=LOSS_TOL), (loss, g["loss"])
     check_grads(net, g, what="unconditional, T=179")
     assert (179, 64, 0) in rec.attn_fwd and (179, 64, 0) in rec.attn_bwd, (rec.attn_fwd, rec.attn_bwd)
-    assert (256, 32, 1) in rec.attn_fwd            # the decoder still runs all 256 tokens on the tcgen05 kernels
+    assert (256, 32, 1) in rec.attn_fwd            # the decoder still runs all 256 tokens on the wgmma kernels
 
 
 def test_full_size_config4_properties():
-    """BASELINE config 4 at FULL per-GPU size (XL/2, 64x64x4 latents, mask 0.5, batch 128: 512 kept / 1024 decoder tokens
-    per sample, the blocked attention kernels, a 108 GB workspace) through size-independent properties: the forward is
-    row-independent bit for bit (first rows of the batch-128 loss == a batch-2 run on the same rows), the mask path
+    """BASELINE config 4 at the largest per-GPU batch an 80 GB H100 holds (XL/2, 64x64x4 latents, mask 0.5, batch 64:
+    512 kept / 1024 decoder tokens per sample, a 54 GB workspace) through size-independent properties: the forward is
+    row-independent bit for bit (first rows of the batch-64 loss == a batch-2 run on the same rows), the mask path
     invariants hold for every row, one backward leaves finite gradients everywhere."""
     from maskdit_b200.loss import EDMLoss
     import gc
     gc.collect()
-    torch.cuda.empty_cache()          # the 108 GB workspace needs the blocks earlier tests left in the caching allocator
+    torch.cuda.empty_cache()          # the 54 GB workspace needs the blocks earlier tests left in the caching allocator
     torch.manual_seed(0)
     net, cfg, _ = build("DiT-XL/2", 64, 1000)
     net.train()
-    B, L = 128, 1024
+    B, L = 64, 1024
     g = torch.Generator().manual_seed(6)
     images = (torch.randn(B, 4, 64, 64, generator=g) * 0.5).cuda()
     labels = torch.nn.functional.one_hot(torch.randint(0, 1000, (B,), generator=g), 1000).float().cuda()

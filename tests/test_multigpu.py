@@ -1,4 +1,4 @@
-"""GPU, >= 2 devices (run with `gpurun --gpus 2`): data-parallel equivalence of the training step's gradient exchange."""
+"""GPU, >= 2 devices (skipped on a machine with fewer): data-parallel equivalence of the training step's gradient exchange."""
 import os
 import subprocess
 import sys

@@ -1,9 +1,11 @@
 """Host-side test of the persistent GEMM's work-unit order: the header the kernel includes
 (`maskdit_b200/csrc/unit_sched.h`) is compiled with g++ and walked for every CTA group.
 
-Checks: every (k-slice, m, n) tile is produced exactly once and identically by both CTAs of a pair; for the
-N = 1152 GEMMs of the XL/2 encoder (4.5 column tiles of 256) the paired order has the same makespan as LPT
-(8 tile-times on 74 SM pairs) while an m-panel's column tiles stay within adjacent waves (L2 locality of the A panel).
+Checks: every (k-slice, m, n) tile is produced exactly once, and identically by every CTA of a group when a tile is
+shared (cg = 2, kept as a property of the scheduler; the shipped kernel runs cg = 1); for the N = 1152 GEMMs of the
+XL/2 encoder (4.5 column tiles of 256) the paired order has the same makespan as LPT while an m-panel's column tiles
+stay within adjacent waves (L2 locality of the A panel), both in the shipped H100 geometry (256 row tiles of 128 on
+132 CTAs) and in a 2-CTA one (128 row tiles of 256 on 74 CTA pairs).
 """
 import os
 import shutil
@@ -32,8 +34,17 @@ def checker(tmp_path_factory):
     return run
 
 
+def test_encoder_n1152_orders_h100(checker):
+    # the shipped launch: M = 32768 (256 row tiles of 128), N = 1152 (4 full + 1 half column tile), K = 4608, 132 CTAs
+    lpt = checker(256, 5, 72, 1, 1, 0, 132, 1)
+    paired = checker(256, 5, 72, 1, 1, 1, 132, 1)
+    assert lpt["makespan"] == paired["makespan"]                 # 1152 units of work on 132 CTAs
+    assert paired["makespan"] <= 2 * (256 * 4.5 / 132 + 1) + 1e-9  # within one full tile of the ideal share
+    assert lpt["gap"] >= 7 and paired["gap"] <= 1               # LPT revisits every A panel at the very end
+
+
 def test_encoder_n1152_orders(checker):
-    # M = 32768 (128 row tiles of 256), N = 1152 (4 full + 1 half column tile), K = 4608, 74 SM pairs
+    # M = 32768 (128 row tiles of 256), N = 1152 (4 full + 1 half column tile), K = 4608, 74 CTA pairs
     lpt = checker(128, 5, 72, 1, 1, 0, 148, 2)
     paired = checker(128, 5, 72, 1, 1, 1, 148, 2)
     assert lpt["makespan"] == paired["makespan"] == 16.0        # 8 full tile-times (7.78 of work)
@@ -43,7 +54,7 @@ def test_encoder_n1152_orders(checker):
 
 
 @pytest.mark.parametrize("mt,nt", [(1, 5), (2, 5), (3, 2), (7, 3), (129, 5), (64, 2), (255, 9)])
-@pytest.mark.parametrize("grid,cg", [(148, 2), (148, 1), (4, 2), (6, 1)])
+@pytest.mark.parametrize("grid,cg", [(148, 2), (148, 1), (4, 2), (6, 1), (132, 1)])
 def test_paired_order_covers_every_tile(checker, mt, nt, grid, cg):
     r = checker(mt, nt, 18, 1, 1, 1, grid, cg)
     groups = grid // cg

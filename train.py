@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Training entry point with the reference's CLI / YAML surface (train.py:294-333, configs/train/*.yaml), driving
-the B200 engine.  Launch one process per GPU:
+the H100 engine.  Launch one process per GPU:
 
     torchrun --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 train.py --config <yaml> [--synthetic]
 
