@@ -305,10 +305,12 @@ int mdt_nccl_comm_destroy(void* comm);
 int mdt_allreduce_grads(void* comm, void* grad, long long n, int bf16, void* stream);
 
 /* ============================================================================================================
- * Sampler tail: SD-VAE decode (sample.py:275 `vae.decode(z)`; autoencoder.py:306-453).  Activations are pixel-major
+ * SD-VAE: decode, the sampler tail (sample.py:275 `vae.decode(z)`; autoencoder.py:306-453), and encode, the latent
+ * extraction (extract_latent.py:66; autoencoder.py:212-303,431-442).  Activations are pixel-major
  * fp32 row matrices [B*H*W, C]; every convolution is mdt_gemm_bf16 on an im2col operand built by mdt_vae_im2col with
  * the GroupNorm(32) affine, the swish and the nearest-2x upsample of its source fused in.  The host sequencing is
- * maskdit_b200/vae.py (same state-dict keys as FrozenAutoencoderKL: `decoder.*`, `post_quant_conv.*`).
+ * maskdit_b200/vae.py (same state-dict keys as FrozenAutoencoderKL: `decoder.*`, `post_quant_conv.*`, `encoder.*`,
+ * `quant_conv.*`).
  * ============================================================================================================ */
 /* out [B*P, C] f32 = post_quant_conv(z / scale_factor), z [B,C,h,w] NCHW (autoencoder.py:449-451); C <= 8           */
 int mdt_vae_post_quant(const float* z, const float* W, const float* bias, float scale_factor, float* out, int B,
@@ -321,10 +323,26 @@ int mdt_vae_gn_stats(const float* x, double* sums, float* scratch, int B, int P,
  * norm_out inputs (autoencoder.py:49-53,117-137,404-406); columns >= ks*ks*C are zero.                              */
 int mdt_vae_im2col(const float* src, const double* sums, const float* gamma, const float* beta, int silu, int ks,
                    int up, void* A_bf16, int B, int H, int W, int C, int Kp, void* stream);
+/* The same with a stride and an explicit low-side padding: A[(b,y,x),(ky,kx,c)] = f(src[b, s*y+ky-pad, s*x+kx-pad, c]),
+ * 0 outside the s*H x s*W source; stride = 1 | 2 (up must be 1 when stride = 2), 0 <= pad < ks.  Downsample
+ * (autoencoder.py:56-75: pad (0,1,0,1) + 3x3 stride-2 conv) is ks = 3, stride = 2, pad = 0.  mdt_vae_im2col is
+ * stride = 1, pad = ks / 2.                                                                                       */
+int mdt_vae_im2col_strided(const float* src, const double* sums, const float* gamma, const float* beta, int silu,
+                           int ks, int up, int stride, int pad, void* A_bf16, int B, int H, int W, int C, int Kp,
+                           void* stream);
 /* P [rows, cols] bf16 = softmax(scale * S) along columns (AttnBlock, autoencoder.py:185-187)                        */
 int mdt_vae_softmax_rows(const float* S, float scale, void* P_bf16, int rows, int cols, void* stream);
 /* x [B,P,ldx] f32 (first C columns) -> out [B,C,P] f32: the NCHW image `decode` returns                             */
 int mdt_vae_rows_to_nchw(const float* x, float* out, int B, int P, int C, int ldx, void* stream);
+/* Encode half (FrozenAutoencoderKL.encode_moments / encode, autoencoder.py:212-303,431-446):
+ * img [B,3,H,W] f32 NCHW -> rows [B*H*W, 4] f32 (channel 3 zero; flip != 0: horizontally mirrored, the --xflip pass
+ * of extract_latent.py:87), the conv_in operand.                                                                  */
+int mdt_vae_image_to_rows(const float* img, float* rows, int B, int H, int W, int flip, void* stream);
+/* moments [B,C,P] f32 NCHW = quant_conv(x), x [B*P, ldx] f32 (conv_out rows, first C valid), W [C,C], C <= 8 even;
+ * eps [B,C/2,P] or NULL: z [B,C/2,P] = scale_factor * (mean + exp(0.5 * clamp(logvar,-30,20)) * eps) (sample,
+ * autoencoder.py:436-442).                                                                                         */
+int mdt_vae_quant_moments(const float* x, int ldx, const float* W, const float* bias, const float* eps,
+                          float scale_factor, float* moments, float* z, int B, int C, int P, void* stream);
 
 #ifdef __cplusplus
 }

@@ -1,6 +1,8 @@
 // Sampler tail: the SD-VAE DECODE path the reference runs on every batch of sampled latents (sample.py:275
 // `images = vae.decode(z)`; autoencoder.py:306-453: post_quant_conv, conv_in, ResnetBlocks with GroupNorm(32)+swish,
-// one single-head AttnBlock, nearest-2x Upsample + conv, norm_out + conv_out).
+// one single-head AttnBlock, nearest-2x Upsample + conv, norm_out + conv_out), and the ENCODE path that turns a dataset
+// into training latents (extract_latent.py:66 `model(img, fn='encode_moments')`; autoencoder.py:212-303: conv_in,
+// ResnetBlocks, stride-2 Downsample convolutions, the AttnBlock, norm_out + conv_out, then quant_conv).
 //
 // Layout: activations are pixel-major ("NHWC") fp32 row matrices [B*H*W, C], so every convolution is a GEMM on the
 // wgmma kernel of gemm_wgmma.cu: a 3x3 convolution reads an im2col operand A[(b,y,x), (ky,kx,c)] (bf16) that ONE
@@ -73,19 +75,23 @@ __global__ void vae_gn_finish_kernel(const float* __restrict__ partial, double* 
   sums[static_cast<long long>(b) * 64 + t] = acc;
 }
 
-// im2col with the producer fused in:  A[(b, y, x), (ky, kx, c)] = f(src[b, (y+ky-pad)/up, (x+kx-pad)/up, c])  (0 outside)
+// im2col with the producer fused in:
+//   A[(b, y, x), (ky, kx, c)] = f(src[b, (s*y+ky-pad)/up, (s*x+kx-pad)/up, c])  (0 outside the s*H x s*W input)
 //   f = identity | GroupNorm affine (sums / gamma / beta given) | GroupNorm affine then swish (silu != 0)
-//   ks = 3 (pad 1) or 1 (pad 0);  up = 1 or 2 (nearest upsample of the source, Upsample.forward autoencoder.py:49-53)
-//   src [B, H/up, W/up, C] f32  ->  A [B*H*W, Kp] bf16,  Kp >= ks*ks*C (extra columns zero)
+//   ks = 3 or 1; pad = low-side zero padding (ks/2 for the "same" convolutions; 0 for Downsample, whose padding
+//   (0,1,0,1) only adds a high-side border, autoencoder.py:56-75); up = 1 or 2 (nearest upsample of the source,
+//   Upsample.forward autoencoder.py:49-53); stride s = 1 or 2 (not together with up = 2)
+//   src [B, s*H/up, s*W/up, C] f32  ->  A [B*H*W, Kp] bf16,  Kp >= ks*ks*C (extra columns zero)
 // Thread = 4 channels; blockDim = (C/4, 256/(C/4)) (C = 4: 1 x 256); each y-lane walks output pixels.
 __global__ void __launch_bounds__(256)
 vae_im2col_kernel(const float* __restrict__ src, const double* __restrict__ sums, const float* __restrict__ gamma,
-                  const float* __restrict__ beta, int silu_on, int ks, int up, __nv_bfloat16* __restrict__ A, int B,
-                  int H, int W, int C, int Kp, float eps) {
+                  const float* __restrict__ beta, int silu_on, int ks, int up, int stride, int pad,
+                  __nv_bfloat16* __restrict__ A, int B, int H, int W, int C, int Kp, float eps) {
   const int tx = threadIdx.x, c = 4 * tx;
-  const int Hs = H / up, Ws = W / up;
+  const int Hi = stride * H, Wi = stride * W;  // input extent (after the upsample)
+  const int Hs = Hi / up, Ws = Wi / up;
   const long long npix = static_cast<long long>(B) * H * W;
-  const int pad = ks / 2, taps = ks * ks;
+  const int taps = ks * ks;
   float4 ga = make_float4(1.f, 1.f, 1.f, 1.f), be = make_float4(0.f, 0.f, 0.f, 0.f);
   if (sums) {
     ga = *reinterpret_cast<const float4*>(gamma + c);
@@ -109,9 +115,9 @@ vae_im2col_kernel(const float* __restrict__ src, const double* __restrict__ sums
     __nv_bfloat16* arow = A + pix * Kp;
     for (int t = 0; t < taps; ++t) {
       const int ky = t / ks, kx = t - ky * ks;
-      const int sy = y + ky - pad, sx = x + kx - pad;
+      const int sy = stride * y + ky - pad, sx = stride * x + kx - pad;
       uint2 o = make_uint2(0u, 0u);
-      if (sy >= 0 && sy < H && sx >= 0 && sx < W) {
+      if (sy >= 0 && sy < Hi && sx >= 0 && sx < Wi) {
         const float4 v = *reinterpret_cast<const float4*>(
             src + ((static_cast<long long>(b) * Hs + sy / up) * Ws + sx / up) * C + c);
         float4 r = v;
@@ -154,6 +160,46 @@ __global__ void vae_rows_to_nchw_kernel(const float* __restrict__ x, float* __re
   out[i] = x[(static_cast<long long>(b) * P + p) * ldx + c];
 }
 
+// ---- encode half (FrozenAutoencoderKL.encode_moments / encode, autoencoder.py:212-303,431-446) ----------------------
+// img [B,3,H,W] f32 (NCHW, [-1, 1]) -> rows [B*H*W, 4] f32, channel 3 zero (conv_in then runs the C = 4 im2col);
+// flip != 0 reads column W-1-x (the `img.flip(dims=[-1])` pass of extract_latent.py:87)
+__global__ void vae_image_to_rows_kernel(const float* __restrict__ img, float* __restrict__ rows, int B, int H, int W,
+                                         int flip) {
+  const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;  // (b, y, x)
+  const long long P = static_cast<long long>(H) * W;
+  if (i >= B * P) return;
+  const int b = static_cast<int>(i / P), yx = static_cast<int>(i % P);
+  const int y = yx / W, x = yx - y * W;
+  const long long s = (static_cast<long long>(b) * 3 * H + y) * W + (flip ? W - 1 - x : x);
+  *reinterpret_cast<float4*>(rows + 4 * i) = make_float4(img[s], img[s + P], img[s + 2 * P], 0.f);
+}
+
+// x [B*P, ldx] f32 (conv_out rows, first C valid) -> moments [B,C,P] f32 = quant_conv(x) (1x1, C -> C, C <= 8);
+// z (if eps given) [B,C/2,P] = sf * (mean + exp(0.5 * clamp(logvar, -30, 20)) * eps): FrozenAutoencoderKL.sample,
+// rounded step by step as the reference's separate tensor ops are (autoencoder.py:436-442)
+__global__ void vae_quant_moments_kernel(const float* __restrict__ x, int ldx, const float* __restrict__ W,
+                                         const float* __restrict__ bias, const float* __restrict__ eps, float sf,
+                                         float* __restrict__ moments, float* __restrict__ z, int B, int C, int P) {
+  const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;  // (b, pixel)
+  if (i >= static_cast<long long>(B) * P) return;
+  const int b = static_cast<int>(i / P), p = static_cast<int>(i % P);
+  float v[8], m[8];
+  for (int c = 0; c < C; ++c) v[c] = x[i * ldx + c];
+  for (int o = 0; o < C; ++o) {
+    float acc = bias[o];
+    for (int c = 0; c < C; ++c) acc = fmaf(W[o * C + c], v[c], acc);
+    m[o] = acc;
+    moments[(static_cast<long long>(b) * C + o) * P + p] = acc;
+  }
+  if (!eps) return;
+  const int h = C / 2;
+  for (int o = 0; o < h; ++o) {
+    const long long zi = (static_cast<long long>(b) * h + o) * P + p;
+    const float std_ = expf(__fmul_rn(0.5f, fminf(fmaxf(m[h + o], -30.f), 20.f)));
+    z[zi] = __fmul_rn(sf, __fadd_rn(m[o], __fmul_rn(std_, eps[zi])));
+  }
+}
+
 }  // namespace mdt
 
 using namespace mdt;
@@ -181,8 +227,15 @@ int mdt_vae_gn_stats(const float* x, double* sums, float* scratch, int B, int P,
 
 int mdt_vae_im2col(const float* src, const double* sums, const float* gamma, const float* beta, int silu, int ks,
                    int up, void* A_bf16, int B, int H, int W, int C, int Kp, void* stream) {
+  return mdt_vae_im2col_strided(src, sums, gamma, beta, silu, ks, up, 1, ks / 2, A_bf16, B, H, W, C, Kp, stream);
+}
+
+int mdt_vae_im2col_strided(const float* src, const double* sums, const float* gamma, const float* beta, int silu,
+                           int ks, int up, int stride, int pad, void* A_bf16, int B, int H, int W, int C, int Kp,
+                           void* stream) {
   if (!src || !A_bf16 || B <= 0 || H <= 0 || W <= 0 || C % 4 || C > 1024 || (ks != 1 && ks != 3) ||
-      (up != 1 && up != 2) || H % up || W % up || Kp < ks * ks * C || Kp % 8)
+      (up != 1 && up != 2) || (stride != 1 && stride != 2) || (up == 2 && stride == 2) || pad < 0 || pad >= ks ||
+      H % up || W % up || Kp < ks * ks * C || Kp % 8)
     return MDT_ERR_ARG;
   if (sums && (!gamma || !beta || C % 128)) return MDT_ERR_ARG;
   if ((reinterpret_cast<uintptr_t>(src) | reinterpret_cast<uintptr_t>(A_bf16)) & 15) return MDT_ERR_ARG;
@@ -191,7 +244,7 @@ int mdt_vae_im2col(const float* src, const double* sums, const float* gamma, con
   long long blocks = (npix + ty - 1) / ty;
   if (blocks > kNumSMsDefault * 16) blocks = kNumSMsDefault * 16;
   vae_im2col_kernel<<<static_cast<int>(blocks), dim3(tx, ty), 0, VS(stream)>>>(
-      src, sums, gamma, beta, silu, ks, up, static_cast<__nv_bfloat16*>(A_bf16), B, H, W, C, Kp, 1e-6f);
+      src, sums, gamma, beta, silu, ks, up, stride, pad, static_cast<__nv_bfloat16*>(A_bf16), B, H, W, C, Kp, 1e-6f);
   return vae_status();
 }
 
@@ -206,6 +259,23 @@ int mdt_vae_rows_to_nchw(const float* x, float* out, int B, int P, int C, int ld
   if (!x || !out || B <= 0 || P <= 0 || C <= 0 || ldx < C) return MDT_ERR_ARG;
   const long long n = static_cast<long long>(B) * C * P;
   vae_rows_to_nchw_kernel<<<static_cast<int>((n + 255) / 256), 256, 0, VS(stream)>>>(x, out, B, P, C, ldx);
+  return vae_status();
+}
+
+int mdt_vae_image_to_rows(const float* img, float* rows, int B, int H, int W, int flip, void* stream) {
+  if (!img || !rows || B <= 0 || H <= 0 || W <= 0 || (reinterpret_cast<uintptr_t>(rows) & 15)) return MDT_ERR_ARG;
+  const long long n = static_cast<long long>(B) * H * W;
+  vae_image_to_rows_kernel<<<static_cast<int>((n + 255) / 256), 256, 0, VS(stream)>>>(img, rows, B, H, W, flip != 0);
+  return vae_status();
+}
+
+int mdt_vae_quant_moments(const float* x, int ldx, const float* W, const float* bias, const float* eps,
+                          float scale_factor, float* moments, float* z, int B, int C, int P, void* stream) {
+  if (!x || !W || !bias || !moments || B <= 0 || C <= 0 || C > 8 || C % 2 || ldx < C || P <= 0) return MDT_ERR_ARG;
+  if (eps && !z) return MDT_ERR_ARG;
+  const long long n = static_cast<long long>(B) * P;
+  vae_quant_moments_kernel<<<static_cast<int>((n + 255) / 256), 256, 0, VS(stream)>>>(x, ldx, W, bias, eps,
+                                                                                     scale_factor, moments, z, B, C, P);
   return vae_status();
 }
 

@@ -9,7 +9,7 @@ into the float one-hot the label embedder consumes.
 The `lmdb` Python module is not part of this image, so `MdbReader` below is a read-only walker of LMDB's on-disk
 B+tree (`data.mdb`: two meta pages, branch / leaf / overflow pages) written from the published file format; when
 `lmdb` IS importable it is used instead.  PARITY UNPINNED against liblmdb itself (no liblmdb here to produce a
-fixture): `tests/test_data.py` round-trips files produced by `write_mdb` (the same format, bulk-loaded).
+fixture): `tests/test_data.py` round-trips files produced by `MdbWriter` / `write_mdb` (the same format, bulk-loaded).
 
 Nothing here runs on the GPU: batches are assembled in pinned host memory and copied by the caller; the arithmetic
 that follows (moments -> latent, label dropout, noise injection) is `ops.step_front` (csrc/loss_optim.cu).
@@ -106,21 +106,62 @@ class MdbReader:
             return None
 
 
-def write_mdb(path, items, psize=4096):
-    """Bulk-load `items` (dict bytes -> bytes) into a fresh single-database LMDB file `<path>/data.mdb` (tests and
-    synthetic datasets; the reference writes these with liblmdb, extract_latent.py:60-106)."""
-    os.makedirs(path, exist_ok=True)
-    keys = sorted(items)
-    pages = {}          # pgno -> bytes
-    next_pg = [2]
-    n_leaf = n_branch = n_over = 0
+class MdbWriter:
+    """Stream a fresh single-database LMDB file `<path>/data.mdb` (main database, byte-wise key order, 64-bit layout).
 
-    def alloc(n=1):
-        p = next_pg[0]
-        next_pg[0] += n
+    `put(key, value)` appends a value too large for a leaf node (every latent) to the file at once as overflow pages,
+    so memory holds only the keys, their (overflow page, size) pairs and the small inline values; `close()` sorts the
+    keys and writes the leaf and branch pages after the overflow pages, then the two meta pages (pages 0 and 1, reserved
+    at open).  This is how extract_latent.py writes hundreds of GB of moments; the reference uses liblmdb
+    (extract_latent.py:60-106)."""
+
+    def __init__(self, path, psize=4096):
+        os.makedirs(path, exist_ok=True)
+        self.psize = psize
+        self._f = open(os.path.join(path, "data.mdb"), "wb")
+        self._f.write(bytes(2 * psize))                      # pages 0 and 1: the meta pages, written by close()
+        self._next = 2
+        self._small, self._big = {}, {}                      # key -> value bytes | key -> (first overflow page, size)
+        self._n_over = 0
+        self._nodemax = psize // 2 - PAGEHDR
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, exc_type, *exc):
+        if self._f is None:
+            return
+        if exc_type is None:
+            self.close()
+        else:                                                # leave an unfinished file rather than a valid-looking one
+            self._f.close()
+            self._f = None
+
+    def _alloc(self, n=1):
+        p = self._next
+        self._next += n
         return p
 
-    def build_page(pgno, flags, nodes):
+    def put(self, key, value):
+        key = bytes(key)
+        if key in self._small or key in self._big:
+            raise KeyError(f"duplicate key {key!r}")
+        mv = memoryview(value).cast("B")
+        n = mv.nbytes
+        if 8 + len(key) + n <= self._nodemax:
+            self._small[key] = mv.tobytes()
+            return
+        npg = (PAGEHDR + n + self.psize - 1) // self.psize     # value goes to overflow pages
+        ov = self._alloc(npg)
+        self._f.write(struct.pack("<QHHI", ov, 0, P_OVERFLOW, npg))
+        self._f.write(mv)
+        self._f.write(bytes(npg * self.psize - PAGEHDR - n))
+        self._n_over += npg
+        self._big[key] = (ov, n)
+
+    def _page(self, flags, nodes):
+        pgno = self._alloc()
+        psize = self.psize
         buf = bytearray(psize)
         upper = psize
         ptrs = []
@@ -132,79 +173,77 @@ def write_mdb(path, items, psize=4096):
         assert lower <= upper
         struct.pack_into("<QHHHH", buf, 0, pgno, 0, flags, lower, upper)
         struct.pack_into(f"<{len(ptrs)}H", buf, PAGEHDR, *ptrs)
-        pages[pgno] = bytes(buf)
+        self._f.write(buf)
+        return pgno
 
-    def fits(nodes, nd):
-        used = sum(len(x) + (len(x) & 1) for x in nodes) + len(nd) + (len(nd) & 1)
-        return PAGEHDR + 2 * (len(nodes) + 1) + used <= psize
+    def _fits(self, used, count, nd):
+        return PAGEHDR + 2 * (count + 1) + used + len(nd) + (len(nd) & 1) <= self.psize
 
-    nodemax = psize // 2 - PAGEHDR
-    level = []          # (first key, pgno)
-    cur, first = [], None
-    for k in keys:
-        v = items[k]
-        if 8 + len(k) + len(v) > nodemax:                          # value goes to overflow pages
-            npg = (PAGEHDR + len(v) + psize - 1) // psize
-            ov = alloc(npg)
-            buf = bytearray(npg * psize)
-            struct.pack_into("<QHHI", buf, 0, ov, 0, P_OVERFLOW, npg)
-            buf[PAGEHDR:PAGEHDR + len(v)] = v
-            for j in range(npg):
-                pages[ov + j] = bytes(buf[j * psize:(j + 1) * psize])
-            n_over += npg
-            nd = struct.pack("<HHHH", len(v) & 0xFFFF, len(v) >> 16, F_BIGDATA, len(k)) + k + struct.pack("<Q", ov)
-        else:
-            nd = struct.pack("<HHHH", len(v) & 0xFFFF, len(v) >> 16, 0, len(k)) + k + v
-        if cur and not fits(cur, nd):
-            pg = alloc()
-            build_page(pg, P_LEAF, cur)
-            level.append((first, pg))
-            n_leaf += 1
-            cur, first = [], None
-        if first is None:
-            first = k
-        cur.append(nd)
-    if cur:
-        pg = alloc()
-        build_page(pg, P_LEAF, cur)
-        level.append((first, pg))
-        n_leaf += 1
-    depth = 1 if level else 0
-    while len(level) > 1:
-        nxt, cur, first = [], [], None
-        for k, pg in level:
-            kk = b"" if not cur else k
-            nd = struct.pack("<HHHH", pg & 0xFFFF, (pg >> 16) & 0xFFFF, (pg >> 32) & 0xFFFF, len(kk)) + kk
-            if cur and not fits(cur, nd):
-                bp = alloc()
-                build_page(bp, P_BRANCH, cur)
-                nxt.append((first, bp))
-                n_branch += 1
-                cur, first = [], None
-                nd = struct.pack("<HHHH", pg & 0xFFFF, (pg >> 16) & 0xFFFF, (pg >> 32) & 0xFFFF, 0)
+    def close(self):
+        keys = sorted([*self._small, *self._big])
+        n_leaf = n_branch = 0
+        level = []          # (first key, pgno)
+        cur, used, first = [], 0, None
+        for k in keys:
+            if k in self._big:
+                ov, n = self._big[k]
+                nd = struct.pack("<HHHH", n & 0xFFFF, n >> 16, F_BIGDATA, len(k)) + k + struct.pack("<Q", ov)
+            else:
+                v = self._small[k]
+                nd = struct.pack("<HHHH", len(v) & 0xFFFF, len(v) >> 16, 0, len(k)) + k + v
+            if cur and not self._fits(used, len(cur), nd):
+                level.append((first, self._page(P_LEAF, cur)))
+                n_leaf += 1
+                cur, used, first = [], 0, None
             if first is None:
                 first = k
             cur.append(nd)
-        bp = alloc()
-        build_page(bp, P_BRANCH, cur)
-        nxt.append((first, bp))
-        n_branch += 1
-        level = nxt
-        depth += 1
-    root = level[0][1] if level else P_INVALID
-    last_pg = next_pg[0] - 1
-    for m in (0, 1):
-        buf = bytearray(psize)
-        struct.pack_into("<QHHI", buf, 0, m, 0, P_META, 0)
-        b = PAGEHDR
-        struct.pack_into("<IIQQ", buf, b, MDB_MAGIC, 1, 0, max(1 << 20, (last_pg + 1) * psize))
-        struct.pack_into("<IHHQQQQQ", buf, b + 24, psize, 0, 0, 0, 0, 0, 0, P_INVALID)        # free DB (empty)
-        struct.pack_into("<IHHQQQQQ", buf, b + 72, 0, 0, depth, n_branch, n_leaf, n_over, len(keys), root)
-        struct.pack_into("<QQ", buf, b + 120, last_pg, 1 if m == 1 else 0)
-        pages[m] = bytes(buf)
-    with open(os.path.join(path, "data.mdb"), "wb") as f:
-        for pg in range(next_pg[0]):
-            f.write(pages[pg])
+            used += len(nd) + (len(nd) & 1)
+        if cur:
+            level.append((first, self._page(P_LEAF, cur)))
+            n_leaf += 1
+        depth = 1 if level else 0
+        while len(level) > 1:
+            nxt, cur, used, first = [], [], 0, None
+            for k, pg in level:
+                kk = b"" if not cur else k
+                nd = struct.pack("<HHHH", pg & 0xFFFF, (pg >> 16) & 0xFFFF, (pg >> 32) & 0xFFFF, len(kk)) + kk
+                if cur and not self._fits(used, len(cur), nd):
+                    nxt.append((first, self._page(P_BRANCH, cur)))
+                    n_branch += 1
+                    cur, used, first = [], 0, None
+                    nd = struct.pack("<HHHH", pg & 0xFFFF, (pg >> 16) & 0xFFFF, (pg >> 32) & 0xFFFF, 0)
+                if first is None:
+                    first = k
+                cur.append(nd)
+                used += len(nd) + (len(nd) & 1)
+            nxt.append((first, self._page(P_BRANCH, cur)))
+            n_branch += 1
+            level = nxt
+            depth += 1
+        root = level[0][1] if level else P_INVALID
+        psize, last_pg = self.psize, self._next - 1
+        for m in (0, 1):
+            buf = bytearray(psize)
+            struct.pack_into("<QHHI", buf, 0, m, 0, P_META, 0)
+            b = PAGEHDR
+            struct.pack_into("<IIQQ", buf, b, MDB_MAGIC, 1, 0, max(1 << 20, (last_pg + 1) * psize))
+            struct.pack_into("<IHHQQQQQ", buf, b + 24, psize, 0, 0, 0, 0, 0, 0, P_INVALID)    # free DB (empty)
+            struct.pack_into("<IHHQQQQQ", buf, b + 72, 0, 0, depth, n_branch, n_leaf, self._n_over, len(keys), root)
+            struct.pack_into("<QQ", buf, b + 120, last_pg, 1 if m == 1 else 0)
+            self._f.seek(m * psize)
+            self._f.write(buf)
+        self._f.close()
+        self._f = None
+        self._small, self._big = {}, {}
+
+
+def write_mdb(path, items, psize=4096):
+    """Bulk-load `items` (dict bytes -> bytes) into a fresh single-database LMDB file `<path>/data.mdb` (tests and
+    synthetic datasets; the reference writes these with liblmdb, extract_latent.py:60-106)."""
+    with MdbWriter(path, psize) as w:
+        for k, v in items.items():
+            w.put(k, v)
 
 
 def write_latent_lmdb(root, moments, labels, split="train"):
@@ -214,6 +253,50 @@ def write_latent_lmdb(root, moments, labels, split="train"):
         items[f"z-{i}".encode()] = np.ascontiguousarray(z, dtype="<f4").tobytes()
         items[f"y-{i}".encode()] = str(int(y)).encode()
     write_mdb(os.path.join(root, split), items)
+
+
+# ---- image side of the latent extraction (extract_latent.py:16-110) --------------------------------------------------
+IMG_EXTENSIONS = (".jpg", ".jpeg", ".png", ".ppm", ".bmp", ".pgm", ".tif", ".tiff", ".webp")   # torchvision's list
+
+
+def image_folder_samples(root):
+    """(path, class index) of every image under `root` in ImageFolder order: class directories sorted by name and
+    numbered in that order, each walked recursively with sorted directories and sorted file names, files kept by
+    (case-insensitive) image extension.  This is the order `ImageFolder.imgs` gives extract_latent.py's dataset
+    (train_utils/datasets.py:73-77), so z-{i} / y-{i} are numbered as the reference numbers them."""
+    classes = sorted(e.name for e in os.scandir(root) if e.is_dir())
+    if not classes:
+        raise FileNotFoundError(f"no class directories under {root}")
+    out = []
+    for idx, c in enumerate(classes):
+        for d, _, fnames in sorted(os.walk(os.path.join(root, c), followlinks=True)):
+            for f in sorted(fnames):
+                if f.lower().endswith(IMG_EXTENSIONS):
+                    out.append((os.path.join(d, f), idx))
+    return out, classes
+
+
+def center_crop_arr(pil_image, image_size):
+    """ADM centre crop (the rule of train_utils/datasets.py:19-37): halve with a BOX filter while the short side is at
+    least twice the target, resize BICUBIC so the short side equals the target, crop the centre.  -> uint8 [R, R, C]."""
+    from PIL import Image
+    while min(*pil_image.size) >= 2 * image_size:
+        pil_image = pil_image.resize(tuple(x // 2 for x in pil_image.size), resample=Image.BOX)
+    scale = image_size / min(*pil_image.size)
+    pil_image = pil_image.resize(tuple(round(x * scale) for x in pil_image.size), resample=Image.BICUBIC)
+    arr = np.asarray(pil_image)
+    y0, x0 = (arr.shape[0] - image_size) // 2, (arr.shape[1] - image_size) // 2
+    return arr[y0:y0 + image_size, x0:x0 + image_size]
+
+
+def load_image(path, resolution):
+    """One extract_latent.py input: PIL decode, RGB, centre crop, then ToTensor + Normalize(0.5, 0.5) arithmetic
+    (x / 255 then (x - 0.5) / 0.5 in fp32) -> float32 [3, R, R] in [-1, 1]."""
+    from PIL import Image
+    with Image.open(path) as im:
+        arr = center_crop_arr(im.convert("RGB"), resolution)
+    x = np.ascontiguousarray(arr.transpose(2, 0, 1)).astype(np.float32) / np.float32(255)
+    return (x - np.float32(0.5)) / np.float32(0.5)
 
 
 class ImageNetLatentDataset:
