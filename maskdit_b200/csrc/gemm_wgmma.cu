@@ -222,6 +222,8 @@ __device__ __noinline__ void epilogue_ragged(const GemmParams& p, uint32_t stg, 
 
 // One staged 16 x 32 chunk of a warp -> global.  Kept out of line: the consumer loop around it holds the whole
 // accumulator in registers, and inlining the epilogue arithmetic there pushes the accumulator into local memory.
+// `p` is the kernel's __grid_constant__ parameter, so the reference points into parameter space: a plain by-value
+// kernel parameter would be copied to a stack frame for its address and every field read here would be a local load.
 template <int EPI>
 __device__ __noinline__ void epilogue_staged(const GemmParams& p, uint32_t stg, int row_base, int nrows, int col0,
                                              int lane) {
@@ -328,7 +330,7 @@ MDT_DEVINL void consumer_loop(const GemmParams& p, UnitSched& sched, uint8_t* sm
 template <int BLOCK_N, bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                  const GemmParams p) {
+                  const __grid_constant__ GemmParams p) {
   using Cfg = GemmCfg<BLOCK_N>;
   constexpr int kStages = Cfg::kStages;
   extern __shared__ uint8_t smem_raw[];
