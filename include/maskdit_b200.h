@@ -167,13 +167,18 @@ int mdt_attention_impl_log(int* out4, int cap);
 /* ------------------------------------------------------------------------------------------------------------
  * unmask_tokens + decoder_pos_embed (models/maskdit.py:157-163,543-545):
  *   out[b,l,:] = (ids_restore[b,l] < T ? u[b, ids_restore[b,l], :] : mask_token) + pos[l,:]
- * ids_restore NULL = eval path (no masking): out = u + pos.
+ * ids_restore NULL = eval path (no masking): out = u + pos.  mask_token NULL: zeros; pos NULL: no position term (the
+ * decoder-less DiT's zero-filled output scatter, models/maskdit.py:551-553, is mask_token = pos = NULL).
  * Backward: du_bf16[b,i,:] = g[b, ids_keep[b,i], :] ; dmask_token[:] += sum over removed positions of g.
  * ------------------------------------------------------------------------------------------------------------ */
 int mdt_unmask_tokens(const float* u, const float* mask_token, const float* pos, const int64_t* ids_restore,
                       float* out, int B, int T, int L, int D, void* stream);
 int mdt_unmask_tokens_bwd(const float* g, const int64_t* ids_keep, const int64_t* ids_restore, void* du_bf16,
                           float* dmask_token, int B, int T, int L, int D, void* stream);
+/* Row gather: out_bf16[b*T + i, :] = in_bf16[b*L + idx[b*T + i], :], idx [B,T] int64 (ids_keep), D % 4 == 0.  The
+ * decoder-less DiT's backward through the zero-filled scatter: the gradient of the kept tokens' rows only.       */
+int mdt_gather_rows_bf16(const void* in_bf16, const int64_t* idx, void* out_bf16, int B, int T, int L, int D,
+                         void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * unpatchify + EDM preconditioning + EDM/MAE loss, forward and the gradient seed in one pass.
@@ -255,12 +260,19 @@ int mdt_get_sm_budget(void);
  *   [adaLN_modulation.1.weight of blocks 0..depth-1, decoder_layer, decoder_blocks 0.., final_layer]
  *   [the matching adaLN biases] [all other trainable tensors in registration order] [pos_embed, decoder_pos_embed]
  * every tensor on a 64-element boundary; names = the reference's state-dict keys (models/maskdit.py:242-332).
+ *
+ * Decoder-less DiT (use_decoder=False, the reference's default, models/maskdit.py:254): dec_hidden = dec_depth =
+ * dec_heads = dec_mlp_hidden = 0 and has_mask_token = 0.  Any other combination with a zero dec_* field is rejected.
+ * There is no decoder_layer, no decoder block, no decoder_pos_embed and no mask token; the final layer reads the
+ * encoder width ([p*p*C, hidden], adaLN [2*hidden, hidden]) and the modulation vector is blocks 0..depth-1, final:
+ * depth*6*hidden + 2*hidden columns.  Training with a mask runs the final layer on the T kept tokens and scatters them
+ * into F with zero rows for the removed tokens (:550-553); the removed rows get no gradient.
  * ============================================================================================================ */
 typedef struct mdt_model_cfg {
   int img_resolution, img_channels, patch_size, num_classes; /* EDMPrecond / DiT ctor, models/maskdit.py:722-741     */
   int hidden, depth, heads, mlp_hidden;                      /* encoder DiTBlocks (DiT_models, :645-715)              */
-  int dec_hidden, dec_depth, dec_heads, dec_mlp_hidden;      /* decoder (:310-312: 512, 8, 16, 2048)                  */
-  int has_mask_token;                                        /* mae_loss_coef > 0 (:297-299)                          */
+  int dec_hidden, dec_depth, dec_heads, dec_mlp_hidden;      /* decoder (:310-312: 512, 8, 16, 2048); all 0: none     */
+  int has_mask_token;                                        /* decoder and mae_loss_coef > 0 (:323-324)              */
   float sigma_data;
 } mdt_model_cfg;
 typedef struct mdt_model mdt_model; /* host-side layout object: no device memory, no CUDA calls */

@@ -82,6 +82,7 @@ _SIGS = {
     "mdt_gemm_last_config": [],
     "mdt_unmask_tokens": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
     "mdt_unmask_tokens_bwd": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
+    "mdt_gather_rows_bf16": [_P, _P, _P, _I, _I, _I, _I, _P],
     "mdt_edm_loss": [_P, _P, _P, _P, _P, _P, _F, _F, _P, _P, _P, _I, _I, _I, _I, _P],
     "mdt_step_front": [_P, _P, _P, _P, _P, _F, _F, _F, _F, _P, _P, _P, _P, _I, _I, _I, _I, _P],
     "mdt_edm_precond_out": [_P, _P, _P, _F, _P, _I, _I, _I, _I, _P],

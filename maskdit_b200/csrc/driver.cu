@@ -12,7 +12,9 @@
 // Packed parameter blob (fp32 master `w32`, bf16 shadow `w16`, fp32 gradient `grad`: same element offsets):
 //   [adaLN_modulation.1.weight of blocks 0..depth-1, decoder_layer, decoder_blocks 0..dec_depth-1, final_layer]
 //   [the matching adaLN biases] [every other trainable tensor in registration order] [pos_embed, decoder_pos_embed]
-// each tensor starting on a 64-element boundary - `mdt_model_param_info` enumerates it, `maskdit_b200/flat.py`
+// each tensor starting on a 64-element boundary.  The decoder-less DiT (use_decoder=False, models/maskdit.py:254,
+// 308-331: all four dec_* fields 0) has no decoder_layer, decoder blocks, decoder_pos_embed or mask token, and its
+// final layer reads the encoder width - `mdt_model_param_info` enumerates it, `maskdit_b200/flat.py`
 // builds exactly this layout for the nn.Module (tests/test_host.py compares the two).
 #include <dlfcn.h>
 #include <string.h>
@@ -53,6 +55,8 @@ struct NamedTensor {
 struct mdt_model {
   mdt_model_cfg cfg;
   int D, Dd, L, G, pd, NA, H4e, H4d, Kp;
+  bool has_dec;  // false: decoder-less DiT, the final layer runs on the encoder's T kept tokens (width D)
+  int Df;        // final-layer input width: Dd, or D without a decoder
   std::vector<BlockP> enc, dec;
   Tensor pos, dpos, mask_token, xw, xb, t0w, t0b, t2w, t2b, ytab, dlw, dlb, flw, flb;
   std::vector<Tensor> ada_w, ada_b;  // per head, in blob order
@@ -69,6 +73,8 @@ void build_layout(mdt_model* m) {
   const mdt_model_cfg& c = m->cfg;
   const int D = c.hidden, Dd = c.dec_hidden;
   m->D = D, m->Dd = Dd;
+  m->has_dec = c.dec_hidden > 0;
+  m->Df = m->has_dec ? Dd : D;
   m->G = c.img_resolution / c.patch_size;
   m->L = m->G * m->G;
   m->pd = c.patch_size * c.patch_size * c.img_channels;
@@ -76,15 +82,15 @@ void build_layout(mdt_model* m) {
   m->Kp = static_cast<int>(round_up(c.num_classes, 8));
   m->enc.resize(c.depth);
   m->dec.resize(c.dec_depth);
-  m->ada_w.resize(c.depth + c.dec_depth + 2);
-  m->ada_b.resize(c.depth + c.dec_depth + 2);
+  m->ada_w.resize(c.depth + c.dec_depth + (m->has_dec ? 2 : 1));
+  m->ada_b.resize(c.depth + c.dec_depth + (m->has_dec ? 2 : 1));
   auto& nm = m->named;
   auto add = [&](const std::string& name, Tensor* t, i64 numel, int group, int rank = 0) {
     nm.push_back(NamedTensor{name, t, numel, group, rank});
   };
   // registration order of the reference module (models/maskdit.py:242-332)
   add("model.pos_embed", &m->pos, static_cast<i64>(m->L) * D, 3);
-  add("model.decoder_pos_embed", &m->dpos, static_cast<i64>(m->L) * Dd, 3);
+  if (m->has_dec) add("model.decoder_pos_embed", &m->dpos, static_cast<i64>(m->L) * Dd, 3);
   if (c.has_mask_token) add("model.mask_token", &m->mask_token, Dd, 2);
   add("model.x_embedder.proj.weight", &m->xw, static_cast<i64>(D) * m->pd, 2);
   add("model.x_embedder.proj.bias", &m->xb, D, 2);
@@ -111,21 +117,25 @@ void build_layout(mdt_model* m) {
     ++head;
   };
   for (int i = 0; i < c.depth; ++i) add_block("model.blocks." + std::to_string(i), m->enc[i], D, c.heads, m->H4e);
-  m->off_declayer = mod;
-  mod += 2 * D;
-  add("model.decoder_layer.linear.weight", &m->dlw, static_cast<i64>(Dd) * D, 2);
-  add("model.decoder_layer.linear.bias", &m->dlb, Dd, 2);
-  add("model.decoder_layer.adaLN_modulation.1.weight", &m->ada_w[head], 2ll * D * D, 0, head);
-  add("model.decoder_layer.adaLN_modulation.1.bias", &m->ada_b[head], 2ll * D, 1, head);
-  ++head;
-  for (int i = 0; i < c.dec_depth; ++i)
-    add_block("model.decoder_blocks." + std::to_string(i), m->dec[i], Dd, c.dec_heads, m->H4d);
+  m->off_declayer = -1;
+  if (m->has_dec) {
+    m->off_declayer = mod;
+    mod += 2 * D;
+    add("model.decoder_layer.linear.weight", &m->dlw, static_cast<i64>(Dd) * D, 2);
+    add("model.decoder_layer.linear.bias", &m->dlb, Dd, 2);
+    add("model.decoder_layer.adaLN_modulation.1.weight", &m->ada_w[head], 2ll * D * D, 0, head);
+    add("model.decoder_layer.adaLN_modulation.1.bias", &m->ada_b[head], 2ll * D, 1, head);
+    ++head;
+    for (int i = 0; i < c.dec_depth; ++i)
+      add_block("model.decoder_blocks." + std::to_string(i), m->dec[i], Dd, c.dec_heads, m->H4d);
+  }
+  const int Df = m->Df;
   m->off_final = mod;
-  mod += 2 * Dd;
-  add("model.final_layer.linear.weight", &m->flw, static_cast<i64>(m->pd) * Dd, 2);
+  mod += 2 * Df;
+  add("model.final_layer.linear.weight", &m->flw, static_cast<i64>(m->pd) * Df, 2);
   add("model.final_layer.linear.bias", &m->flb, m->pd, 2);
-  add("model.final_layer.adaLN_modulation.1.weight", &m->ada_w[head], 2ll * Dd * D, 0, head);
-  add("model.final_layer.adaLN_modulation.1.bias", &m->ada_b[head], 2ll * Dd, 1, head);
+  add("model.final_layer.adaLN_modulation.1.weight", &m->ada_w[head], 2ll * Df * D, 0, head);
+  add("model.final_layer.adaLN_modulation.1.bias", &m->ada_b[head], 2ll * Df, 1, head);
   m->NA = static_cast<int>(mod);
   // blob order: group 0 by rank, group 1 by rank, group 2 in registration order, group 3 last
   i64 off = 0;
@@ -168,6 +178,7 @@ struct Plan {
   i64 X0, tf, th_pre, th, c, c2, y16, y16p, wyp, sc, mod;
   std::vector<BlockBuf> enc, dec;
   i64 xmd, mean_d, rstd_d, u, Z, xf, mean_f, rstd_f;
+  i64 fk;  // decoder-less + masked: final-layer output of the kept tokens [B*T, pd] f32, in the backward their dF bf16
   // backward scratch
   i64 dmod, dxf, Gz, dyA, dyB, dh, dxm, dO, dqkv, du, dxmd, Ge, dmod16, dsc, dc32, dc16, dth, dpre32, dpre16, ytmp;
   i64 total;
@@ -214,29 +225,33 @@ Plan make_plan(const mdt_model* m, int B, int T, bool save, bool with_backward) 
     }
   };
   plan_blocks(m->enc, p.enc, Me, T);
-  p.xmd = a.take(Me * D * 2);
-  p.mean_d = a.take(Me * 4);
-  p.rstd_d = a.take(Me * 4);
-  p.u = a.take(Me * Dd * 4);
-  p.Z = a.take(Md * Dd * 4);
-  plan_blocks(m->dec, p.dec, Md, L);
-  p.xf = a.take(Md * Dd * 2);
-  p.mean_f = a.take(Md * 4);
-  p.rstd_f = a.take(Md * 4);
+  p.xmd = p.mean_d = p.rstd_d = p.u = p.Z = p.fk = p.Gz = p.du = p.dxmd = -1;
+  if (m->has_dec) {
+    p.xmd = a.take(Me * D * 2);
+    p.mean_d = a.take(Me * 4);
+    p.rstd_d = a.take(Me * 4);
+    p.u = a.take(Me * Dd * 4);
+    p.Z = a.take(Md * Dd * 4);
+    plan_blocks(m->dec, p.dec, Md, L);
+  }
+  const i64 Mf = m->has_dec ? Md : Me;  // final-layer rows
+  p.xf = a.take(Mf * m->Df * 2);
+  p.mean_f = a.take(Mf * 4);
+  p.rstd_f = a.take(Mf * 4);
+  if (!m->has_dec) p.fk = a.take(Me * m->pd * 4);
   if (with_backward) {
     const i64 Mmax_d = Me * D > Md * Dd ? Me * D : Md * Dd;                    // max over (enc, dec) of M * dim
     const i64 Mmax_h = Me * m->H4e > Md * m->H4d ? Me * m->H4e : Md * m->H4d;  // M * mlp hidden
     p.dmod = a.take(static_cast<i64>(B) * NA * 4);
-    p.dxf = a.take(Md * Dd * 2);
-    p.Gz = a.take(Md * Dd * 4);
+    p.dxf = a.take(Mf * m->Df * 2);
+    if (m->has_dec) p.Gz = a.take(Md * Dd * 4);
     p.dyA = a.take(Mmax_d * 2);
     p.dyB = a.take(Mmax_d * 2);
     p.dh = a.take(Mmax_h * 2);
     p.dxm = a.take(Mmax_d * 2);
     p.dO = a.take(Mmax_d * 2);
     p.dqkv = a.take(Mmax_d * 3 * 2);
-    p.du = a.take(Me * Dd * 2);
-    p.dxmd = a.take(Me * D * 2);
+    if (m->has_dec) p.du = a.take(Me * Dd * 2), p.dxmd = a.take(Me * D * 2);
     p.Ge = a.take(Me * D * 4);
     p.dmod16 = a.take(static_cast<i64>(B) * NA * 2);
     p.dsc = a.take(static_cast<i64>(B) * D * 4);
@@ -398,10 +413,14 @@ extern "C" {
 
 int mdt_model_create(const mdt_model_cfg* cfg, mdt_model** out) {
   if (!cfg || !out) return MDT_ERR_ARG;
-  if (cfg->hidden <= 0 || cfg->depth < 0 || cfg->heads <= 0 || cfg->hidden % cfg->heads || cfg->dec_hidden <= 0 ||
-      cfg->dec_heads <= 0 || cfg->dec_hidden % cfg->dec_heads || cfg->patch_size <= 0 ||
-      cfg->img_resolution % cfg->patch_size || cfg->img_channels <= 0 || cfg->num_classes < 0 ||
-      cfg->mlp_hidden <= 0 || cfg->dec_mlp_hidden <= 0)
+  if (cfg->hidden <= 0 || cfg->depth < 0 || cfg->heads <= 0 || cfg->hidden % cfg->heads || cfg->patch_size <= 0 ||
+      cfg->img_resolution % cfg->patch_size || cfg->img_channels <= 0 || cfg->num_classes < 0 || cfg->mlp_hidden <= 0)
+    return MDT_ERR_ARG;
+  // no decoder: every dec_* field 0 and no mask token; otherwise a complete decoder description
+  const bool no_dec = cfg->dec_hidden == 0 && cfg->dec_depth == 0 && cfg->dec_heads == 0 && cfg->dec_mlp_hidden == 0;
+  if (no_dec ? cfg->has_mask_token != 0
+             : (cfg->dec_hidden <= 0 || cfg->dec_depth < 0 || cfg->dec_heads <= 0 || cfg->dec_hidden % cfg->dec_heads ||
+                cfg->dec_mlp_hidden <= 0))
     return MDT_ERR_ARG;
   mdt_model* m = new mdt_model();
   m->cfg = *cfg;
@@ -489,8 +508,20 @@ int mdt_forward(const mdt_model* m, const float* w32, const void* w16, const flo
 
   for (size_t i = 0; i < m->enc.size(); ++i) X = block_fwd(c, m->enc[i], p.enc[i], X, mod, B, T, save != 0);
 
+  i64 o = m->off_final;
+  if (!m->has_dec) {
+    // FinalLayer on the encoder's tokens (models/maskdit.py:550); training with a mask scatters the kept rows back and
+    // fills the removed ones with zeros (:551-553)
+    c.ck(mdt_ln_modulate(X, mod + o, mod + o + D, NA, T, c.at<void>(p.xf), save ? c.at<float>(p.mean_f) : nullptr,
+                         save ? c.at<float>(p.rstd_f) : nullptr, static_cast<int>(Me), D, 1e-6f, stream));
+    float* Fk = ids_restore ? c.at<float>(p.fk) : F_out;
+    Gemm(c.at<void>(p.xf), c.W16(m->flw), Me, m->pd, D).out32(Fk).bias(c.W32(m->flb)).run(c);
+    if (ids_restore) c.ck(mdt_unmask_tokens(Fk, nullptr, nullptr, ids_restore, F_out, B, T, L, m->pd, stream));
+    return c.rc;
+  }
+
   // DecoderLayer (models/maskdit.py:209-213) + unmask_tokens + decoder_pos_embed (:539-545)
-  i64 o = m->off_declayer;
+  o = m->off_declayer;
   c.ck(mdt_ln_modulate(X, mod + o, mod + o + D, NA, T, c.at<void>(p.xmd), save ? c.at<float>(p.mean_d) : nullptr,
                        save ? c.at<float>(p.rstd_d) : nullptr, static_cast<int>(Me), D, 1e-6f, stream));
   float* u = c.at<float>(p.u);
@@ -525,44 +556,63 @@ int mdt_backward(const mdt_model* m, const float* w32, const void* w16, float* g
   float* dmod = c.at<float>(p.dmod);
   if (cudaMemsetAsync(dmod, 0, static_cast<size_t>(B) * NA * 4, cs) != cudaSuccess) return MDT_ERR_CUDA;
 
-  // ---- final layer
-  i64 o = m->off_final;
-  const int nd = static_cast<int>(m->dec.size()), ne = static_cast<int>(m->enc.size());
-  const float* Z_out = nd ? c.at<float>(p.dec[nd - 1].X2) : c.at<float>(p.Z);
-  wgrad(c, dF_bf16, c.at<void>(p.xf), pd, Dd, Md, c.Gd(m->flw));
-  c.ck(mdt_colsum_bf16(dF_bf16, static_cast<int>(Md), pd, pd, c.Gd(m->flb), stream));
-  Gemm(dF_bf16, c.W16(m->flw), Md, Dd, pd, false, true).out16(c.at<void>(p.dxf)).run(c);
-  float* Gz = c.at<float>(p.Gz);
+  const int ne = static_cast<int>(m->enc.size());
   void* dyA = c.at<void>(p.dyA);
-  // every LN backward finishes the residual-stream gradient that the NEXT gate backward consumes: one fused pass
-  {
-    GateNext gn;
-    if (nd) gn = mlp_gate(c, m->dec[nd - 1], p.dec[nd - 1], mod, dmod, dyA);
-    ln_bwd_gate(c, c.at<void>(p.dxf), Z_out, c.at<float>(p.mean_f), c.at<float>(p.rstd_f), mod + o + Dd, L, Gz, 0,
-                dmod + o, dmod + o + Dd, Md, Dd, nd ? &gn : nullptr);
+  // the LN backward that starts the encoder's residual-stream gradient: of the decoder layer, or of the final layer
+  // when there is no decoder (its adaLN offset, input gradient and saved statistics)
+  i64 o = m->off_final;
+  const void* dx_top = c.at<void>(p.dxf);
+  const float *mean_top = c.at<float>(p.mean_f), *rstd_top = c.at<float>(p.rstd_f);
+  if (!m->has_dec) {
+    // ---- final layer on the kept tokens: the rows of removed tokens are constant zeros in the forward
+    // (models/maskdit.py:551-553), so their dF (the MAE term's gradient seed) is dropped
+    const void* dFk = dF_bf16;
+    if (ids_keep) {
+      c.ck(mdt_gather_rows_bf16(dF_bf16, ids_keep, c.at<void>(p.fk), B, T, L, pd, stream));
+      dFk = c.at<void>(p.fk);
+    }
+    wgrad(c, dFk, c.at<void>(p.xf), pd, D, Me, c.Gd(m->flw));
+    c.ck(mdt_colsum_bf16(dFk, static_cast<int>(Me), pd, pd, c.Gd(m->flb), stream));
+    Gemm(dFk, c.W16(m->flw), Me, D, pd, false, true).out16(c.at<void>(p.dxf)).run(c);
+  } else {
+    // ---- final layer
+    const int nd = static_cast<int>(m->dec.size());
+    const float* Z_out = nd ? c.at<float>(p.dec[nd - 1].X2) : c.at<float>(p.Z);
+    wgrad(c, dF_bf16, c.at<void>(p.xf), pd, Dd, Md, c.Gd(m->flw));
+    c.ck(mdt_colsum_bf16(dF_bf16, static_cast<int>(Md), pd, pd, c.Gd(m->flb), stream));
+    Gemm(dF_bf16, c.W16(m->flw), Md, Dd, pd, false, true).out16(c.at<void>(p.dxf)).run(c);
+    float* Gz = c.at<float>(p.Gz);
+    // every LN backward finishes the residual-stream gradient that the NEXT gate backward consumes: one fused pass
+    {
+      GateNext gn;
+      if (nd) gn = mlp_gate(c, m->dec[nd - 1], p.dec[nd - 1], mod, dmod, dyA);
+      ln_bwd_gate(c, c.at<void>(p.dxf), Z_out, c.at<float>(p.mean_f), c.at<float>(p.rstd_f), mod + o + Dd, L, Gz, 0,
+                  dmod + o, dmod + o + Dd, Md, Dd, nd ? &gn : nullptr);
+    }
+    // ---- decoder blocks (last to first)
+    for (int i = nd - 1; i >= 0; --i) {
+      const float* Xin = i > 0 ? c.at<float>(p.dec[i - 1].X2) : c.at<float>(p.Z);
+      GateNext gn;
+      if (i > 0) gn = mlp_gate(c, m->dec[i - 1], p.dec[i - 1], mod, dmod, dyA);
+      block_bwd(c, p, m->dec[i], p.dec[i], Xin, Gz, mod, dmod, B, L, dyA, i > 0 ? &gn : nullptr);
+      if (on_ready && c.rc == MDT_OK) on_ready(user, m->dec[i].lo, m->dec[i].hi);
+    }
+    // ---- unmask + decoder layer
+    float* tok_g = (cf.has_mask_token && ids_restore) ? c.Gd(m->mask_token) : nullptr;
+    c.ck(mdt_unmask_tokens_bwd(Gz, nullptr, ids_restore, c.at<void>(p.du), tok_g, B, T, L, Dd, stream));
+    o = m->off_declayer;
+    wgrad(c, c.at<void>(p.du), c.at<void>(p.xmd), Dd, D, Me, c.Gd(m->dlw));
+    c.ck(mdt_colsum_bf16(c.at<void>(p.du), static_cast<int>(Me), Dd, Dd, c.Gd(m->dlb), stream));
+    Gemm(c.at<void>(p.du), c.W16(m->dlw), Me, D, Dd, false, true).out16(c.at<void>(p.dxmd)).run(c);
+    dx_top = c.at<void>(p.dxmd), mean_top = c.at<float>(p.mean_d), rstd_top = c.at<float>(p.rstd_d);
   }
-  // ---- decoder blocks (last to first)
-  for (int i = nd - 1; i >= 0; --i) {
-    const float* Xin = i > 0 ? c.at<float>(p.dec[i - 1].X2) : c.at<float>(p.Z);
-    GateNext gn;
-    if (i > 0) gn = mlp_gate(c, m->dec[i - 1], p.dec[i - 1], mod, dmod, dyA);
-    block_bwd(c, p, m->dec[i], p.dec[i], Xin, Gz, mod, dmod, B, L, dyA, i > 0 ? &gn : nullptr);
-    if (on_ready && c.rc == MDT_OK) on_ready(user, m->dec[i].lo, m->dec[i].hi);
-  }
-  // ---- unmask + decoder layer
-  float* tok_g = (cf.has_mask_token && ids_restore) ? c.Gd(m->mask_token) : nullptr;
-  c.ck(mdt_unmask_tokens_bwd(Gz, nullptr, ids_restore, c.at<void>(p.du), tok_g, B, T, L, Dd, stream));
-  o = m->off_declayer;
-  wgrad(c, c.at<void>(p.du), c.at<void>(p.xmd), Dd, D, Me, c.Gd(m->dlw));
-  c.ck(mdt_colsum_bf16(c.at<void>(p.du), static_cast<int>(Me), Dd, Dd, c.Gd(m->dlb), stream));
-  Gemm(c.at<void>(p.du), c.W16(m->dlw), Me, D, Dd, false, true).out16(c.at<void>(p.dxmd)).run(c);
   float* Ge = c.at<float>(p.Ge);
   const float* X_enc = ne ? c.at<float>(p.enc[ne - 1].X2) : c.at<float>(p.X0);
   {
     GateNext gn;
     if (ne) gn = mlp_gate(c, m->enc[ne - 1], p.enc[ne - 1], mod, dmod, dyA);
-    ln_bwd_gate(c, c.at<void>(p.dxmd), X_enc, c.at<float>(p.mean_d), c.at<float>(p.rstd_d), mod + o + D, T, Ge, 0,
-                dmod + o, dmod + o + D, Me, D, ne ? &gn : nullptr);
+    ln_bwd_gate(c, dx_top, X_enc, mean_top, rstd_top, mod + o + D, T, Ge, 0, dmod + o, dmod + o + D, Me, D,
+                ne ? &gn : nullptr);
   }
   // ---- encoder blocks
   for (int i = ne - 1; i >= 0; --i) {

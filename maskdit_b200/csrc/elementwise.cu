@@ -504,6 +504,7 @@ ln_bwd_gate_kernel(const __nv_bfloat16* __restrict__ dxmod, const float* __restr
 // unmask_tokens (+ decoder_pos_embed) and its backward.  Thread owns 4 columns; block = D/4 threads x 16 positions.
 // =========================================================================================================
 constexpr int kUmPos = 64;  // positions per block (backward: one 16-byte mask-token reduction per thread and block)
+template <bool kPos>  // false: no position term (the decoder-less DiT's zero-filled output scatter)
 __global__ void unmask_kernel(const float* __restrict__ u, const float* __restrict__ mask_token,
                               const float* __restrict__ pos, const int64_t* __restrict__ ids_restore,
                               float* __restrict__ out, int T, int L, int D) {
@@ -522,7 +523,7 @@ __global__ void unmask_kernel(const float* __restrict__ u, const float* __restri
     for (int j = 0; j < 4; ++j) {
       if (r[j] < 0) continue;
       v[j] = (r[j] < T) ? *reinterpret_cast<const float4*>(u + (static_cast<size_t>(b) * T + r[j]) * D + c) : mt;
-      pe[j] = *reinterpret_cast<const float4*>(pos + static_cast<size_t>(l + j) * D + c);
+      pe[j] = kPos ? *reinterpret_cast<const float4*>(pos + static_cast<size_t>(l + j) * D + c) : make_float4(0, 0, 0, 0);
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -563,6 +564,19 @@ __global__ void unmask_bwd_kernel(const float* __restrict__ g, const int64_t* __
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dmask_token + c), "f"(acc.x), "f"(acc.y),
                  "f"(acc.z), "f"(acc.w)
                  : "memory");
+  }
+}
+
+
+// Row gather of a bf16 matrix: out[b*T + i, :] = in[b*L + idx[b*T + i], :].  Thread moves 4 elements (8 bytes).
+__global__ void gather_rows_bf16_kernel(const uint2* __restrict__ in, const int64_t* __restrict__ idx,
+                                        uint2* __restrict__ out, int T, int L, int D4, long long n) {
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long row = i / D4;
+    const int c = static_cast<int>(i - row * D4);
+    const long long b = row / T;
+    out[i] = in[(b * L + idx[row]) * D4 + c];
   }
 }
 
@@ -732,10 +746,14 @@ int mdt_ln_modulate_bwd_gate(const void* dxmod_bf16, const float* x, const float
 
 int mdt_unmask_tokens(const float* u, const float* mask_token, const float* pos, const int64_t* ids_restore,
                       float* out, int B, int T, int L, int D, void* stream) {
-  if (!u || !pos || !out || B <= 0 || T <= 0 || L <= 0 || D % 4 || D > 4096) return MDT_ERR_ARG;
+  if (!u || !out || B <= 0 || T <= 0 || L <= 0 || D % 4 || D > 4096) return MDT_ERR_ARG;
   if (!ids_restore && T != L) return MDT_ERR_ARG;
   dim3 grid((L + kUmPos - 1) / kUmPos, B);
-  unmask_kernel<<<grid, ((D / 4 + 31) / 32) * 32, 0, S(stream)>>>(u, mask_token, pos, ids_restore, out, T, L, D);
+  const int threads = ((D / 4 + 31) / 32) * 32;
+  if (pos)
+    unmask_kernel<true><<<grid, threads, 0, S(stream)>>>(u, mask_token, pos, ids_restore, out, T, L, D);
+  else
+    unmask_kernel<false><<<grid, threads, 0, S(stream)>>>(u, mask_token, nullptr, ids_restore, out, T, L, D);
   return launch_status();
 }
 
@@ -747,6 +765,16 @@ int mdt_unmask_tokens_bwd(const float* g, const int64_t* ids_keep, const int64_t
   dim3 grid((L + kUmPos - 1) / kUmPos, B);
   unmask_bwd_kernel<<<grid, ((D / 4 + 31) / 32) * 32, 0, S(stream)>>>(
       g, ids_restore, static_cast<__nv_bfloat16*>(du_bf16), dmask_token, T, L, D);
+  return launch_status();
+}
+
+int mdt_gather_rows_bf16(const void* in_bf16, const int64_t* idx, void* out_bf16, int B, int T, int L, int D,
+                         void* stream) {
+  if (!in_bf16 || !idx || !out_bf16 || B <= 0 || T <= 0 || T > L || D <= 0 || D % 4) return MDT_ERR_ARG;
+  if ((reinterpret_cast<uintptr_t>(in_bf16) | reinterpret_cast<uintptr_t>(out_bf16)) & 7) return MDT_ERR_ARG;
+  const long long n = static_cast<long long>(B) * T * (D / 4);
+  gather_rows_bf16_kernel<<<ew_grid(n), 256, 0, S(stream)>>>(static_cast<const uint2*>(in_bf16), idx,
+                                                              static_cast<uint2*>(out_bf16), T, L, D / 4, n);
   return launch_status();
 }
 

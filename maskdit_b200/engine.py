@@ -32,19 +32,24 @@ class Engine:
     def __init__(self, cfg, store):
         self.cfg, self.store = cfg, store
         D, Dd = cfg.hidden, cfg.dec_hidden
+        # dec_hidden == 0: the decoder-less DiT (use_decoder=False), final layer on the encoder width
+        self.has_dec = Dd > 0
         off = 0
         self.enc = []
         for i in range(cfg.depth):
             self.enc.append(BlockSpec(f"model.blocks.{i}", D, cfg.heads, off))
             off += 6 * D
-        self.off_declayer = off
-        off += 2 * D
+        self.off_declayer = None
         self.dec = []
-        for i in range(cfg.dec_depth):
-            self.dec.append(BlockSpec(f"model.decoder_blocks.{i}", Dd, cfg.dec_heads, off))
-            off += 6 * Dd
+        if self.has_dec:
+            self.off_declayer = off
+            off += 2 * D
+            for i in range(cfg.dec_depth):
+                self.dec.append(BlockSpec(f"model.decoder_blocks.{i}", Dd, cfg.dec_heads, off))
+                off += 6 * Dd
+        self.Df = Dd if self.has_dec else D
         self.off_final = off
-        off += 2 * Dd
+        off += 2 * self.Df
         self.NA = off
         assert store.ada_w_range[1] == self.NA, (store.ada_w_range, self.NA)
 
@@ -116,6 +121,20 @@ class Engine:
             if save:
                 ctx["enc"].append(saved)
 
+        pd = cfg.patch_dim
+        if not self.has_dec:
+            # FinalLayer on the encoder's tokens (models/maskdit.py:550); with a mask the kept rows are scattered back
+            # and the removed ones are zeros (:551-553)
+            o = self.off_final
+            xf, mean_f, rstd_f = ops.ln_modulate(X, mod[:, o:], mod[:, o + D:], NA, T, Me, D, save_stats=save)
+            Fk = torch.empty(Me, pd, dtype=f32, device=X.device)
+            gemm(xf, self.w16("model.final_layer.linear.weight"), Me, pd, D, out=Fk,
+                 bias=self.w32("model.final_layer.linear.bias"))
+            Fo = Fk if ids_restore is None else ops.unmask_tokens(Fk, None, None, ids_restore, B, T, L, pd).view(Md, pd)
+            if save:
+                ctx.update(X_enc=X, xf=xf, mean_f=mean_f, rstd_f=rstd_f)
+            return Fo, ctx
+
         # DecoderLayer (models/maskdit.py:209-213) + unmask_tokens + decoder_pos_embed (:539-545)
         o = self.off_declayer
         xmd, mean_d, rstd_d = ops.ln_modulate(X, mod[:, o:], mod[:, o + D:], NA, T, Me, D, save_stats=save)
@@ -134,7 +153,6 @@ class Engine:
         # FinalLayer (models/maskdit.py:230-234)
         o = self.off_final
         xf, mean_f, rstd_f = ops.ln_modulate(Z, mod[:, o:], mod[:, o + Dd:], NA, L, Md, Dd, save_stats=save)
-        pd = cfg.patch_dim
         Fo = torch.empty(Md, pd, dtype=f32, device=X.device)
         gemm(xf, self.w16("model.final_layer.linear.weight"), Md, pd, Dd, out=Fo,
              bias=self.w32("model.final_layer.linear.bias"))
@@ -188,39 +206,55 @@ class Engine:
         dev = mod.device
         dmod = torch.zeros(B, NA, dtype=f32, device=dev)
 
-        # ---- final layer
+        # the LN backward that starts the encoder's residual-stream gradient: of the decoder layer, or of the final
+        # layer when there is no decoder
         o = self.off_final
-        self._wgrad(dF16, ctx["xf"], pd, Dd, Md, G("model.final_layer.linear.weight"))
-        ops.colsum(dF16, G("model.final_layer.linear.bias"))
-        dxf = torch.empty(Md, Dd, dtype=bf16, device=dev)
-        gemm(dF16, self.w16("model.final_layer.linear.weight"), Md, Dd, pd, b_mn=True, out=dxf)
-        Gz = torch.empty(Md, Dd, dtype=f32, device=dev)
-        # every LN backward finishes the residual-stream gradient that the NEXT gate backward consumes: one fused pass
-        dec, dec_sv = list(reversed(self.dec)), list(reversed(ctx["dec"]))
-        dy2 = ops.ln_modulate_bwd_gate(dxf, ctx["Z_out"], ctx["mean_f"], ctx["rstd_f"], mod[:, o + Dd:], NA, L, Gz,
-                                       False, dmod[:, o:], dmod[:, o + Dd:], NA, Md, Dd,
-                                       gate_next=self._mlp_gate(dec[0], dec_sv[0], mod, dmod) if dec else None)
-        # ---- decoder blocks
-        for i, (spec, saved) in enumerate(zip(dec, dec_sv)):
-            nxt = self._mlp_gate(dec[i + 1], dec_sv[i + 1], mod, dmod) if i + 1 < len(dec) else None
-            dy2 = self._block_bwd(spec, saved, Gz, mod, dmod, B, L, dy2, nxt)
-            if on_ready is not None:
-                on_ready(*st.prefix_range(spec.prefix + "."))
-        # ---- unmask + decoder layer
-        tok_g = G("model.mask_token").view(Dd) if "model.mask_token" in st.offsets and ctx["ids_restore"] is not None \
-            else None
-        du = ops.unmask_tokens_bwd(Gz, ctx["ids_restore"], tok_g, B, T, L, Dd)
-        del Gz
-        o = self.off_declayer
-        self._wgrad(du, ctx["xmd"], Dd, D, Me, G("model.decoder_layer.linear.weight"))
-        ops.colsum(du, G("model.decoder_layer.linear.bias"))
-        dxmd = torch.empty(Me, D, dtype=bf16, device=dev)
-        gemm(du, self.w16("model.decoder_layer.linear.weight"), Me, D, Dd, b_mn=True, out=dxmd)
+        if not self.has_dec:
+            # ---- final layer on the kept tokens: the removed tokens' rows are constant zeros in the forward
+            # (models/maskdit.py:551-553), so their dF (the MAE term's gradient seed) is dropped
+            dFk = dF16 if ctx["ids_keep"] is None else ops.gather_rows_bf16(dF16, ctx["ids_keep"], B, T, L, pd)
+            self._wgrad(dFk, ctx["xf"], pd, D, Me, G("model.final_layer.linear.weight"))
+            ops.colsum(dFk, G("model.final_layer.linear.bias"))
+            dx_top = torch.empty(Me, D, dtype=bf16, device=dev)
+            gemm(dFk, self.w16("model.final_layer.linear.weight"), Me, D, pd, b_mn=True, out=dx_top)
+            del dFk
+            mean_top, rstd_top = ctx["mean_f"], ctx["rstd_f"]
+        else:
+            # ---- final layer
+            self._wgrad(dF16, ctx["xf"], pd, Dd, Md, G("model.final_layer.linear.weight"))
+            ops.colsum(dF16, G("model.final_layer.linear.bias"))
+            dxf = torch.empty(Md, Dd, dtype=bf16, device=dev)
+            gemm(dF16, self.w16("model.final_layer.linear.weight"), Md, Dd, pd, b_mn=True, out=dxf)
+            Gz = torch.empty(Md, Dd, dtype=f32, device=dev)
+            # every LN backward finishes the residual-stream gradient that the NEXT gate backward consumes: one fused
+            # pass
+            dec, dec_sv = list(reversed(self.dec)), list(reversed(ctx["dec"]))
+            dy2 = ops.ln_modulate_bwd_gate(dxf, ctx["Z_out"], ctx["mean_f"], ctx["rstd_f"], mod[:, o + Dd:], NA, L, Gz,
+                                           False, dmod[:, o:], dmod[:, o + Dd:], NA, Md, Dd,
+                                           gate_next=self._mlp_gate(dec[0], dec_sv[0], mod, dmod) if dec else None)
+            # ---- decoder blocks
+            for i, (spec, saved) in enumerate(zip(dec, dec_sv)):
+                nxt = self._mlp_gate(dec[i + 1], dec_sv[i + 1], mod, dmod) if i + 1 < len(dec) else None
+                dy2 = self._block_bwd(spec, saved, Gz, mod, dmod, B, L, dy2, nxt)
+                if on_ready is not None:
+                    on_ready(*st.prefix_range(spec.prefix + "."))
+            # ---- unmask + decoder layer
+            tok_g = G("model.mask_token").view(Dd) if "model.mask_token" in st.offsets and \
+                ctx["ids_restore"] is not None else None
+            du = ops.unmask_tokens_bwd(Gz, ctx["ids_restore"], tok_g, B, T, L, Dd)
+            del Gz
+            o = self.off_declayer
+            self._wgrad(du, ctx["xmd"], Dd, D, Me, G("model.decoder_layer.linear.weight"))
+            ops.colsum(du, G("model.decoder_layer.linear.bias"))
+            dx_top = torch.empty(Me, D, dtype=bf16, device=dev)
+            gemm(du, self.w16("model.decoder_layer.linear.weight"), Me, D, Dd, b_mn=True, out=dx_top)
+            mean_top, rstd_top = ctx["mean_d"], ctx["rstd_d"]
         Ge = torch.empty(Me, D, dtype=f32, device=dev)
         enc, enc_sv = list(reversed(self.enc)), list(reversed(ctx["enc"]))
-        dy2 = ops.ln_modulate_bwd_gate(dxmd, ctx["X_enc"], ctx["mean_d"], ctx["rstd_d"], mod[:, o + D:], NA, T, Ge,
+        dy2 = ops.ln_modulate_bwd_gate(dx_top, ctx["X_enc"], mean_top, rstd_top, mod[:, o + D:], NA, T, Ge,
                                        False, dmod[:, o:], dmod[:, o + D:], NA, Me, D,
                                        gate_next=self._mlp_gate(enc[0], enc_sv[0], mod, dmod) if enc else None)
+        del dx_top
         # ---- encoder blocks
         for i, (spec, saved) in enumerate(zip(enc, enc_sv)):
             nxt = self._mlp_gate(enc[i + 1], enc_sv[i + 1], mod, dmod) if i + 1 < len(enc) else None
@@ -359,10 +393,14 @@ class CEngine:
             raise ops.L.MdtError("mdt_workspace_bytes failed")
         return n
 
-    def _count(self, save):
+    def _count(self, masked):
         """Kernel launches of one forward / backward (for bench.py's gpu_launches claim): same sequence as `Engine`."""
         c = self.cfg
         nb = c.depth + c.dec_depth
+        if c.dec_hidden == 0:   # no decoder: final 2 (+ zero-filled scatter) / final 4 (+ kept-row gather of dF)
+            fwd = 9 + (2 if c.num_classes else 0) + 7 * nb + int(masked)          # embed/conditioning 7
+            bwd = 16 + 13 * nb + (1 if c.num_classes else 0) + int(masked)        # patch-embed 1, conditioning 11
+            return fwd, bwd
         fwd = 12 + (2 if c.num_classes else 0) + 7 * nb          # embed/conditioning 7, decoder layer 3, final 2
         bwd = 21 + 13 * nb + (1 if c.num_classes else 0)         # final 4, transition 5, patch-embed 1, conditioning 11
         return fwd, bwd
@@ -382,7 +420,7 @@ class CEngine:
         ops.check(self._L.mdt_forward(self._h, ops.ptr(st.w32), ops.ptr(st.w16), ops.ptr(x_in), ops.ptr(sigma),
                                       ops.ptr(labels), ops.ptr(ids_keep), ops.ptr(ids_restore), B, T, int(save),
                                       ops.ptr(ws), nbytes, ops.ptr(Fo), ops.stream_ptr()), "mdt_forward",
-                  self._count(save)[0])
+                  self._count(ids_restore is not None)[0])
         ctx = None
         if save:
             ctx = dict(ws=ws, nbytes=nbytes, x_in=x_in, sigma=sigma, ids_keep=ids_keep, ids_restore=ids_restore, B=B,
@@ -398,7 +436,8 @@ class CEngine:
         ops.check(self._L.mdt_backward(self._h, ops.ptr(st.w32), ops.ptr(st.w16), ops.ptr(st.grad), ops.ptr(ctx["x_in"]),
                                        ops.ptr(ctx["sigma"]), ops.ptr(ctx["ids_keep"]), ops.ptr(ctx["ids_restore"]),
                                        ops.ptr(dF16), ctx["B"], ctx["T"], ops.ptr(ctx["ws"]), ctx["nbytes"], cb, None,
-                                       ops.stream_ptr()), "mdt_backward", self._count(True)[1])
+                                       ops.stream_ptr()), "mdt_backward",
+                  self._count(ctx["ids_restore"] is not None)[1])
 
 
 def make_engine(cfg, store):

@@ -8,8 +8,11 @@ Exports the same registries the reference's entry points consume (SURVEY.md §8b
 checkpoints and the reference's own `EDMLoss`/`edm_sampler` work against it unchanged.  Its arithmetic is the
 CUDA engine (`engine.py`); there is no PyTorch fallback: calling it with CPU tensors raises.
 
-Scope (matches every config the reference ships): use_decoder=True, pad_cls_token=False, ext_feature_dim=0,
-use_encoder_feat=False, learn_sigma=False.  Other flag combinations raise NotImplementedError.
+Scope: the asymmetric encoder-decoder MaskDiT (use_decoder=True, every config the reference ships) and the plain
+decoder-less DiT (use_decoder=False, the reference's default: the final layer runs on the encoder width, and training
+with a mask fills the removed patches of the output with zeros, models/maskdit.py:550-553), each at any mask ratio,
+with or without classes.  pad_cls_token, direct_cls_token, ext_feature_dim, use_encoder_feat and learn_sigma must be
+off; other flag combinations raise NotImplementedError.
 """
 from __future__ import annotations
 
@@ -64,9 +67,6 @@ class DiT(nn.Module):
         if learn_sigma or pad_cls_token or direct_cls_token or ext_feature_dim or use_encoder_feat:
             raise NotImplementedError("maskdit_b200 covers the shipped configs: learn_sigma/pad_cls_token/"
                                       "ext_feature_dim/use_encoder_feat must be off")
-        if not use_decoder:
-            raise NotImplementedError("maskdit_b200 implements the asymmetric encoder-decoder MaskDiT "
-                                      "(use_decoder=True), as in every reference config")
         self.learn_sigma, self.in_channels, self.out_channels = learn_sigma, in_channels, in_channels
         self.patch_size, self.num_heads, self.class_dropout_prob = patch_size, num_heads, class_dropout_prob
         self.num_classes, self.use_decoder, self.mae_loss_coef = num_classes, use_decoder, mae_loss_coef
@@ -74,7 +74,8 @@ class DiT(nn.Module):
         self.ext_feature_dim, self.use_encoder_feat = 0, False
         self.cls_token, self.extras, self.decoder_extras = None, 0, 0
         self.input_size, self.hidden_size, self.depth, self.mlp_ratio = input_size, hidden_size, depth, mlp_ratio
-        self.decoder_hidden_size, self.decoder_depth, self.decoder_num_heads = 512, 8, 16  # maskdit.py:310-312
+        # decoder: maskdit.py:310-312; none without use_decoder (final layer on the encoder width, :308,329-331)
+        self.decoder_hidden_size, self.decoder_depth, self.decoder_num_heads = (512, 8, 16) if use_decoder else (0, 0, 0)
         grid = input_size // patch_size
         self.num_patches = grid * grid
         D, Dd, L = hidden_size, self.decoder_hidden_size, self.num_patches
@@ -111,12 +112,15 @@ class DiT(nn.Module):
         self.t_embedder = seq(mlp=seq(_0=linear(D, 256), _2=linear(D, D)))
         self.y_embedder = seq(embedding_table=linear(D, num_classes, bias=False)) if num_classes else None
         self.blocks = nn.ModuleList([block(D, D) for _ in range(depth)])
-        self.decoder_pos_embed = P(1, L, Dd, grad=False)
-        self.decoder_layer = seq(linear=linear(Dd, D), adaLN_modulation=seq(_1=linear(2 * D, D)))
-        self.decoder_blocks = nn.ModuleList([block(Dd, D) for _ in range(self.decoder_depth)])
-        self.mask_token = P(1, 1, Dd) if mae_loss_coef > 0 else None
-        self.final_layer = seq(linear=linear(patch_size * patch_size * self.out_channels, Dd),
-                               adaLN_modulation=seq(_1=linear(2 * Dd, D)))
+        self.decoder_pos_embed = self.decoder_layer = self.decoder_blocks = self.mask_token = None
+        if use_decoder:
+            self.decoder_pos_embed = P(1, L, Dd, grad=False)
+            self.decoder_layer = seq(linear=linear(Dd, D), adaLN_modulation=seq(_1=linear(2 * D, D)))
+            self.decoder_blocks = nn.ModuleList([block(Dd, D) for _ in range(self.decoder_depth)])
+            self.mask_token = P(1, 1, Dd) if mae_loss_coef > 0 else None
+        Df = Dd if use_decoder else D
+        self.final_layer = seq(linear=linear(patch_size * patch_size * self.out_channels, Df),
+                               adaLN_modulation=seq(_1=linear(2 * Df, D)))
         self.reset_parameters()
 
     @torch.no_grad()

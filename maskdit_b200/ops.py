@@ -161,6 +161,14 @@ def unmask_tokens_bwd(g, ids_restore, dmask_token, B, T, Lt, D):
     return du
 
 
+def gather_rows_bf16(x, idx, B, T, Lt, D):
+    """out[b*T + i] = x[b*Lt + idx[b, i]] for a bf16 x [B*Lt, D] and idx [B, T] int64 -> [B*T, D] bf16."""
+    _c(x, bf16), _c(idx, torch.int64)
+    out = torch.empty(B * T, D, dtype=bf16, device=x.device)
+    check(lib().mdt_gather_rows_bf16(ptr(x), ptr(idx), ptr(out), B, T, Lt, D, stream_ptr()), "mdt_gather_rows_bf16")
+    return out
+
+
 def edm_loss(F, xin, y, sigma, mask, gl, sigma_data, mae_coef, p, want_D=False, want_dF=True):
     B, C, R, _ = xin.shape
     loss = torch.empty(B, dtype=f32, device=xin.device)

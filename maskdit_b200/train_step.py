@@ -178,7 +178,8 @@ class TrainStep:
     def state_dict(self):
         """AdamW state laid out like `torch.optim.AdamW(net.parameters()).state_dict()` / apex FusedAdam's
         (train.py:141,262): `state` is keyed by the parameter's POSITION in `net.parameters()` — frozen tensors
-        (pos_embed = 0, decoder_pos_embed = 1) keep their index but own no state, so the first key is 2 — with
+        (pos_embed = 0, decoder_pos_embed = 1) keep their index but own no state, so the first key is 2 (1 for the
+        decoder-less DiT, whose only frozen tensor is pos_embed) — with
         `exp_avg` / `exp_avg_sq` and a per-parameter `step` (torch layout); the step count is also stored in the
         param_group (apex layout).  Tensors are copies on the current device."""
         state, n_all = {}, 0
