@@ -100,6 +100,9 @@ int mdt_mask_indices(const float* noise, int B, int L, int len_keep, int64_t* id
  *   W [D, C*p*p] f32 (Conv2d weight flattened (c,ph,pw)), bias [D], pos [L,D] f32,
  *   ids_keep [B,T] i64 or NULL (NULL: T == L, identity) -> out [B,T,D] f32
  * Backward: gW [D, C*p*p] += sum g (x) patch, gb [D] += sum g    (no input gradient is needed)
+ * Supported: cpp = C*p*p <= 384 (every DiT_models patch size at 4 channels: 16, 64, 256), so one block's patch
+ * rows stay within 48 KB of shared memory; MDT_ERR_UNSUPPORTED above.  The backward takes 128 tokens per block for
+ * cpp <= 96 and 32 above.
  * ------------------------------------------------------------------------------------------------------------ */
 int mdt_patch_embed(const float* x, const float* sigma, float sigma_data, const float* W, const float* bias,
                     const float* pos, const int64_t* ids_keep, float* out, int B, int C, int R, int p, int D, int T,
@@ -188,6 +191,8 @@ int mdt_gather_rows_bf16(const void* in_bf16, const int64_t* idx, void* out_bf16
  *                                                            train_utils/loss.py:37,44-52,73-101
  *   mask == NULL: loss[b] = mean(w (D-y)^2)                  loss.py:54
  *   dF_bf16 (optional) = d(sum_b gl[b]*loss[b]) / dF ; Dx (optional) [B,C,R,R] f32.
+ * Any pd = p*p*C: up to 64 (patch 2 and 4 at 4 channels) a token's D and xin are held in registers; above (patch 8:
+ * pd 256) the later passes re-read F and xin.  The output scaling below has no pd bound.
  * ------------------------------------------------------------------------------------------------------------ */
 int mdt_edm_loss(const float* F, const float* xin, const float* y, const float* sigma, const float* mask,
                  const float* gl, float sigma_data, float mae_coef, float* loss, float* Dx, void* dF_bf16, int B,

@@ -36,10 +36,10 @@ __global__ void mask_indices_kernel(const float* __restrict__ noise, int L, int 
 }
 
 // =========================================================================================================
-// PatchEmbed (+c_in, +pos_embed, +kept-token gather).  Block = 8 tokens of one sample, threads over D.
+// PatchEmbed (+c_in, +pos_embed, +kept-token gather).  Block = kPeTok tokens of one sample, threads over D.
 // =========================================================================================================
 constexpr int kPeTok = 32;   // tokens per block: the weight row of a channel (C*p*p floats) is read once per 32 tokens
-constexpr int kPeMaxCpp = 64;
+constexpr int kPeMaxCpp = 48 * 1024 / (kPeTok * 4);   // 384: the [kPeTok][cpp] patch block within 48 KB of smem
 __global__ void patch_embed_kernel(const float* __restrict__ x, const float* __restrict__ sigma, float sigma_data,
                                    const float* __restrict__ W, const float* __restrict__ bias,
                                    const float* __restrict__ pos, const int64_t* __restrict__ ids_keep,
@@ -95,8 +95,11 @@ __global__ void patch_embed_kernel(const float* __restrict__ x, const float* __r
   }
 }
 
-// gW[d, j] += sum_tokens g[tok, d] * patch[tok, j]; gb[d] += sum g.  Block = 64 tokens of one sample.
-constexpr int kPebTok = 128;  // tokens per block (one atomic per (channel, weight) per block)
+// gW[d, j] += sum_tokens g[tok, d] * patch[tok, j]; gb[d] += sum g.  Block = kPebTok tokens of one sample.
+// kPebTok = 128 tokens per block (one atomic per (channel, weight) per block) for cpp <= 96 (patch 2 and 4 at 4
+// channels); 32 for cpp <= 384 (patch 8: cpp = 256), so the [kPebTok][cpp] patch block stays within 48 KB of smem.
+constexpr int kPebMaxCpp = 48 * 1024 / (32 * 4);
+template <int kPebTok>
 __global__ void patch_embed_bwd_kernel(const float* __restrict__ x, const float* __restrict__ sigma,
                                        float sigma_data, const int64_t* __restrict__ ids_keep,
                                        const float* __restrict__ g, float* __restrict__ gW, float* __restrict__ gb,
@@ -604,6 +607,7 @@ int mdt_patch_embed(const float* x, const float* sigma, float sigma_data, const 
                     void* stream) {
   if (!x || !W || !bias || !pos || !out || B <= 0 || T <= 0 || R % p) return MDT_ERR_ARG;
   const int cpp = C * p * p;
+  if (cpp > kPeMaxCpp) return MDT_ERR_UNSUPPORTED;
   dim3 grid((T + kPeTok - 1) / kPeTok, B);
   patch_embed_kernel<<<grid, 384, kPeTok * cpp * sizeof(float), S(stream)>>>(x, sigma, sigma_data, W, bias, pos,
                                                                              ids_keep, out, C, R, p, D, T);
@@ -614,10 +618,16 @@ int mdt_patch_embed_bwd(const float* x, const float* sigma, float sigma_data, co
                         const float* g, float* gW, float* gb, int B, int C, int R, int p, int D, int T, void* stream) {
   if (!x || !g || !gW || !gb || B <= 0 || T <= 0 || R % p) return MDT_ERR_ARG;
   const int cpp = C * p * p;
-  if (kPebTok * cpp * sizeof(float) > 48 * 1024) return MDT_ERR_UNSUPPORTED;
-  dim3 grid((T + kPebTok - 1) / kPebTok, B);
-  patch_embed_bwd_kernel<<<grid, 384, kPebTok * cpp * sizeof(float), S(stream)>>>(x, sigma, sigma_data, ids_keep, g,
-                                                                                  gW, gb, C, R, p, D, T);
+  if (cpp > kPebMaxCpp) return MDT_ERR_UNSUPPORTED;
+  if (128 * cpp * sizeof(float) <= 48 * 1024) {
+    dim3 grid((T + 127) / 128, B);
+    patch_embed_bwd_kernel<128><<<grid, 384, 128 * cpp * sizeof(float), S(stream)>>>(x, sigma, sigma_data, ids_keep,
+                                                                                      g, gW, gb, C, R, p, D, T);
+  } else {
+    dim3 grid((T + 31) / 32, B);
+    patch_embed_bwd_kernel<32><<<grid, 384, 32 * cpp * sizeof(float), S(stream)>>>(x, sigma, sigma_data, ids_keep, g,
+                                                                                    gW, gb, C, R, p, D, T);
+  }
   return launch_status();
 }
 

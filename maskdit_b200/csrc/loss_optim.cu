@@ -9,7 +9,7 @@ namespace mdt {
 static inline cudaStream_t S(void* s) { return static_cast<cudaStream_t>(s); }
 static inline int launch_status() { return cudaGetLastError() == cudaSuccess ? MDT_OK : MDT_ERR_CUDA; }
 
-constexpr int kMaxPD = 64;  // p*p*C per patch (16 for patch 2 x 4 channels)
+constexpr int kMaxPD = 64;  // p*p*C per patch held in registers by edm_loss (16 for patch 2 x 4 channels)
 
 struct PatchGeom {
   int C, R, p, G, L, pd;
@@ -35,7 +35,9 @@ MDT_DEVINL float block_sum(float v, float* s_buf) {
   return t;
 }
 
-// One block per sample.  Thread per token.
+// One block per sample.  Thread per token.  kReg: the token's D and x live in registers (pd <= kMaxPD); otherwise
+// (patch 8: pd = 256) every later pass re-reads F and xin and recomputes D with the same expression.
+template <bool kReg>
 __global__ void __launch_bounds__(256)
 edm_loss_kernel(const float* __restrict__ F, const float* __restrict__ xin, const float* __restrict__ y,
                 const float* __restrict__ sigma, const float* __restrict__ mask, const float* __restrict__ gl,
@@ -58,7 +60,15 @@ edm_loss_kernel(const float* __restrict__ F, const float* __restrict__ xin, cons
   float acc = 0.f;
   for (int l = threadIdx.x; l < gm.L; l += blockDim.x) {
     const float* f = F + (static_cast<size_t>(b) * gm.L + l) * gm.pd;
-    float dv[kMaxPD], xv[kMaxPD];
+    float dv[kReg ? kMaxPD : 1], xv[kReg ? kMaxPD : 1];
+    auto xat = [&](int j) -> float {
+      if constexpr (kReg) return xv[j];
+      else return xin[gm.pix(b, l, j)];
+    };
+    auto dat = [&](int j) -> float {
+      if constexpr (kReg) return dv[j];
+      else return c_skip * xin[gm.pix(b, l, j)] + c_out * f[j];
+    };
     float se = 0.f, sx = 0.f;
     for (int j = 0; j < gm.pd; ++j) {
       const size_t px = gm.pix(b, l, j);
@@ -66,7 +76,7 @@ edm_loss_kernel(const float* __restrict__ F, const float* __restrict__ xin, cons
       const float d = c_skip * xi + c_out * f[j];
       if (Dx) Dx[px] = d;
       const float e = d - y[px];
-      dv[j] = d, xv[j] = xi;
+      if constexpr (kReg) dv[j] = d, xv[j] = xi;
       se += e * e, sx += xi;
     }
     const float inv_pd = 1.f / gm.pd;
@@ -75,7 +85,7 @@ edm_loss_kernel(const float* __restrict__ F, const float* __restrict__ xin, cons
       if (dF) {
         const float k = glb * w * 2.f * c_out / (static_cast<float>(gm.L) * gm.pd);
         for (int j = 0; j < gm.pd; ++j)
-          dF[(static_cast<size_t>(b) * gm.L + l) * gm.pd + j] = __float2bfloat16_rn(k * (dv[j] - y[gm.pix(b, l, j)]));
+          dF[(static_cast<size_t>(b) * gm.L + l) * gm.pd + j] = __float2bfloat16_rn(k * (dat(j) - y[gm.pix(b, l, j)]));
       }
     } else {
       const float mk = mask[static_cast<size_t>(b) * gm.L + l];
@@ -86,12 +96,12 @@ edm_loss_kernel(const float* __restrict__ F, const float* __restrict__ xin, cons
         // mae_loss (train_utils/loss.py:87-101): target = per-patch normalised NOISY INPUT, unbiased variance
         mu = sx * inv_pd;
         float var = 0.f;
-        for (int j = 0; j < gm.pd; ++j) var += (xv[j] - mu) * (xv[j] - mu);
+        for (int j = 0; j < gm.pd; ++j) var += (xat(j) - mu) * (xat(j) - mu);
         var /= static_cast<float>(gm.pd - 1);
         rstd = rsqrtf(var + 1e-6f);
         float sm = 0.f;
         for (int j = 0; j < gm.pd; ++j) {
-          const float e = dv[j] - (xv[j] - mu) * rstd;
+          const float e = dat(j) - (xat(j) - mu) * rstd;
           sm += e * e;
         }
         contrib += mae_coef * mk * sm * inv_pd / n_mask;
@@ -100,8 +110,9 @@ edm_loss_kernel(const float* __restrict__ F, const float* __restrict__ xin, cons
       acc += contrib;
       if (dF) {
         for (int j = 0; j < gm.pd; ++j) {
-          float gval = k_edm * (dv[j] - y[gm.pix(b, l, j)]);
-          if (k_mae != 0.f) gval += k_mae * (dv[j] - (xv[j] - mu) * rstd);
+          const float dj = dat(j);
+          float gval = k_edm * (dj - y[gm.pix(b, l, j)]);
+          if (k_mae != 0.f) gval += k_mae * (dj - (xat(j) - mu) * rstd);
           dF[(static_cast<size_t>(b) * gm.L + l) * gm.pd + j] = __float2bfloat16_rn(gval);
         }
       }
@@ -280,7 +291,7 @@ using namespace mdt;
 static int make_geom(PatchGeom* gm, int C, int R, int p) {
   if (C <= 0 || R <= 0 || p <= 0 || R % p) return MDT_ERR_ARG;
   gm->C = C, gm->R = R, gm->p = p, gm->G = R / p, gm->L = gm->G * gm->G, gm->pd = p * p * C;
-  return gm->pd <= kMaxPD ? MDT_OK : MDT_ERR_UNSUPPORTED;
+  return MDT_OK;
 }
 
 extern "C" {
@@ -292,8 +303,9 @@ int mdt_edm_loss(const float* F, const float* xin, const float* y, const float* 
   if (dF_bf16 && !gl) return MDT_ERR_ARG;
   PatchGeom gm;
   if (int rc = make_geom(&gm, C, R, p)) return rc;
-  edm_loss_kernel<<<B, 256, 0, S(stream)>>>(F, xin, y, sigma, mask, gl, sigma_data, mae_coef, loss, Dx,
-                                            static_cast<__nv_bfloat16*>(dF_bf16), gm);
+  auto kern = gm.pd <= kMaxPD ? edm_loss_kernel<true> : edm_loss_kernel<false>;
+  kern<<<B, 256, 0, S(stream)>>>(F, xin, y, sigma, mask, gl, sigma_data, mae_coef, loss, Dx,
+                                 static_cast<__nv_bfloat16*>(dF_bf16), gm);
   return launch_status();
 }
 
