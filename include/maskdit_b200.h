@@ -239,6 +239,8 @@ int mdt_to_uint8_nhwc(const float* img, unsigned char* out, int B, int C, int H,
  * weight-shadow refresh over flat buffers:  one pass instead of apex multi_tensor_adam + a 376-launch EMA loop.
  *   g is multiplied by grad_scale first (1/world_size after a SUM all-reduce).  ema / w_bf16 may be NULL.
  *   max_blocks > 0 caps the grid (a background launch overlapped with the backward GEMMs needs only a few CTAs).
+ *   n % 4 == 0; w, m, v, ema and an fp32 g 16-byte aligned, w_bf16 and a bf16 g 8-byte aligned (MDT_ERR_ARG otherwise):
+ *   a flat-buffer slice qualifies when it starts at a multiple of 4 elements.
  * ------------------------------------------------------------------------------------------------------------ */
 int mdt_adamw_ema(float* w, const float* g, float* m, float* v, float* ema, void* w_bf16, long long n, float lr,
                   float beta1, float beta2, float eps, float weight_decay, int step, float ema_decay,

@@ -367,6 +367,12 @@ static int adamw_launch(bool g16, float* w, const void* g, float* m, float* v, f
                         float lr, float beta1, float beta2, float eps, float weight_decay, int step, float ema_decay,
                         float grad_scale, int max_blocks, void* stream) {
   if (!w || !g || !m || !v || n <= 0 || step < 1 || (n & 3)) return MDT_ERR_ARG;
+  // the kernel moves 4 elements per access: float4 for the fp32 buffers, uint2 for the bf16 ones
+  const uintptr_t a16 = reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(m) |
+                        reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(ema) |
+                        (g16 ? 0 : reinterpret_cast<uintptr_t>(g));
+  const uintptr_t a8 = reinterpret_cast<uintptr_t>(w_bf16) | (g16 ? reinterpret_cast<uintptr_t>(g) : 0);
+  if ((a16 & 15) || (a8 & 7)) return MDT_ERR_ARG;
   const float inv_bc1 = static_cast<float>(1.0 / (1.0 - pow(static_cast<double>(beta1), step)));
   const float inv_bc2 = static_cast<float>(1.0 / (1.0 - pow(static_cast<double>(beta2), step)));
   long long blocks = (n / 4 + 255) / 256;

@@ -115,8 +115,9 @@ class TrainStep:
                       accumulation, moments and master weights stay fp32.  2-rank vs 1-GPU gradient rel-L2 2.3e-3.
                       'fp32': the 2.92 GB buffer is reduced as is (DDP's arithmetic; rel-L2 1e-5, order noise).
           overlap     the exchange of a block's gradients starts as soon as its backward is enqueued, on a side stream,
-                      through a communicator confined to `comm_ctas` CTAs while the persistent GEMM / attention grids
-                      are sized for (SMs - comm_ctas) (`mdt_set_sm_budget`).  Off by default, kept for A/B.
+                      through a communicator confined to `comm_ctas` CTAs while the persistent GEMM grids are sized
+                      for (SMs - comm_ctas) (`mdt_set_sm_budget`; the other kernels' grids are not budgeted).  Off by
+                      default, kept for A/B.
         Environment overrides: MDT_COLLECTIVE, MDT_GRAD_AR, MDT_OVERLAP, MDT_COMM_CTAS."""
         self.net, self.ema = net, ema
         self.lr, self.betas, self.eps, self.wd, self.ema_decay = lr, betas, eps, weight_decay, ema_decay

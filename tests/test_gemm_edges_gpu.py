@@ -130,6 +130,32 @@ def test_dgelu_colsum_ragged_n(ops, M, N):
     check(got, want, f"dgelu M={M} N={N}")
 
 
+@pytest.fixture
+def sm_budget(ops):
+    L = ops.lib()
+    yield L
+    assert L.mdt_set_sm_budget(0) == 0
+
+
+@pytest.mark.parametrize("budget", [1, 7, 124])
+def test_sm_budget_every_epilogue(ops, sm_budget, budget):
+    """A persistent grid narrowed by `mdt_set_sm_budget` (the backward next to the overlapped gradient exchange) deals
+    the same tiles to fewer CTAs: paired half tiles, ragged M.  A tile's arithmetic does not depend on which CTA runs
+    it, so every non-accumulating output is bit-identical to the full-width run; the accumulating epilogue's k-slice
+    count follows the budget, so it is held to the reference."""
+    M, N, K = 5 * 128 + 37, 1152, 256
+    for epi in EPIS:
+        b_mn = epi in ("dgelu", "atomic")
+        full, _ = run(ops, epi, M, N, K, seed=budget, b_mn=b_mn)
+        assert sm_budget.mdt_set_sm_budget(budget) == 0
+        got, want = run(ops, epi, M, N, K, seed=budget, b_mn=b_mn)
+        assert sm_budget.mdt_set_sm_budget(0) == 0
+        check(got, want, f"{epi} budget={budget}")
+        for k in got:
+            if epi != "atomic" and k != "colsum":    # fp32 red.add: summation order varies
+                assert torch.equal(got[k], full[k]), f"{epi} {k} differs under budget {budget}"
+
+
 @pytest.mark.parametrize("epi", [e for e in EPIS if e != "atomic"])
 def test_two_runs_bit_identical(ops, epi):
     M, N, K = 9 * 128 + 65, 3456, 1152

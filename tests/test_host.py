@@ -282,3 +282,66 @@ def test_gemm_dispatch_plan_for_the_xl2_step():
         P(0, 16, 16)
     with pytest.raises(_lib.MdtError):
         P(128, 128, 100)      # lda = 100: TMA needs 16-byte row strides
+
+
+@pytest.fixture
+def sm_budget():
+    """The library's SM budget, restored to its value before the test."""
+    from maskdit_b200 import _lib
+    L = _lib.lib()
+    before = L.mdt_get_sm_budget()
+    yield L
+    assert L.mdt_set_sm_budget(before) == 0
+
+
+def test_gemm_plan_under_sm_budget(sm_budget):
+    """`mdt_set_sm_budget(n)` sizes the persistent GEMM grid for n SMs (the overlapped gradient exchange runs on the
+    rest); a budget at or above the SM count changes nothing, a negative one is refused."""
+    from maskdit_b200 import _lib
+    L, P = sm_budget, _lib.gemm_plan
+    shapes = [((32768, 1152, 1152), {}), ((5 * 128 + 37, 1152, 256), {"epi": _lib.EPI_GATE_RESID}),
+              ((1152, 4608, 32768), {"a_mn": True, "b_mn": True, "epi": _lib.EPI_ATOMIC}), ((1024, 16, 512), {})]
+    assert L.mdt_set_sm_budget(0) == 0
+    full = [P(*s, **kw) for s, kw in shapes]
+    sms = full[0]["grid"]
+    assert full[0]["units"] > sms and full[3]["units"] == 8
+    for n in (1, 8, 124, sms, sms + 50):
+        assert L.mdt_set_sm_budget(n) == 0 and L.mdt_get_sm_budget() == n
+        for (s, kw), f in zip(shapes, full):
+            p = P(*s, **kw)
+            assert p["grid"] == min(p["units"], n, sms), (n, s, p)
+            if n >= sms:
+                assert p == f, (n, s)
+            elif kw.get("epi") != _lib.EPI_ATOMIC:
+                assert p["units"] == f["units"], (n, s)   # only the k-slice count depends on the budget
+    assert L.mdt_set_sm_budget(-1) == -1 and L.mdt_get_sm_budget() == sms + 50
+    assert L.mdt_set_sm_budget(0) == 0 and P(*shapes[0][0]) == full[0]
+
+
+@pytest.mark.skipif(torch.cuda.is_available(), reason="the aligned calls launch the kernel on dummy pointers")
+@pytest.mark.parametrize("g16", [False, True])
+def test_adamw_rejects_misaligned_buffers(g16):
+    """The AdamW kernel reads w, m, v, ema and an fp32 g as float4 and a bf16 g and w_bf16 as uint2: misaligned
+    pointers are refused with MDT_ERR_ARG.  Pointers are dummies; a call that passes the checks fails at the launch
+    (no device here, MDT_ERR_CUDA)."""
+    from maskdit_b200 import _lib
+    L = _lib.lib()
+    fn = L.mdt_adamw_ema_g16 if g16 else L.mdt_adamw_ema
+    base = dict(w=1 << 20, g=2 << 20, m=3 << 20, v=4 << 20, ema=5 << 20, w16=6 << 20)
+
+    def call(**shift):
+        p = {k: (0 if shift.get(k) is None and k in shift else base[k] + shift.get(k, 0)) for k in base}
+        return fn(p["w"], p["g"], p["m"], p["v"], p["ema"], p["w16"], 1024, 1e-3, 0.9, 0.999, 1e-8, 0.0, 1, 0.9999,
+                  1.0, 0, None)
+
+    ARG, CUDA = -1, -2
+    assert call() == CUDA
+    assert call(ema=None, w16=None) == CUDA
+    for k in ("w", "m", "v", "ema"):
+        for off in (4, 8):
+            assert call(**{k: off}) == ARG, (k, off)
+    assert call(w16=4) == ARG and call(w16=8) == CUDA and call(w16=2) == ARG
+    if g16:
+        assert call(g=2) == ARG and call(g=4) == ARG and call(g=8) == CUDA
+    else:
+        assert call(g=4) == ARG and call(g=8) == ARG and call(g=16) == CUDA

@@ -244,10 +244,11 @@ def test_xl2_config1_forward_vs_reference_golden():
     assert torch.allclose(loss.cpu(), g["loss"], rtol=LOSS_TOL)
 
 
-@pytest.mark.parametrize("overlap", [False, True])
-def test_train_step_matches_oracle_adamw_and_ema(overlap):
+@pytest.mark.parametrize("graph", [False, True])
+def test_train_step_matches_oracle_adamw_and_ema(graph):
     """Full step (loss fwd/bwd + AdamW + EMA) for 2 steps vs the CPU oracle; also deepcopy/state_dict round trip.
-    overlap=True exercises the per-block side-stream reduce+step path."""
+    graph=True replays the zero-grad + forward + backward from a CUDA graph.  (The data-parallel exchange paths are
+    tests/test_dp_step_gpu.py's.)"""
     from maskdit_b200.train_step import TrainStep
     from oracle import maskdit_oracle as O
     g = load("s2_train_mask")
@@ -255,14 +256,14 @@ def test_train_step_matches_oracle_adamw_and_ema(overlap):
     net.train()
     ema = copy.deepcopy(net).eval()
     assert set(ema.state_dict().keys()) == set(sd.keys())
-    ts = TrainStep(net, ema, lr=1e-3, loss_fn=None, overlap=overlap)
+    # one loss object for the whole run: a captured graph keeps reading the draws it was captured with
+    ts = TrainStep(net, ema, lr=1e-3, loss_fn=GoldenLoss(g), graph=graph)
     sdr = {k: v.clone().requires_grad_(not k.endswith("pos_embed")) for k, v in sd.items()}
     er = {k: v.clone() for k, v in sd.items()}
     mo = {k: torch.zeros_like(v) for k, v in sd.items()}
     vo = {k: torch.zeros_like(v) for k, v in sd.items()}
     md = O.mask_from_noise(g["mask_noise"], 0.5)
     for step in (1, 2):
-        ts.loss_fn = GoldenLoss(g)
         loss = ts.step(g["images"].cuda(), g["labels"].cuda(), 0.5, 0.1)
         lo, _ = O.edm_loss(sdr, cfg, g["images"], g["labels"], g["rnd_normal"], g["noise_unit"], md, 0.1)
         assert torch.allclose(loss.cpu(), lo.detach(), rtol=1e-2), (step, loss, lo)
