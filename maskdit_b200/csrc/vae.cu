@@ -38,8 +38,13 @@ __global__ void vae_post_quant_kernel(const float* __restrict__ z, const float* 
 
 // GroupNorm(32) statistics of x [B, P, C] f32, DETERMINISTIC (no atomics: with bf16 GEMM operands downstream, 1e-7
 // order noise in a mean flips bf16 roundings and shows up as 4e-3 run-to-run differences in the decoded image, measured):
-//   pass 1: block (b, chunk of kGnPix pixels) -> partial[b][chunk][g] = (sum, sum of squares) fp32, fixed-order tree
-//   pass 2: sums[b][g] = fixed-order fp64 sum of the partials.
+//   pass 1: block (b, chunk of kGnPix pixels) -> partial[b][chunk][g] = (sum, sum of squares) of x - K fp32,
+//           fixed-order tree
+//   pass 2: sums[b][g] = fixed-order fp64 sum of the partials, with the shift K folded back in fp64.
+// K is the group's first value (pixel 0, its first channel).  Summing x - K instead of x keeps the fp32 partials at the
+// scale of the group's spread, so a group whose mean is large against its spread does not lose its variance to
+// cancellation (the one-pass q/n - m^2 that mdt_vae_im2col forms then cancels in fp64), and an exactly constant group
+// sums to exactly zero deviation.
 // Thread = 4 channels of one pixel lane; block = C/4 x (256 / (C/4)) threads: always 8 threads per group.
 constexpr int kGnPix = 256;
 __global__ void __launch_bounds__(256)
@@ -47,15 +52,17 @@ vae_gn_partial_kernel(const float* __restrict__ x, float* __restrict__ partial, 
   __shared__ float s_part[256][2];
   const int tx = threadIdx.x, ty = threadIdx.y, b = blockIdx.y;
   const int p0 = blockIdx.x * kGnPix;
+  const int tpg = (C / 32) / 4;                       // threads per group along x (1, 2 or 4)
+  const int g = tx / tpg, member = ty * tpg + (tx - g * tpg);
+  const float k = x[static_cast<long long>(b) * P * C + g * (C / 32)];
   float s = 0.f, ss = 0.f;
   for (int p = p0 + ty; p < min(P, p0 + kGnPix); p += blockDim.y) {
-    const float4 v = *reinterpret_cast<const float4*>(x + (static_cast<long long>(b) * P + p) * C + 4 * tx);
+    float4 v = *reinterpret_cast<const float4*>(x + (static_cast<long long>(b) * P + p) * C + 4 * tx);
+    v.x -= k, v.y -= k, v.z -= k, v.w -= k;
     s += (v.x + v.y) + (v.z + v.w);
     ss += (v.x * v.x + v.y * v.y) + (v.z * v.z + v.w * v.w);
   }
   // slot = (group, member): the 8 threads of a group occupy 8 consecutive slots
-  const int tpg = (C / 32) / 4;                       // threads per group along x (1, 2 or 4)
-  const int g = tx / tpg, member = ty * tpg + (tx - g * tpg);
   s_part[g * 8 + member][0] = s;
   s_part[g * 8 + member][1] = ss;
   __syncthreads();
@@ -68,11 +75,19 @@ vae_gn_partial_kernel(const float* __restrict__ x, float* __restrict__ partial, 
     partial[((static_cast<long long>(b) * gridDim.x + blockIdx.x) * 32 + gg) * 2 + w] = acc;
   }
 }
-__global__ void vae_gn_finish_kernel(const float* __restrict__ partial, double* __restrict__ sums, int nchunk) {
-  const int b = blockIdx.x, t = threadIdx.x;  // 64 threads: (group, which)
-  double acc = 0.0;
-  for (int k = 0; k < nchunk; ++k) acc += static_cast<double>(partial[(static_cast<long long>(b) * nchunk + k) * 64 + t]);
-  sums[static_cast<long long>(b) * 64 + t] = acc;
+__global__ void vae_gn_finish_kernel(const float* __restrict__ x, const float* __restrict__ partial,
+                                     double* __restrict__ sums, int nchunk, int P, int C) {
+  const int b = blockIdx.x, g = threadIdx.x;  // 32 threads: one group each
+  double s = 0.0, q = 0.0;
+  for (int k = 0; k < nchunk; ++k) {
+    const float2 v = *reinterpret_cast<const float2*>(partial + (static_cast<long long>(b) * nchunk + k) * 64 + 2 * g);
+    s += static_cast<double>(v.x);
+    q += static_cast<double>(v.y);
+  }
+  const double K = x[static_cast<long long>(b) * P * C + g * (C / 32)];
+  const double n = static_cast<double>(P) * (C / 32);
+  sums[(static_cast<long long>(b) * 32 + g) * 2] = fma(n, K, s);                 // sum x   = nK + S
+  sums[(static_cast<long long>(b) * 32 + g) * 2 + 1] = fma(K, fma(n, K, 2.0 * s), q);  // sum x^2 = K(nK + 2S) + Q
 }
 
 // im2col with the producer fused in:
@@ -99,18 +114,25 @@ vae_im2col_kernel(const float* __restrict__ src, const double* __restrict__ sums
   }
   const int cg = C / 32 > 0 ? C / 32 : 1;
   const double cnt = static_cast<double>(Hs) * Ws * cg;
+  // GroupNorm of this thread's group in the current image, recomputed only when the image changes.
+  // mean = mean_hi + mean_lo: x - mean_hi is exact for x near a large mean, so normalising a group whose mean is
+  // large against its spread keeps the fp32 accuracy of x - mean.  The one-pass variance may round below zero
+  // (a constant group): it is clamped before eps.
+  float mean_hi = 0.f, mean_lo = 0.f, rstd = 1.f;
+  int stats_b = -1;
   for (long long pix = blockIdx.x * static_cast<long long>(blockDim.y) + threadIdx.y; pix < npix;
        pix += static_cast<long long>(gridDim.x) * blockDim.y) {
     const int b = static_cast<int>(pix / (static_cast<long long>(H) * W));
     const int yx = static_cast<int>(pix - static_cast<long long>(b) * H * W);
     const int y = yx / W, x = yx - y * W;
-    float mean = 0.f, rstd = 1.f;
-    if (sums) {
+    if (sums && b != stats_b) {
       const int g = c / cg;
       const double s = sums[(static_cast<long long>(b) * 32 + g) * 2], q = sums[(static_cast<long long>(b) * 32 + g) * 2 + 1];
       const double m = s / cnt;
-      mean = static_cast<float>(m);
-      rstd = rsqrtf(static_cast<float>(q / cnt - m * m) + eps);
+      mean_hi = static_cast<float>(m);
+      mean_lo = static_cast<float>(m - static_cast<double>(mean_hi));
+      rstd = rsqrtf(fmaxf(static_cast<float>(q / cnt - m * m), 0.f) + eps);
+      stats_b = b;
     }
     __nv_bfloat16* arow = A + pix * Kp;
     for (int t = 0; t < taps; ++t) {
@@ -122,8 +144,10 @@ vae_im2col_kernel(const float* __restrict__ src, const double* __restrict__ sums
             src + ((static_cast<long long>(b) * Hs + sy / up) * Ws + sx / up) * C + c);
         float4 r = v;
         if (sums) {
-          r.x = fmaf((v.x - mean) * rstd, ga.x, be.x), r.y = fmaf((v.y - mean) * rstd, ga.y, be.y);
-          r.z = fmaf((v.z - mean) * rstd, ga.z, be.z), r.w = fmaf((v.w - mean) * rstd, ga.w, be.w);
+          r.x = fmaf(((v.x - mean_hi) - mean_lo) * rstd, ga.x, be.x);
+          r.y = fmaf(((v.y - mean_hi) - mean_lo) * rstd, ga.y, be.y);
+          r.z = fmaf(((v.z - mean_hi) - mean_lo) * rstd, ga.z, be.z);
+          r.w = fmaf(((v.w - mean_hi) - mean_lo) * rstd, ga.w, be.w);
         }
         if (silu_on) r = make_float4(silu(r.x), silu(r.y), silu(r.z), silu(r.w));
         o = make_uint2(pack_bf16(r.x, r.y), pack_bf16(r.z, r.w));
@@ -221,7 +245,7 @@ int mdt_vae_gn_stats(const float* x, double* sums, float* scratch, int B, int P,
   const int nchunk = (P + kGnPix - 1) / kGnPix;
   dim3 block(C / 4, 256 / (C / 4)), grid(nchunk, B);
   vae_gn_partial_kernel<<<grid, block, 0, VS(stream)>>>(x, scratch, P, C);
-  vae_gn_finish_kernel<<<B, 64, 0, VS(stream)>>>(scratch, sums, nchunk);
+  vae_gn_finish_kernel<<<B, 32, 0, VS(stream)>>>(x, scratch, sums, nchunk, P, C);
   return vae_status();
 }
 
