@@ -362,20 +362,72 @@ def batches(dataset, batch, rank=0, world=1, start=0, pin=True):
 
 
 # ---- WebDataset shards (lmdb2wds.py:26, train_wds.py:58-64) ------------------------------------------------------------
+class WdsShardWriter:
+    """Stream samples into the tar shards `pattern % 0`, `pattern % 1`, ... in the layout lmdb2wds.py writes:
+    `<key>.latent` = pickle of the [2C,R,R] float32 array, `<key>.cls` = the class index as ASCII (webdataset's default
+    encoding of an int).  A shard holds at most `maxcount` samples and at most `maxsize` payload bytes (the member
+    contents, as `webdataset.ShardWriter` counts them): a sample that would push the current shard past `maxsize` starts
+    the next one, and a sample larger than `maxsize` gets a shard of its own.  The first shard is opened at once, so no
+    samples give one empty shard, as with webdataset.  Only the open shard's tar stream is held, so any number of samples
+    can be written.  `paths` lists the shards written so far; a run that raises removes the unfinished shard."""
+
+    def __init__(self, pattern, maxcount=100000, maxsize=3e9):
+        if maxcount < 1 or maxsize <= 0:
+            raise ValueError(f"maxcount ({maxcount}) and maxsize ({maxsize}) must be positive")
+        self.pattern, self.maxcount, self.maxsize = pattern, maxcount, maxsize
+        self.paths, self._tar = [], None
+        self._next_shard()
+
+    def _next_shard(self):
+        import tarfile
+        self.close()
+        self.paths.append(self.pattern % len(self.paths))
+        self._tar = tarfile.open(self.paths[-1], "w")
+        self._count = self._size = 0
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, exc_type, *exc):
+        if self._tar is None:
+            return
+        if exc_type is None:
+            self.close()
+        else:
+            self._tar.close()
+            self._tar = None
+            os.remove(self.paths.pop())
+
+    def write(self, key, moments, label):
+        import io
+        import pickle
+        import tarfile
+        if self._tar is None:
+            raise ValueError("write to a closed WdsShardWriter")
+        members = (("latent", pickle.dumps(np.ascontiguousarray(moments, dtype=np.float32))),
+                   ("cls", str(int(label)).encode()))
+        size = sum(len(p) for _, p in members)
+        if self._count >= self.maxcount or (self._count and self._size + size > self.maxsize):
+            self._next_shard()
+        for ext, payload in members:
+            ti = tarfile.TarInfo(f"{key}.{ext}")
+            ti.size = len(payload)
+            self._tar.addfile(ti, io.BytesIO(payload))
+        self._count += 1
+        self._size += size
+
+    def close(self):
+        if self._tar is not None:
+            self._tar.close()
+            self._tar = None
+
+
 def write_wds_shard(path, moments, labels, start=0):
-    """One tar shard in the layout lmdb2wds.py writes: `<key>.latent` = pickle of the [2C,R,R] float32 array,
-    `<key>.cls` = the class index as ASCII (webdataset's default encoding of an int)."""
-    import io
-    import pickle
-    import tarfile
-    with tarfile.open(path, "w") as tf:
+    """One tar shard holding every sample, keys `{start + i:07d}` (`WdsShardWriter`'s layout)."""
+    pattern = "%.0s" + path.replace("%", "%%")          # the shard number formats to nothing: the shard is `path`
+    with WdsShardWriter(pattern, maxcount=float("inf"), maxsize=float("inf")) as w:
         for i, (z, y) in enumerate(zip(moments, labels)):
-            key = f"{start + i:07d}"
-            for ext, payload in (("latent", pickle.dumps(np.ascontiguousarray(z, dtype=np.float32))),
-                                 ("cls", str(int(y)).encode())):
-                ti = tarfile.TarInfo(f"{key}.{ext}")
-                ti.size = len(payload)
-                tf.addfile(ti, io.BytesIO(payload))
+            w.write(f"{start + i:07d}", z, y)
 
 
 def wds_samples(shards, rank=0, world=1, num_classes=1000):
