@@ -6,16 +6,16 @@
 // backward, issued from C++ on the caller's stream: ~280 launches forward, ~500 backward, no allocation (every
 // activation is a fixed slice of the workspace, planned once per (B, T, mode)), no Python between launches.  The
 // reference gets this sequencing from autograd + torch.compile (train.py:179,216-220); the per-kernel entry points
-// it is built from stay exported (the parity tests drive them one by one; `maskdit_b200/engine.py` issues the same
-// sequence from Python and must agree bit for bit in the forward).
+// it is built from stay exported (the parity tests drive them one by one; the tests' reference `maskdit_b200/engine.py::
+// Engine` issues the same sequence from Python and must agree bit for bit in the forward).
 //
 // Packed parameter blob (fp32 master `w32`, bf16 shadow `w16`, fp32 gradient `grad`: same element offsets):
 //   [adaLN_modulation.1.weight of blocks 0..depth-1, decoder_layer, decoder_blocks 0..dec_depth-1, final_layer]
 //   [the matching adaLN biases] [every other trainable tensor in registration order] [pos_embed, decoder_pos_embed]
 // each tensor starting on a 64-element boundary.  The decoder-less DiT (use_decoder=False, models/maskdit.py:254,
 // 308-331: all four dec_* fields 0) has no decoder_layer, decoder blocks, decoder_pos_embed or mask token, and its
-// final layer reads the encoder width - `mdt_model_param_info` enumerates it, `maskdit_b200/flat.py`
-// builds exactly this layout for the nn.Module (tests/test_host.py compares the two).
+// final layer reads the encoder width.  `build_layout` is the only place these offsets are decided:
+// `mdt_model_param_info` enumerates them and `maskdit_b200/flat.py` lays the nn.Module's parameters out from it.
 #include <dlfcn.h>
 #include <string.h>
 

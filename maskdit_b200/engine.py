@@ -14,6 +14,8 @@ fp32; GEMM operands are bf16 with fp32 accumulation in registers.  Nothing here 
 """
 from __future__ import annotations
 
+import ctypes
+
 import torch
 
 from . import ops
@@ -31,27 +33,20 @@ class BlockSpec:
 class Engine:
     def __init__(self, cfg, store):
         self.cfg, self.store = cfg, store
-        D, Dd = cfg.hidden, cfg.dec_hidden
         # dec_hidden == 0: the decoder-less DiT (use_decoder=False), final layer on the encoder width
-        self.has_dec = Dd > 0
-        off = 0
-        self.enc = []
-        for i in range(cfg.depth):
-            self.enc.append(BlockSpec(f"model.blocks.{i}", D, cfg.heads, off))
-            off += 6 * D
-        self.off_declayer = None
-        self.dec = []
-        if self.has_dec:
-            self.off_declayer = off
-            off += 2 * D
-            for i in range(cfg.dec_depth):
-                self.dec.append(BlockSpec(f"model.decoder_blocks.{i}", Dd, cfg.dec_heads, off))
-                off += 6 * Dd
-        self.Df = Dd if self.has_dec else D
-        self.off_final = off
-        off += 2 * self.Df
-        self.NA = off
-        assert store.ada_w_range[1] == self.NA, (store.ada_w_range, self.NA)
+        self.has_dec = cfg.dec_hidden > 0
+        o0, self.NA, hidden = store.ada_w_range
+
+        def mod_off(prefix):
+            """Column of the head's modulation vector: the first row of its adaLN weight in the [NA, hidden] matrix."""
+            return (store.offsets[f"{prefix}.adaLN_modulation.1.weight"][0] - o0) // hidden
+
+        self.enc = [BlockSpec(p, cfg.hidden, cfg.heads, mod_off(p))
+                    for p in (f"model.blocks.{i}" for i in range(cfg.depth))]
+        self.dec = [BlockSpec(p, cfg.dec_hidden, cfg.dec_heads, mod_off(p))
+                    for p in (f"model.decoder_blocks.{i}" for i in range(cfg.dec_depth))]
+        self.off_declayer = mod_off("model.decoder_layer") if self.has_dec else None
+        self.off_final = mod_off("model.final_layer")
 
     # ------------------------------------------------------------------------------------------------------
     def w16(self, key):
@@ -350,42 +345,41 @@ class CEngine:
     C-ABI call each over the packed parameter blob and one workspace buffer, instead of ~780 ctypes calls and a
     `torch.empty` per activation (70 ms of host time per step in round 1, which bound the 128-samples-per-GPU config).
     `Engine` above issues the identical launch sequence kernel by kernel and is kept as the cross-check
-    (tests/test_model_gpu_extra.py::test_c_driver_matches_python_engine); MDT_ENGINE=py selects it."""
+    (tests/test_model_gpu.py::check_c_driver_matches_engine).
 
-    def __init__(self, cfg, store):
-        import ctypes
-        self.cfg, self.store = cfg, store
+    The C model handle it creates from the network's config is the one place the packed parameter layout is decided:
+    the `FlatStore` of the module is built from it (`tensors`, `param_count`, `NA`) and assigned to `store`."""
+
+    def __init__(self, cfg):
+        self.cfg, self.store = cfg, None
         L = ops.lib()
-        has_tok = "model.mask_token" in store.offsets
-        h4e = store.offsets["model.blocks.0.mlp.fc1.weight"][2][0] if cfg.depth else 4 * cfg.hidden
-        h4d = store.offsets["model.decoder_blocks.0.mlp.fc1.weight"][2][0] if cfg.dec_depth else 4 * cfg.dec_hidden
-        R = int(round(cfg.num_patches ** 0.5)) * cfg.patch
-        mc = ops.L.ModelCfg(R, cfg.img_channels, cfg.patch, cfg.num_classes, cfg.hidden, cfg.depth, cfg.heads, h4e,
-                            cfg.dec_hidden, cfg.dec_depth, cfg.dec_heads, h4d, int(has_tok), cfg.sigma_data)
+        mc = ops.L.ModelCfg(cfg.img_resolution, cfg.img_channels, cfg.patch, cfg.num_classes, cfg.hidden, cfg.depth,
+                            cfg.heads, cfg.mlp_hidden, cfg.dec_hidden, cfg.dec_depth, cfg.dec_heads, cfg.dec_mlp_hidden,
+                            int(cfg.has_mask_token), cfg.sigma_data)
         h = ctypes.c_void_p()
         ops.check(L.mdt_model_create(ctypes.byref(mc), ctypes.byref(h)), "mdt_model_create", 0)
         self._h, self._L = h, L
-        # the C driver's packed layout must be the store's: compare every tensor once
-        n = L.mdt_model_num_tensors(h)
-        if n != len(store.offsets):
-            raise ops.L.MdtError(f"driver layout has {n} tensors, the module {len(store.offsets)}")
-        name = ctypes.create_string_buffer(160)
-        off, num = ctypes.c_longlong(), ctypes.c_longlong()
-        for i in range(n):
-            L.mdt_model_param_info(h, i, name, 160, ctypes.byref(off), ctypes.byref(num))
-            k = name.value.decode()
-            if k not in store.offsets or store.offsets[k][:2] != (off.value, num.value):
-                raise ops.L.MdtError(f"driver layout mismatch at {k}: {store.offsets.get(k)} vs {(off.value, num.value)}")
-        if L.mdt_model_param_count(h, 1) != store.n_train or L.mdt_model_param_count(h, 0) != store.n_total:
-            raise ops.L.MdtError("driver blob length differs from the flat store")
-        self.NA = L.mdt_model_mod_width(h)
-        self.launches = {}
+        self.NA = L.mdt_model_mod_width(h)   # width of the modulation vector = rows of the adaLN weight matrix
 
     def __del__(self):
         try:
             self._L.mdt_model_destroy(self._h)
         except Exception:
             pass
+
+    def tensors(self):
+        """{name: (offset, numel)} of every packed tensor, in blob order (`mdt_model_param_info`)."""
+        name, off, num = ctypes.create_string_buffer(160), ctypes.c_longlong(), ctypes.c_longlong()
+        out = {}
+        for i in range(self._L.mdt_model_num_tensors(self._h)):
+            ops.check(self._L.mdt_model_param_info(self._h, i, name, 160, ctypes.byref(off), ctypes.byref(num)),
+                      "mdt_model_param_info", 0)
+            out[name.value.decode()] = (off.value, num.value)
+        return out
+
+    def param_count(self, trainable_only):
+        """Elements of the trainable region, or of the whole blob (`mdt_model_param_count`)."""
+        return self._L.mdt_model_param_count(self._h, int(trainable_only))
 
     def workspace_bytes(self, B, T, training):
         n = self._L.mdt_workspace_bytes(self._h, B, T, int(training))
@@ -438,9 +432,3 @@ class CEngine:
                                        ops.ptr(dF16), ctx["B"], ctx["T"], ops.ptr(ctx["ws"]), ctx["nbytes"], cb, None,
                                        ops.stream_ptr()), "mdt_backward",
                   self._count(ctx["ids_restore"] is not None)[1])
-
-
-def make_engine(cfg, store):
-    """MDT_ENGINE=py: kernel-by-kernel launches from Python (`Engine`); default: the C++ step driver (`CEngine`)."""
-    import os
-    return Engine(cfg, store) if os.environ.get("MDT_ENGINE", "c") == "py" else CEngine(cfg, store)

@@ -8,93 +8,51 @@ behave exactly as for the reference module (SURVEY.md §8b) while the engine get
   * a bf16 shadow with identical offsets for the tensor-core GEMMs;
   * all 38 adaLN projection matrices contiguous, so the modulation of every block is ONE GEMM per step
     (the conditioning vector c is shared by all blocks: models/maskdit.py:505-506,547-548).
+The layout is the C step driver's (csrc/driver.cu `build_layout`): the store reads it from the driver's model handle.
 """
 from __future__ import annotations
 
+import math
+
 import torch
 
-ALIGN = 64  # elements (256 B fp32 / 128 B bf16): keeps every tensor TMA- and float4-aligned
+from ._lib import MdtError
+
+ALIGN = 64  # elements (256 B fp32 / 128 B bf16): the driver starts every tensor on this boundary
 
 
 def _round_up(n, a=ALIGN):
     return (n + a - 1) // a * a
 
 
-def layout_order(keys):
-    """Trainable layout: adaLN weights (encoder blocks, decoder_layer, decoder blocks, final) contiguous, then
-    the matching biases contiguous, then everything else in registration order; frozen tensors last."""
-    def ada_rank(k):
-        parts = k.split(".")
-        if "blocks" == parts[1]:
-            return (0, int(parts[2]))
-        if parts[1] == "decoder_layer":
-            return (1, 0)
-        if parts[1] == "decoder_blocks":
-            return (2, int(parts[2]))
-        return (3, 0)  # final_layer
-
-    ada_w = sorted([k for k in keys if "adaLN_modulation" in k and k.endswith("weight")], key=ada_rank)
-    ada_b = sorted([k for k in keys if "adaLN_modulation" in k and k.endswith("bias")], key=ada_rank)
-    frozen = [k for k in keys if k.endswith("pos_embed")]
-    rest = [k for k in keys if k not in ada_w and k not in ada_b and k not in frozen]
-    return ada_w, ada_b, rest, frozen
-
-
 class FlatStore:
     """Owns the flat buffers of one module.  `attach(named_params)` (re)builds them on the params' device."""
 
-    def __init__(self):
+    def __init__(self, model, named_shapes):
+        """`model`: the `CEngine` whose C model handle lays out the blob; `named_shapes`: the module's parameter
+        shapes, whose names and element counts must be the handle's tensors."""
+        layout = model.tensors()
+        for k in sorted(set(layout) ^ set(named_shapes)):
+            where = "the driver's layout" if k in layout else "the module"
+            raise MdtError(f"parameter {k} is only in {where}")
+        self.offsets = {}      # key -> (offset, numel, shape), in blob order
+        for k, (o, n) in layout.items():
+            shp = tuple(named_shapes[k])
+            if math.prod(shp) != n:
+                raise MdtError(f"parameter {k}: the module's shape {shp} does not hold the driver's {n} elements")
+            self.offsets[k] = (o, n, shp)
+        self.n_train = model.param_count(trainable_only=True)   # elements in the trainable region
+        self.n_total = model.param_count(trainable_only=False)
+        # the adaLN projections lead the blob: all weights as one [NA, hidden] matrix, then all biases
+        w0 = next(v for k, v in self.offsets.items() if "adaLN_modulation" in k and k.endswith("weight"))
+        b0 = next(v for k, v in self.offsets.items() if "adaLN_modulation" in k and k.endswith("bias"))
+        self.ada_w_range = (w0[0], model.NA, w0[2][1])   # (offset, rows, hidden)
+        self.ada_b_range = (b0[0], model.NA)
         self.device = None
-        self.offsets = {}      # key -> (offset, numel, shape)
-        self.n_train = 0       # elements in the trainable region (multiple of ALIGN)
-        self.n_total = 0
         self.w32 = None
         self.w16 = None
         self.grad = None
-        self.ada_w_range = None  # (offset, rows) of the concatenated adaLN weight [rows, hidden]
-        self.ada_b_range = None
         self._versions = None
-        self._ptr0 = None
-
-    # -- layout ------------------------------------------------------------------------------------------------
-    def plan(self, named_shapes):
-        keys = list(named_shapes.keys())
-        ada_w, ada_b, rest, frozen = layout_order(keys)
-        off = 0
-        self.offsets = {}
-        for group in (ada_w, ada_b, rest):
-            for k in group:
-                n = 1
-                for s in named_shapes[k]:
-                    n *= s
-                self.offsets[k] = (off, n, tuple(named_shapes[k]))
-                off += _round_up(n)
-        self.n_train = off
-        for k in frozen:
-            n = 1
-            for s in named_shapes[k]:
-                n *= s
-            self.offsets[k] = (off, n, tuple(named_shapes[k]))
-            off += _round_up(n)
-        self.n_total = off
-        if ada_w:
-            o0 = self.offsets[ada_w[0]][0]
-            rows, cur = 0, o0
-            hidden = named_shapes[ada_w[0]][1]
-            for k in ada_w:
-                o, n, shp = self.offsets[k]
-                assert o == cur and shp[1] == hidden, "adaLN weights must be contiguous"
-                rows += shp[0]
-                cur += n  # n is a multiple of ALIGN for every registry model (6*D*D etc.)
-                assert n % ALIGN == 0
-            self.ada_w_range = (o0, rows, hidden)
-            b0 = self.offsets[ada_b[0]][0]
-            cur = b0
-            for k in ada_b:
-                o, n, _ = self.offsets[k]
-                assert o == cur and n % ALIGN == 0, "adaLN biases must be contiguous"
-                cur += n
-            self.ada_b_range = (b0, rows)
 
     # -- storage -----------------------------------------------------------------------------------------------
     def is_attached(self, params: dict) -> bool:

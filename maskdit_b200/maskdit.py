@@ -26,7 +26,7 @@ import torch
 import torch.nn as nn
 
 from . import ops
-from .engine import Engine, make_engine  # noqa: F401
+from .engine import CEngine
 from .flat import FlatStore
 
 # (depth, hidden, heads) — models/maskdit.py:649-706
@@ -195,12 +195,25 @@ class EDMPrecond(nn.Module):
         c, m = _Cfg(), self.model
         c.hidden, c.depth, c.heads, c.patch = m.hidden_size, m.depth, m.num_heads, m.patch_size
         c.dec_hidden, c.dec_depth, c.dec_heads = m.decoder_hidden_size, m.decoder_depth, m.decoder_num_heads
+        # MLP widths as DiT.__init__ sizes fc1 (0 without a decoder)
+        c.mlp_hidden, c.dec_mlp_hidden = int(m.hidden_size * m.mlp_ratio), int(m.decoder_hidden_size * m.mlp_ratio)
+        c.has_mask_token = m.mask_token is not None
         c.num_patches, c.num_classes, c.sigma_data = m.num_patches, self.num_classes, self.sigma_data
-        c.img_channels, c.patch_dim = self.img_channels, m.patch_size * m.patch_size * m.out_channels
+        c.img_resolution, c.img_channels = self.img_resolution, self.img_channels
+        c.patch_dim = m.patch_size * m.patch_size * m.out_channels
         return c
 
     def _params(self):
         return dict(self.named_parameters())
+
+    def _layout(self):
+        """The step driver (its C model handle) and the flat store it lays out.  Both depend only on the config, so
+        they are built once, without a device."""
+        if self._engine is None:
+            self._engine = CEngine(self._cfg())
+            self._store = self._engine.store = FlatStore(self._engine,
+                                                         {k: tuple(p.shape) for k, p in self.named_parameters()})
+        return self._engine, self._store
 
     def _ready(self, device):
         """Flatten parameters on `device` (once / after .to()) and refresh the bf16 weight shadow when any
@@ -208,13 +221,9 @@ class EDMPrecond(nn.Module):
         if device.type != "cuda":
             raise ops.L.MdtError("maskdit_b200 runs on CUDA (sm_90a) only — there is no CPU fallback")
         params = self._params()
-        if self._store is None:
-            self._store = FlatStore()
-            self._store.plan({k: tuple(p.shape) for k, p in params.items()})
-        st = self._store
+        _, st = self._layout()
         if not st.is_attached(params) or st.device != device:
             st.attach(params, device)
-            self._engine = make_engine(self._cfg(), st)
             self._anchor = torch.zeros(1, device=device, requires_grad=True)
             self._graphs = {}
         if st.shadow_stale(params):

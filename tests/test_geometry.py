@@ -1,7 +1,6 @@
 """CPU tests of the DiT_models geometries beyond the shipped XL/2 (patch 4 and 8, DiT-B / L / H): the CPU fp32 oracle
 against the unmodified reference's goldens of tests/golden/make_golden_geometry.py, which pins those goldens, and the C
 driver's model config, packed layout and workspace plan for all 15 names with and without the decoder."""
-import ctypes
 import os
 import sys
 
@@ -102,48 +101,67 @@ def test_h2_bf16_autocast_yardstick_is_recorded():
 
 # ---- C driver: every model name, with and without the decoder ---------------------------------------------------------
 MODELS = [f"DiT-{a}/{p}" for a in ("H", "XL", "L", "B", "S") for p in (2, 4, 8)]
+# (model, latent resolution, classes): every name at 32x32 with 1000 classes, then 8x8 and 16x16 with class counts
+# that are not multiples of 8, and XL/2 at 64x64 (512 px)
+GEOMS = [(mt, 32, 1000) for mt in MODELS] + [("DiT-S/2", 8, 10), ("DiT-B/4", 16, 7), ("DiT-XL/2", 64, 1000)]
 
 
 @pytest.mark.parametrize("use_decoder", [True, False])
-@pytest.mark.parametrize("mt", MODELS)
-def test_model_create_layout_and_workspace_every_model(mt, use_decoder):
-    """`mdt_model_create` accepts the model; its packed tensors are FlatStore's layout in the reference's order; the
-    modulation width is the Python engine's; the workspace plan grows with the batch and training needs more than
-    eval."""
-    from maskdit_b200 import _lib
+@pytest.mark.parametrize("mt,R,ncls", GEOMS)
+def test_packed_layout_rules_and_workspace(mt, R, ncls, use_decoder):
+    """`mdt_model_create` accepts the model, and the packed layout FlatStore reads from its handle follows the blob's
+    rules against the nn.Module: the module's tensors; adaLN weights contiguous in head order, then their biases in
+    the same order, then the other trainable tensors in registration order, then the frozen pos-embeds; 64-element
+    aligned, increasing, disjoint.  Each head's modulation column is the Python engine's; the workspace plan grows
+    with the batch and the token count, training needs more than eval, and B = 0 is refused."""
+    from maskdit_b200._lib import MdtError
     from maskdit_b200.engine import Engine
-    from maskdit_b200.flat import FlatStore
     from maskdit_b200.maskdit import Precond_models
-    R = 32
-    c = cfg(mt, R, 1000, use_decoder)
+    c = cfg(mt, R, ncls, use_decoder)
     with torch.device("meta"):
-        net = Precond_models["edm"](R, 4, num_classes=1000, model_type=mt, use_decoder=use_decoder, mae_loss_coef=0.1)
-    shapes = {k: tuple(p.shape) for k, p in net.named_parameters()}
-    want = O.param_shapes(c)
-    assert shapes == {k: tuple(v) for k, v in want.items()}
-    assert any("decoder_blocks" in k for k in shapes) == use_decoder
-    st = FlatStore()
-    st.plan(shapes)
+        net = Precond_models["edm"](R, 4, num_classes=ncls, model_type=mt, use_decoder=use_decoder, mae_loss_coef=0.1)
+    named = dict(net.named_parameters())
+    assert {k: tuple(p.shape) for k, p in named.items()} == {k: tuple(v) for k, v in O.param_shapes(c).items()}
+    assert any("decoder_blocks" in k for k in named) == use_decoder
+    ce, st = net._layout()
+    assert {k: v[1:] for k, v in st.offsets.items()} == {k: (p.numel(), tuple(p.shape)) for k, p in named.items()}
+    D, Dd, dec_depth = (c.hidden, c.dec_hidden, c.dec_depth) if use_decoder else (c.hidden, 0, 0)
+    heads = [f"model.blocks.{i}" for i in range(c.depth)]
+    if use_decoder:
+        heads += ["model.decoder_layer"] + [f"model.decoder_blocks.{i}" for i in range(dec_depth)]
+    heads.append("model.final_layer")
+    ada_w = [f"{h}.adaLN_modulation.1.weight" for h in heads]
+    ada_b = [f"{h}.adaLN_modulation.1.bias" for h in heads]
+    rest = [k for k, p in named.items() if p.requires_grad and "adaLN_modulation" not in k]
+    frozen = [k for k, p in named.items() if not p.requires_grad]
+    assert frozen == ["model.pos_embed", "model.decoder_pos_embed"][:1 + use_decoder]
+    assert list(st.offsets) == ada_w + ada_b + rest + frozen
+    spans = list(st.offsets.values())
+    assert spans[0][0] == 0 and all(o % 64 == 0 for o, _, _ in spans)
+    assert all(o + n <= o2 for (o, n, _), (o2, _, _) in zip(spans, spans[1:]))
+    assert st.offsets[rest[-1]][0] + st.offsets[rest[-1]][1] <= st.n_train <= st.offsets[frozen[0]][0]
+    assert st.offsets[frozen[-1]][0] + st.offsets[frozen[-1]][1] <= st.n_total
+    if (mt, use_decoder, ncls) == ("DiT-XL/2", True, 1000):
+        assert sum(p.numel() for p in named.values() if p.requires_grad) == 730_115_216 <= st.n_train
+    # adaLN: ONE [NA, D] weight matrix, then ONE [NA] bias vector; a head's modulation column is its first row
+    off_declayer = 6 * D * c.depth
+    off_final = off_declayer + (2 * D + 6 * Dd * dec_depth if use_decoder else 0)
+    NA = off_final + 2 * (Dd or D)
+    for keys, width in ((ada_w, D), (ada_b, 1)):
+        cur = st.offsets[keys[0]][0]
+        for k in keys:
+            assert st.offsets[k][0] == cur, k
+            cur += st.offsets[k][1]
+        assert cur - st.offsets[keys[0]][0] == NA * width
+    assert st.ada_w_range == (0, NA, D) and st.ada_b_range == (NA * D, NA) and ce.NA == NA
     eng = Engine(net._cfg(), st)
-    D = c.hidden
-    dec = (c.dec_hidden, c.dec_depth, c.dec_heads, 4 * c.dec_hidden, 1) if use_decoder else (0, 0, 0, 0, 0)
-    L = _lib.lib()
-    mc = _lib.ModelCfg(R, 4, c.patch, 1000, D, c.depth, c.heads, 4 * D, *dec, 0.5)
-    h = ctypes.c_void_p()
-    assert L.mdt_model_create(ctypes.byref(mc), ctypes.byref(h)) == 0
-    try:
-        n = L.mdt_model_num_tensors(h)
-        assert n == len(shapes)
-        name, off, num = ctypes.create_string_buffer(160), ctypes.c_longlong(), ctypes.c_longlong()
-        for i in range(n):
-            assert L.mdt_model_param_info(h, i, name, 160, ctypes.byref(off), ctypes.byref(num)) == 0
-            k = name.value.decode()
-            assert st.offsets[k][:2] == (off.value, num.value), k
-        assert (L.mdt_model_param_count(h, 1), L.mdt_model_param_count(h, 0)) == (st.n_train, st.n_total)
-        assert L.mdt_model_mod_width(h) == eng.NA == st.ada_w_range[1]
-        T = c.num_patches // 2
-        tr, ev = L.mdt_workspace_bytes(h, 8, T, 1), L.mdt_workspace_bytes(h, 8, 0, 0)
-        assert tr > ev > 0 and L.mdt_workspace_bytes(h, 16, T, 1) > tr
-        assert L.mdt_workspace_bytes(h, 8, c.num_patches, 1) > tr
-    finally:
-        L.mdt_model_destroy(h)
+    assert (eng.NA, eng.off_final, eng.off_declayer) == (NA, off_final, off_declayer if use_decoder else None)
+    assert [s.mod_off for s in eng.enc] == [6 * D * i for i in range(c.depth)]
+    assert [s.mod_off for s in eng.dec] == [off_declayer + 2 * D + 6 * Dd * i for i in range(dec_depth)]
+    assert ce._L.mdt_model_param_info(ce._h, len(st.offsets), None, 0, None, None) != 0
+    T = c.num_patches // 2
+    tr, ev = ce.workspace_bytes(8, T, True), ce.workspace_bytes(8, 0, False)
+    assert tr > ev > 0 and ce.workspace_bytes(16, T, True) > tr
+    assert ce.workspace_bytes(8, c.num_patches, True) > tr
+    with pytest.raises(MdtError):
+        ce.workspace_bytes(0, T, True)

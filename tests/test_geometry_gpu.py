@@ -15,8 +15,8 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, ROOT)
-from test_model_gpu import (CFG_TOL, EVAL_TOL, FWD_TOL, LOSS_TOL, GoldenLoss, ImplRecorder, check_grads, load,  # noqa: E402
-                            rel_l2)
+from test_model_gpu import (CFG_TOL, EVAL_TOL, FWD_TOL, LOSS_TOL, GoldenLoss, ImplRecorder,  # noqa: E402
+                            check_c_driver_matches_engine, check_grads, load, rel_l2)
 
 pytestmark = pytest.mark.gpu
 
@@ -81,46 +81,20 @@ def test_loss_D_and_grads_vs_reference_golden(name):
 
 @pytest.mark.parametrize("name", ["geo_s8_mask50", "geo_l4_nd_uncond_mask30"])
 def test_c_driver_matches_python_engine(name):
-    """`mdt_forward` == `Engine.forward` bit for bit; backward within the fp32-atomics order noise (the bounds of
-    test_model_gpu_extra.py::test_c_driver_matches_python_engine).  Decoder-less with a mask: the removed tokens'
-    rows of F are exactly zero."""
-    from maskdit_b200.engine import CEngine, Engine
+    """`mdt_forward` == `Engine.forward` bit for bit; backward within the fp32-atomics order noise
+    (test_model_gpu.py::check_c_driver_matches_engine).  Decoder-less with a mask: the removed tokens' rows of F are
+    exactly zero."""
     (mt, R, ncls, dec), _, _ = CASES[name]
     g = load(name)
     net, cfg = build_geo(mt, R, ncls, dec)
     net.train()
-    st = net.prepare()
-    assert isinstance(net._engine, CEngine)
     sigma, x, lab, md = inputs(g)
     sigma, x = sigma.reshape(-1).contiguous(), x.contiguous()
-    ce, pe = net._engine, Engine(net._cfg(), st)
-    for save in (False, True):
-        Fc, ctx_c = ce.forward(x, sigma, lab, md, save)
-        Fp, ctx_p = pe.forward(x, sigma, lab, md, save)
-        assert torch.equal(Fc, Fp), (save, (Fc - Fp).abs().max())
+    _, _, Fc = check_c_driver_matches_engine(net, x, sigma, lab, md, name)
     assert Fc.shape[-1] == cfg.patch_dim
     if not dec:
         removed = md["mask"].bool().reshape(-1)
         assert (Fc[removed] == 0).all() and (Fc[~removed] != 0).any(dim=1).all()
-    dF = (torch.randn_like(Fc) * 0.1).to(torch.bfloat16)
-
-    def grads(engine, ctx):
-        st.ensure_grad().zero_()
-        engine.backward(ctx, dF)
-        return st.grad.clone()
-
-    gc, gp = grads(ce, ctx_c), grads(pe, ctx_p)
-    worst = 0.0
-    for k, (o, n, _) in st.offsets.items():
-        if o + n > st.n_train:
-            continue
-        a, b = gc[o:o + n], gp[o:o + n]
-        scale = b.abs().max().item() + 1e-30
-        cond = any(t in k for t in ("adaLN_modulation", "t_embedder", "y_embedder"))
-        err = (a - b).abs().max().item() / scale
-        worst = max(worst, err)
-        assert err <= (1e-2 if cond else 5e-5), (k, err)
-    print(name, "C driver vs Python engine: forward bit-equal, worst gradient deviation", worst)
 
 
 def test_s8_eval_cfg_and_short_sampler_vs_reference_golden():

@@ -83,13 +83,14 @@ def test_init_matches_reference_scheme():
     assert abs(sd["model.y_embedder.embedding_table.weight"].std().item() - 0.02) < 2e-3
 
 
-def test_flat_layout_plan():
-    from maskdit_b200.flat import ALIGN, FlatStore
-    from oracle import maskdit_oracle as O
-    cfg = O.Cfg(model_type="DiT-XL/2", img_resolution=32, num_classes=1000)
-    shapes = O.param_shapes(cfg)
-    st = FlatStore()
-    st.plan(shapes)
+def test_flat_store_layout_from_driver():
+    """The XL/2 store laid out by the C model handle: the adaLN matrix rows, aligned disjoint spans, the trainable
+    count, and the per-block gradient ranges."""
+    from maskdit_b200.flat import ALIGN
+    from maskdit_b200.maskdit import Precond_models
+    with torch.device("meta"):
+        net = Precond_models["edm"](32, 4, num_classes=1000, model_type="DiT-XL/2", use_decoder=True, mae_loss_coef=0.1)
+    _, st = net._layout()
     o, rows, hid = st.ada_w_range
     assert o == 0 and hid == 1152 and rows == 28 * 6912 + 2304 + 8 * 3072 + 1024
     spans = sorted((v[0], v[0] + v[1]) for v in st.offsets.values())
@@ -202,47 +203,27 @@ def test_config_schema_and_mask_schedule():
     assert parse_int_list("1,2,5-8") == [1, 2, 5, 6, 7, 8] and parse_float_none("None") is None
 
 
-@pytest.mark.parametrize("mt,R,ncls", [("DiT-S/2", 8, 10), ("DiT-B/4", 16, 7), ("DiT-XL/2", 32, 1000), ("DiT-XL/2", 64, 1000)])
-def test_c_driver_layout_equals_flat_store(mt, R, ncls):
-    """The packed parameter blob `mdt_model_param_info` enumerates (csrc/driver.cu) is exactly the layout FlatStore
-    builds for the nn.Module — names = the reference's state-dict keys — and the workspace planner is monotone."""
-    import ctypes
-    from maskdit_b200 import _lib
+def test_model_handle_and_flat_store_refuse_mismatches():
+    """`mdt_model_create` refuses a config it cannot lay out, and a FlatStore is only built for parameters whose names
+    and element counts are the handle's: a missing, an extra or a resized tensor raises with its name."""
+    from maskdit_b200._lib import MdtError
+    from maskdit_b200.engine import CEngine
     from maskdit_b200.flat import FlatStore
-    from oracle import maskdit_oracle as O
     from maskdit_b200.maskdit import Precond_models
-    cfg = O.Cfg(model_type=mt, img_resolution=R, num_classes=ncls)
-    with torch.device("meta"):   # registration order of the module (= the reference's, see make_golden.py's strict load)
-        net = Precond_models["edm"](R, 4, num_classes=ncls, model_type=mt, use_decoder=True, mae_loss_coef=0.1)
+    net = Precond_models["edm"](8, 4, num_classes=10, model_type="DiT-S/2", use_decoder=True, mae_loss_coef=0.1)
+    bad = net._cfg()
+    bad.hidden += 1                                   # hidden not divisible by heads
+    with pytest.raises(MdtError):
+        CEngine(bad)
+    ce = CEngine(net._cfg())
     shapes = {k: tuple(p.shape) for k, p in net.named_parameters()}
-    assert shapes == {k: tuple(v) for k, v in O.param_shapes(cfg).items()}
-    st = FlatStore()
-    st.plan(shapes)
-    L = _lib.lib()
-    mc = _lib.ModelCfg(R, 4, cfg.patch, ncls, cfg.hidden, cfg.depth, cfg.heads, 4 * cfg.hidden, 512, 8, 16, 2048, 1, 0.5)
-    h = ctypes.c_void_p()
-    assert L.mdt_model_create(ctypes.byref(mc), ctypes.byref(h)) == 0
-    n = L.mdt_model_num_tensors(h)
-    assert n == len(shapes)
-    name, off, num = ctypes.create_string_buffer(160), ctypes.c_longlong(), ctypes.c_longlong()
-    prev = -1
-    for i in range(n):
-        assert L.mdt_model_param_info(h, i, name, 160, ctypes.byref(off), ctypes.byref(num)) == 0
-        k = name.value.decode()
-        assert st.offsets[k][:2] == (off.value, num.value), k
-        assert off.value > prev and off.value % 64 == 0
-        prev = off.value
-    assert L.mdt_model_param_info(h, n, name, 160, None, None) != 0
-    assert (L.mdt_model_param_count(h, 1), L.mdt_model_param_count(h, 0)) == (st.n_train, st.n_total)
-    if mt == "DiT-XL/2":
-        assert L.mdt_model_param_count(h, 1) >= 730_115_216
-    T = cfg.num_patches // 2
-    tr, ev = L.mdt_workspace_bytes(h, 8, T, 1), L.mdt_workspace_bytes(h, 8, 0, 0)
-    assert tr > ev > 0 and L.mdt_workspace_bytes(h, 16, T, 1) > tr and L.mdt_workspace_bytes(h, 0, T, 1) < 0
-    bad = _lib.ModelCfg(R, 4, cfg.patch, ncls, cfg.hidden + 1, cfg.depth, cfg.heads, 4 * cfg.hidden, 512, 8, 16, 2048, 1, 0.5)
-    h2 = ctypes.c_void_p()
-    assert L.mdt_model_create(ctypes.byref(bad), ctypes.byref(h2)) != 0     # hidden not divisible by heads
-    L.mdt_model_destroy(h)
+    assert FlatStore(ce, shapes).offsets.keys() == shapes.keys()
+    fc1 = "model.blocks.3.mlp.fc1.weight"
+    missing = {k: s for k, s in shapes.items() if k != fc1}
+    for wrong, key in ((missing, fc1), (dict(shapes, **{fc1: (1537, 384)}), fc1),
+                       (dict(shapes, **{"model.extra": (4,)}), "model.extra")):
+        with pytest.raises(MdtError, match=re.escape(key)):
+            FlatStore(ce, wrong)
 
 
 def test_gemm_dispatch_plan_for_the_xl2_step():

@@ -68,6 +68,51 @@ def check_grads(net, g, tol=GRAD_TOL, what=""):
     print(what, "worst grad rel-L2", worst, "over", n, "tensors")
 
 
+def check_c_driver_matches_engine(net, x, sigma, lab, md, what="", dF_same_grads=None):
+    """The C++ step driver (`mdt_forward` / `mdt_backward`: one ctypes call each, one workspace) of the training-mode
+    `net` against the kernel-by-kernel Python `Engine` on the same flat store.  The forward agrees BIT FOR BIT, with and
+    without saved activations: same kernels, same order, same operands.  The backward accumulates wgrads with fp32
+    atomics (run-to-run order noise), so the gradients of a random dF agree to 5e-5 of each tensor's scale (1e-2 on the
+    conditioning path, see below).  `dF_same_grads(dF)`, when given, is a second dF for which the driver must give the
+    same gradients.  Returns the driver, its context of the saving forward and its F."""
+    from maskdit_b200.engine import CEngine, Engine
+    st = net.prepare()
+    ce, pe = net._engine, Engine(net._cfg(), st)
+    assert isinstance(ce, CEngine)
+    for save in (False, True):
+        Fc, ctx_c = ce.forward(x, sigma, lab, md, save)
+        Fp, ctx_p = pe.forward(x, sigma, lab, md, save)
+        assert torch.equal(Fc, Fp), (save, (Fc - Fp).abs().max())
+    dF = (torch.randn_like(Fc) * 0.1).to(torch.bfloat16)
+
+    def grads(engine, ctx, dF_):
+        st.ensure_grad().zero_()
+        engine.backward(ctx, dF_)
+        return st.grad.clone()
+
+    got = [grads(ce, ctx_c, dF)]
+    gp = grads(pe, ctx_p, dF)
+    if dF_same_grads is not None:
+        got.append(grads(ce, ctx_c, dF_same_grads(dF)))
+    worst = 0.0
+    for k, (o, n, _) in st.offsets.items():
+        if o + n > st.n_train:
+            continue
+        b = gp[o:o + n]
+        scale = b.abs().max().item() + 1e-30
+        # Order noise of the fp32 atomics: 1e-7 .. 1e-5 on the block tensors.  On the conditioning path the noisy sums
+        # are re-rounded to bf16 several times before GEMMs that contract over only B = 2 rows (dmod -> bf16 -> adaLN
+        # wgrad; dsc -> dc (bf16) -> dth -> dpre (bf16) -> t_embedder wgrad): one flipped bf16 rounding moves an element
+        # by 2^-8, measured up to 2e-3 of a tensor's scale between two runs of the SAME engine - not a code difference.
+        cond = any(t in k for t in ("adaLN_modulation", "t_embedder", "y_embedder"))
+        for g in got:
+            err = (g[o:o + n] - b).abs().max().item() / scale
+            worst = max(worst, err)
+            assert err <= (1e-2 if cond else 5e-5), (k, err)
+    print(what, "C driver vs Python engine: forward bit-equal, worst gradient deviation", worst)
+    return ce, ctx_c, Fc
+
+
 class ImplRecorder:
     """Which GEMM instances (BLOCK_N*10 + CTAs per tile) and which attention kernel families served the calls made
     inside the `with` block — read from the library's own logs (mdt_gemm_configs_seen / mdt_attention_impl_log), so the

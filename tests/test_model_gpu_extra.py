@@ -8,8 +8,8 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from test_model_gpu import (CFG_TOL, EVAL_TOL, FWD_TOL, GRAD_TOL, LOSS_TOL, GoldenLoss, ImplRecorder, build, check_grads, load,  # noqa: E402
-                            rel_l2)
+from test_model_gpu import (CFG_TOL, EVAL_TOL, FWD_TOL, GRAD_TOL, LOSS_TOL, GoldenLoss, ImplRecorder, build,  # noqa: E402
+                            check_c_driver_matches_engine, check_grads, load, rel_l2)
 
 pytestmark = pytest.mark.gpu
 
@@ -305,46 +305,18 @@ def test_optimizer_state_layouts_and_namespace_checkpoint(tmp_path):
 # ---- round 2: the C++ step driver (mdt_forward / mdt_backward) against the kernel-by-kernel Python engine ----------------
 @pytest.mark.parametrize("case", ["s2_train_mask", "s2_train_nomask", "xl2_c1_grads"])
 def test_c_driver_matches_python_engine(case):
-    """`mdt_forward` (one ctypes call, one workspace) == `Engine.forward` (per-kernel ctypes calls) BIT FOR BIT: same
-    kernels, same order, same operands.  The backward accumulates wgrads with fp32 atomics (run-to-run order noise), so
-    gradients are compared at 5e-5 of each tensor's scale (1e-2 on the conditioning path, see below)."""
-    from maskdit_b200.engine import CEngine, Engine
+    """`mdt_forward` == `Engine.forward` bit for bit; backward within the fp32-atomics order noise
+    (test_model_gpu.py::check_c_driver_matches_engine); the workspace contract."""
     g = load(case)
     xl = case.startswith("xl2")
     net, cfg, _ = build("DiT-XL/2", 32, 1000) if xl else build()
     net.train()
-    st = net.prepare()
-    assert isinstance(net._engine, CEngine)
     sigma = (g["rnd_normal"].cuda() * 1.2 - 1.2).exp().reshape(-1).contiguous()
     x = (g["images"].cuda() + g["noise_unit"].cuda() * sigma.view(-1, 1, 1, 1)).contiguous()
     lab = g["labels"].cuda().contiguous()
     md = {k: g[k].cuda() for k in ("mask", "ids_keep", "ids_restore")} if "ids_keep" in g else None
-    ce, pe = net._engine, Engine(net._cfg(), st)
-    for save in (False, True):
-        Fc, ctx_c = ce.forward(x, sigma, lab, md, save)
-        Fp, ctx_p = pe.forward(x, sigma, lab, md, save)
-        assert torch.equal(Fc, Fp), (save, (Fc - Fp).abs().max())
-    dF = (torch.randn_like(Fc) * 0.1).to(torch.bfloat16)
-    st.ensure_grad().zero_()
-    ce.backward(ctx_c, dF)
-    gc = st.grad.clone()
-    st.grad.zero_()
-    pe.backward(ctx_p, dF)
-    gp = st.grad.clone()
-    worst = 0.0
-    for k, (o, n, _) in st.offsets.items():
-        if o + n > st.n_train:
-            continue
-        a, b = gc[o:o + n], gp[o:o + n]
-        err = (a - b).abs().max().item() / (b.abs().max().item() + 1e-30)
-        worst = max(worst, err)
-        # Order noise of the fp32 atomics: 1e-7 .. 1e-5 on the block tensors.  On the conditioning path the noisy sums
-        # are re-rounded to bf16 several times before GEMMs that contract over only B = 2 rows (dmod -> bf16 -> adaLN
-        # wgrad; dsc -> dc (bf16) -> dth -> dpre (bf16) -> t_embedder wgrad): one flipped bf16 rounding moves an element
-        # by 2^-8, measured up to 2e-3 of a tensor's scale between two runs of the SAME engine - not a code difference.
-        cond = any(t in k for t in ("adaLN_modulation", "t_embedder", "y_embedder"))
-        assert err <= (1e-2 if cond else 5e-5), (k, err)
-    print(case, "C driver vs Python engine: forward bit-equal, worst gradient deviation", worst)
+    ce, ctx_c, Fc = check_c_driver_matches_engine(net, x, sigma, lab, md, case)
+    st = net.flat_store()
     # the workspace contract: mdt_workspace_bytes is what mdt_forward checks against
     B, T = x.shape[0], (md["ids_keep"].shape[1] if md else cfg.num_patches)
     assert ctx_c["nbytes"] == ce.workspace_bytes(B, T, True) > ce.workspace_bytes(B, T, False)

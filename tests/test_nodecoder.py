@@ -1,6 +1,6 @@
 """CPU tests of the decoder-less DiT (use_decoder=False, the reference's default, models/maskdit.py:254): a CPU fp32
 restatement of its forward against the unmodified reference (tests/golden/make_golden_nodecoder.py), the module's
-state-dict contract, the C driver's packed layout and its model-config validation."""
+state-dict contract and the C driver's model-config validation."""
 import ctypes
 import os
 import sys
@@ -147,13 +147,10 @@ MODELS = [f"DiT-{a}/{p}" for a in ("H", "XL", "L", "B", "S") for p in (2, 4, 8)]
 
 
 @pytest.mark.parametrize("mt", MODELS)
-def test_state_dict_and_c_layout_every_model(mt):
+def test_state_dict_every_model(mt):
     """For every DiT_models name: state-dict keys, shapes and ORDER equal the reference's (oracle.param_shapes follows
-    the reference's registration order and is pinned by make_golden's strict load), and the C driver's packed blob
-    is exactly FlatStore's layout, with the modulation vector of blocks 0..depth-1 then the final layer."""
-    from maskdit_b200 import _lib
-    from maskdit_b200.engine import Engine
-    from maskdit_b200.flat import FlatStore
+    the reference's registration order and is pinned by make_golden's strict load).  The C driver's layout of these
+    modules: test_geometry.py::test_packed_layout_rules_and_workspace."""
     from maskdit_b200.maskdit import DiT_models
     assert mt in DiT_models
     R = 32
@@ -168,34 +165,6 @@ def test_state_dict_and_c_layout_every_model(mt):
     D = cfg.hidden
     assert shapes["model.final_layer.linear.weight"] == (cfg.patch_dim, D)
     assert shapes["model.final_layer.adaLN_modulation.1.weight"] == (2 * D, D)
-    st = FlatStore()
-    st.plan(shapes)
-    NA = cfg.depth * 6 * D + 2 * D
-    assert st.ada_w_range[1:] == (NA, D)
-    eng = Engine(net._cfg(), st)   # head offsets: blocks 0..depth-1, final (no decoder layer)
-    assert (eng.NA, eng.off_final, eng.dec) == (NA, cfg.depth * 6 * D, [])
-    L = _lib.lib()
-    mc = _lib.ModelCfg(R, 4, cfg.patch, 1000, D, cfg.depth, cfg.heads, 4 * D, 0, 0, 0, 0, 0, 0.5)
-    h = ctypes.c_void_p()
-    assert L.mdt_model_create(ctypes.byref(mc), ctypes.byref(h)) == 0
-    try:
-        n = L.mdt_model_num_tensors(h)
-        assert n == len(shapes)
-        name, off, num = ctypes.create_string_buffer(160), ctypes.c_longlong(), ctypes.c_longlong()
-        prev = -1
-        for i in range(n):
-            assert L.mdt_model_param_info(h, i, name, 160, ctypes.byref(off), ctypes.byref(num)) == 0
-            k = name.value.decode()
-            assert st.offsets[k][:2] == (off.value, num.value), k
-            assert off.value > prev
-            prev = off.value
-        assert (L.mdt_model_param_count(h, 1), L.mdt_model_param_count(h, 0)) == (st.n_train, st.n_total)
-        assert L.mdt_model_mod_width(h) == NA
-        T = cfg.num_patches // 2
-        tr, ev = L.mdt_workspace_bytes(h, 8, T, 1), L.mdt_workspace_bytes(h, 8, 0, 0)
-        assert tr > ev > 0 and L.mdt_workspace_bytes(h, 16, T, 1) > tr
-    finally:
-        L.mdt_model_destroy(h)
 
 
 def test_module_init_and_unconditional_keys():

@@ -17,8 +17,8 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, ROOT)
-from test_model_gpu import (CFG_TOL, EVAL_TOL, FWD_TOL, LOSS_TOL, GoldenLoss, ImplRecorder, check_grads, load,  # noqa: E402
-                            rel_l2)
+from test_model_gpu import (CFG_TOL, EVAL_TOL, FWD_TOL, LOSS_TOL, GoldenLoss, ImplRecorder,  # noqa: E402
+                            check_c_driver_matches_engine, check_grads, load, rel_l2)
 
 pytestmark = pytest.mark.gpu
 
@@ -85,51 +85,22 @@ def test_loss_D_and_grads_vs_reference_golden(name):
 
 @pytest.mark.parametrize("name", list(CASES))
 def test_c_driver_matches_python_engine_and_masked_rows(name):
-    """`mdt_forward` == `Engine.forward` bit for bit; backward within the fp32-atomics order noise (bounds of
-    test_model_gpu_extra.py::test_c_driver_matches_python_engine).  Masked training: the removed tokens' rows of F
-    are exactly zero, and their dF reaches no parameter (a large dF there leaves every gradient unchanged)."""
-    from maskdit_b200.engine import CEngine, Engine
+    """`mdt_forward` == `Engine.forward` bit for bit; backward within the fp32-atomics order noise
+    (test_model_gpu.py::check_c_driver_matches_engine).  Masked training: the removed tokens' rows of F are exactly
+    zero, and their dF reaches no parameter (a large dF there leaves every gradient unchanged)."""
     (mt, R, ncls), _ = CASES[name]
     g = load(name)
     net, cfg, _ = build_nd(mt, R, ncls)
     net.train()
-    st = net.prepare()
-    assert isinstance(net._engine, CEngine)
     sigma, x, lab, md = inputs(g)
     sigma, x = sigma.reshape(-1).contiguous(), x.contiguous()
-    ce, pe = net._engine, Engine(net._cfg(), st)
-    for save in (False, True):
-        Fc, ctx_c = ce.forward(x, sigma, lab, md, save)
-        Fp, ctx_p = pe.forward(x, sigma, lab, md, save)
-        assert torch.equal(Fc, Fp), (save, (Fc - Fp).abs().max())
-    B, L, pd = x.shape[0], cfg.num_patches, cfg.patch_dim
+    B, L = x.shape[0], cfg.num_patches
     removed = md["mask"].bool().reshape(-1) if md else torch.zeros(B * L, dtype=torch.bool, device="cuda")
+    ce, ctx_c, Fc = check_c_driver_matches_engine(net, x, sigma, lab, md, name,
+                                                  dF_same_grads=lambda dF: dF.masked_fill(removed[:, None], 1e3))
     if md:
         assert int(removed.sum()) == B * (L - md["ids_keep"].shape[1])
         assert (Fc[removed] == 0).all() and (Fc[~removed] != 0).any(dim=1).all()
-    dF = (torch.randn_like(Fc) * 0.1).to(torch.bfloat16)
-
-    def grads(engine, ctx, dF_):
-        st.ensure_grad().zero_()
-        engine.backward(ctx, dF_)
-        return st.grad.clone()
-
-    gc, gp = grads(ce, ctx_c, dF), grads(pe, ctx_p, dF)
-    dF_big = dF.clone()
-    dF_big[removed] = 1e3
-    gbig = grads(ce, ctx_c, dF_big)
-    worst = 0.0
-    for k, (o, n, _) in st.offsets.items():
-        if o + n > st.n_train:
-            continue
-        b = gp[o:o + n]
-        scale = b.abs().max().item() + 1e-30
-        cond = any(t in k for t in ("adaLN_modulation", "t_embedder", "y_embedder"))
-        for a in (gc[o:o + n], gbig[o:o + n]):
-            err = (a - b).abs().max().item() / scale
-            worst = max(worst, err)
-            assert err <= (1e-2 if cond else 5e-5), (k, err)
-    print(name, "C driver vs Python engine: forward bit-equal, worst gradient deviation", worst)
     T = md["ids_keep"].shape[1] if md else L
     assert ctx_c["nbytes"] == ce.workspace_bytes(B, T, True) > ce.workspace_bytes(B, T, False)
     assert ce._count(md is not None) == (9 + 2 * bool(ncls) + 7 * cfg.depth + bool(md),

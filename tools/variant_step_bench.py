@@ -58,11 +58,8 @@ def workspace_bytes(use_decoder, B, mask):
     with torch.device("meta"):
         net = xl2(use_decoder)
     from maskdit_b200.engine import CEngine
-    from maskdit_b200.flat import FlatStore
-    st = FlatStore()
-    st.plan({k: tuple(p.shape) for k, p in net.named_parameters()})
     T = int(L * (1 - mask)) if mask > 0 else L
-    return CEngine(net._cfg(), st).workspace_bytes(B, T, True)
+    return CEngine(net._cfg()).workspace_bytes(B, T, True)
 
 
 def largest_batch(use_decoder, mask, cap):
