@@ -257,6 +257,22 @@ int mdt_adamw_ema_g16(float* w, const void* g_bf16, float* m, float* v, float* e
 int mdt_set_sm_budget(int n);
 int mdt_get_sm_budget(void);
 
+/* Deterministic mode (on != 0; 0 = default): every floating-point reduction of the backward runs in an order that is a
+ * function of the shapes alone, so repeated runs give identical bits whatever the SM count or budget.  Host-side
+ * setting of the process, read at launch (the Python layer sets it from torch.are_deterministic_algorithms_enabled()).
+ * What changes under it:
+ *   - MDT_EPI_ATOMIC GEMMs run one k-slice (mdt_gemm_plan reports it); MDT_EPI_DGELU with a colsum pointer writes its
+ *     output, then sums its columns in a fixed order;
+ *   - mdt_colsum_* sum in a fixed order; mdt_ln_modulate_bwd, mdt_gate_bwd and mdt_ln_modulate_bwd_gate run one block
+ *     per sample (rows_per_group rows);
+ *   - mdt_workspace_bytes(training) adds the step driver's scratch for per-block partial sums, after every activation.
+ * Entry points whose deterministic variant needs scratch they have no argument for return MDT_ERR_UNSUPPORTED under
+ * it: mdt_patch_embed_bwd, mdt_gate_bwd with dbias != NULL, mdt_ln_modulate_bwd_gate with y_bf16 and dbias != NULL,
+ * mdt_unmask_tokens_bwd with dmask_token != NULL (the step driver runs all four with workspace scratch).
+ * mdt_ln_modulate_bwd needs 16-byte aligned dshift / dscale and ld_dmod % 4 == 0 under it (MDT_ERR_UNSUPPORTED otherwise). */
+int mdt_set_deterministic(int on);
+int mdt_get_deterministic(void);
+
 /* ============================================================================================================
  * Step driver (SURVEY 8b): the whole network forward / backward as ONE call each over a packed parameter blob and ONE
  * caller-provided workspace — the launch sequence the reference obtains from autograd + torch.compile for

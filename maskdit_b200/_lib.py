@@ -113,6 +113,8 @@ _SIGS = {
     "mdt_adamw_ema_g16": [_P, _P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _F, _I, _F, _F, _I, _P],
     "mdt_set_sm_budget": [_I],
     "mdt_get_sm_budget": [],
+    "mdt_set_deterministic": [_I],
+    "mdt_get_deterministic": [],
     "mdt_adamw_ema": [_P, _P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _F, _I, _F, _F, _I, _P],
 }
 
@@ -164,6 +166,17 @@ def check(status: int, what: str, n_kernels: int = 1):
 
 def stream_ptr() -> int:
     return torch.cuda.current_stream().cuda_stream
+
+
+def sync_deterministic() -> bool:
+    """Set the library's deterministic mode (`mdt_set_deterministic`) from
+    `torch.are_deterministic_algorithms_enabled()`; returns the mode.  Called before the engine and the training step
+    launch, so `torch.use_deterministic_algorithms(True)` is the one switch."""
+    on = bool(torch.are_deterministic_algorithms_enabled())
+    L = lib()
+    if L.mdt_get_deterministic() != int(on):
+        check(L.mdt_set_deterministic(int(on)), "mdt_set_deterministic", 0)
+    return on
 
 
 def ptr(t):

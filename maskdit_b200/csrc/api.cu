@@ -1,4 +1,5 @@
 // extern "C" surface that is not tied to one kernel file: status strings, ABI version, GEMM entry.
+#include "deterministic.h"
 #include "gemm.h"
 
 #include <vector>
@@ -30,6 +31,12 @@ int mdt_set_sm_budget(int n) {
   return MDT_OK;
 }
 int mdt_get_sm_budget(void) { return mdt::g_sm_budget; }
+
+int mdt_set_deterministic(int on) {
+  mdt::g_deterministic = on != 0;
+  return MDT_OK;
+}
+int mdt_get_deterministic(void) { return mdt::g_deterministic; }
 
 int mdt_gemm_last_config(void) { return mdt::g_gemm_last_config; }
 int mdt_gemm_configs_seen(int reset) {
@@ -84,14 +91,24 @@ int mdt_gemm_plan(const mdt_gemm_args* args, long long* out10) {
   return MDT_OK;
 }
 
+// Deterministic mode: the DGELU epilogue's column sum (one reduction per tile and column) is replaced by an ordered
+// column sum of the stored bf16 output, the same values the fused sum adds.
+static int gemm_run(const mdt_gemm_args& a, cudaStream_t stream) {
+  if (!mdt::g_deterministic || a.epi != MDT_EPI_DGELU || !a.colsum) return mdt::gemm_launch(a, stream);
+  mdt_gemm_args b = a;
+  b.colsum = nullptr;
+  const int rc = mdt::gemm_launch(b, stream);
+  return rc == MDT_OK ? mdt::colsum_ordered(a.out, 1, a.M, a.N, a.ldo, a.colsum, stream) : rc;
+}
+
 int mdt_gemm_bf16(const mdt_gemm_args* args, void* stream) {
   if (!args || !args->A || !args->B || !args->out) return MDT_ERR_ARG;
-  if (!g_probe_on) return mdt::gemm_launch(*args, static_cast<cudaStream_t>(stream));
+  if (!g_probe_on) return gemm_run(*args, static_cast<cudaStream_t>(stream));
   GemmProbe p;
   if (cudaEventCreate(&p.e0) != cudaSuccess || cudaEventCreate(&p.e1) != cudaSuccess) return MDT_ERR_CUDA;
   p.flops = 2.0 * args->M * args->N * args->K;
   cudaEventRecord(p.e0, static_cast<cudaStream_t>(stream));
-  const int rc = mdt::gemm_launch(*args, static_cast<cudaStream_t>(stream));
+  const int rc = gemm_run(*args, static_cast<cudaStream_t>(stream));
   cudaEventRecord(p.e1, static_cast<cudaStream_t>(stream));
   g_probes.push_back(p);
   return rc;

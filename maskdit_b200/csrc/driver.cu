@@ -23,6 +23,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "deterministic.h"
 #include "../../include/maskdit_b200.h"
 
 namespace {
@@ -181,6 +182,7 @@ struct Plan {
   i64 fk;  // decoder-less + masked: final-layer output of the kept tokens [B*T, pd] f32, in the backward their dF bf16
   // backward scratch
   i64 dmod, dxf, Gz, dyA, dyB, dh, dxm, dO, dqkv, du, dxmd, Ge, dmod16, dsc, dc32, dc16, dth, dpre32, dpre16, ytmp;
+  i64 det;  // deterministic mode only: per-block partial sums (after everything else, so no other offset moves)
   i64 total;
 };
 
@@ -262,6 +264,9 @@ Plan make_plan(const mdt_model* m, int B, int T, bool save, bool with_backward) 
     p.dpre16 = a.take(static_cast<i64>(B) * D * 2);
     p.ytmp = a.take(static_cast<i64>(D) * m->Kp * 4);
   }
+  p.det = -1;
+  if (with_backward && mdt::g_deterministic)
+    p.det = a.take(mdt::det_scratch_floats(B, T, L, D, Dd, m->pd, m->cfg.has_mask_token) * 4);
   p.total = a.off;
   return p;
 }
@@ -275,6 +280,7 @@ struct Ctx {
   char* ws;
   void* stream;
   int rc = MDT_OK;
+  float* scratch = nullptr;  // Plan::det (deterministic mode)
   template <class T>
   T* at(i64 off) const { return off < 0 ? nullptr : reinterpret_cast<T*>(ws + off); }
   const float* W32(const Tensor& t) const { return w32 + t.off; }
@@ -363,10 +369,10 @@ void ln_bwd_gate(Ctx& c, const void* dxmod, const float* x, const float* mean, c
                  int rows_per_group, float* g, int accumulate, float* dshift, float* dscale, i64 M, int d,
                  const GateNext* gn) {
   const int NA = c.m->NA;
-  c.ck(mdt_ln_modulate_bwd_gate(dxmod, x, mean, rstd, scale, NA, rows_per_group, g, accumulate, dshift, dscale, NA,
-                                gn ? gn->y : nullptr, gn ? gn->gate : nullptr, gn ? NA : 0, gn ? gn->dy : nullptr,
-                                gn ? gn->dgate : nullptr, gn ? NA : 0, gn ? gn->dbias : nullptr, static_cast<int>(M), d,
-                                c.stream));
+  c.ck(mdt::ln_modulate_bwd_gate_s(dxmod, x, mean, rstd, scale, NA, rows_per_group, g, accumulate, dshift, dscale, NA,
+                                   gn ? gn->y : nullptr, gn ? gn->gate : nullptr, gn ? NA : 0, gn ? gn->dy : nullptr,
+                                   gn ? gn->dgate : nullptr, gn ? NA : 0, gn ? gn->dbias : nullptr,
+                                   static_cast<int>(M), d, c.scratch, static_cast<cudaStream_t>(c.stream)));
 }
 
 GateNext mlp_gate(Ctx& c, const BlockP& s, const BlockBuf& b, const float* mod, float* dmod, void* dy) {
@@ -548,6 +554,7 @@ int mdt_backward(const mdt_model* m, const float* w32, const void* w16, float* g
   const Plan p = make_plan(m, B, T, true, true);
   if (p.total > workspace_bytes || (reinterpret_cast<uintptr_t>(workspace) & 255)) return MDT_ERR_ARG;
   Ctx c{m, w32, static_cast<const __nv_bfloat16*>(w16), grad, static_cast<char*>(workspace), stream};
+  c.scratch = c.at<float>(p.det);
   const mdt_model_cfg& cf = m->cfg;
   const int D = m->D, Dd = m->Dd, L = m->L, NA = m->NA, nc = cf.num_classes, pd = m->pd;
   const i64 Me = static_cast<i64>(B) * T, Md = static_cast<i64>(B) * L;
@@ -599,7 +606,7 @@ int mdt_backward(const mdt_model* m, const float* w32, const void* w16, float* g
     }
     // ---- unmask + decoder layer
     float* tok_g = (cf.has_mask_token && ids_restore) ? c.Gd(m->mask_token) : nullptr;
-    c.ck(mdt_unmask_tokens_bwd(Gz, nullptr, ids_restore, c.at<void>(p.du), tok_g, B, T, L, Dd, stream));
+    c.ck(mdt::unmask_tokens_bwd_s(Gz, ids_restore, c.at<void>(p.du), tok_g, B, T, L, Dd, c.scratch, cs));
     o = m->off_declayer;
     wgrad(c, c.at<void>(p.du), c.at<void>(p.xmd), Dd, D, Me, c.Gd(m->dlw));
     c.ck(mdt_colsum_bf16(c.at<void>(p.du), static_cast<int>(Me), Dd, Dd, c.Gd(m->dlb), stream));
@@ -623,8 +630,8 @@ int mdt_backward(const mdt_model* m, const float* w32, const void* w16, float* g
     if (on_ready && c.rc == MDT_OK) on_ready(user, m->enc[i].lo, m->enc[i].hi);
   }
   // ---- patch embedding (no input gradient needed)
-  c.ck(mdt_patch_embed_bwd(x_in, sigma, cf.sigma_data, ids_keep, Ge, c.Gd(m->xw), c.Gd(m->xb), B, cf.img_channels,
-                           cf.img_resolution, cf.patch_size, D, T, stream));
+  c.ck(mdt::patch_embed_bwd_s(x_in, sigma, cf.sigma_data, ids_keep, Ge, c.Gd(m->xw), c.Gd(m->xb), B, cf.img_channels,
+                              cf.img_resolution, cf.patch_size, D, T, c.scratch, cs));
   // ---- adaLN projections of all blocks at once, then the conditioning MLPs
   void* dmod16 = c.at<void>(p.dmod16);
   c.ck(mdt_cast_f32_bf16(dmod, dmod16, static_cast<i64>(B) * NA, stream));

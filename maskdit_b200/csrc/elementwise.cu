@@ -3,6 +3,7 @@
 // All are coalesced, 8/16-byte vectorised streaming kernels with warp-level reductions; none has data reuse that
 // would justify smem tiling (guide: elementwise/reduction kernels are fixed by fusion + vector width).
 #include "common.cuh"
+#include "deterministic.h"
 #include "../../include/maskdit_b200.h"
 
 namespace mdt {
@@ -99,11 +100,13 @@ __global__ void patch_embed_kernel(const float* __restrict__ x, const float* __r
 // kPebTok = 128 tokens per block (one atomic per (channel, weight) per block) for cpp <= 96 (patch 2 and 4 at 4
 // channels); 32 for cpp <= 384 (patch 8: cpp = 256), so the [kPebTok][cpp] patch block stays within 48 KB of smem.
 constexpr int kPebMaxCpp = 48 * 1024 / (32 * 4);
-template <int kPebTok>
-__global__ void patch_embed_bwd_kernel(const float* __restrict__ x, const float* __restrict__ sigma,
-                                       float sigma_data, const int64_t* __restrict__ ids_keep,
-                                       const float* __restrict__ g, float* __restrict__ gW, float* __restrict__ gb,
-                                       int C, int R, int p, int D, int T) {
+// kStore (deterministic mode): the block's sums are stored, not added, into its own row of per-block partials
+// (gW -> [blocks, D * cpp], gb -> [blocks, D]); colsum_ordered reduces the rows afterwards.
+template <int kPebTok, bool kStore>
+__device__ __forceinline__ void patch_embed_bwd_body(const float* __restrict__ x, const float* __restrict__ sigma,
+                                                     float sigma_data, const int64_t* __restrict__ ids_keep,
+                                                     const float* __restrict__ g, float* __restrict__ gW,
+                                                     float* __restrict__ gb, int C, int R, int p, int D, int T) {
   extern __shared__ float s_patch[];  // [kPebTok][cpp]
   const int cpp = C * p * p, G = R / p;
   const int b = blockIdx.y, i0 = blockIdx.x * kPebTok;
@@ -118,6 +121,10 @@ __global__ void patch_embed_bwd_kernel(const float* __restrict__ x, const float*
     s_patch[e] = c_in * x[((static_cast<size_t>(b) * C + c) * R + hh) * R + ww];
   }
   __syncthreads();
+  if (kStore) {
+    const size_t blk = static_cast<size_t>(blockIdx.y) * gridDim.x + blockIdx.x;
+    gW += blk * D * cpp, gb += blk * D;
+  }
   for (int d = threadIdx.x; d < D; d += blockDim.x) {
     float sb = 0.f;
     // cpp is processed in slabs of 16 accumulators to bound registers (cpp = 16 for patch 2, C 4)
@@ -133,11 +140,29 @@ __global__ void patch_embed_bwd_kernel(const float* __restrict__ x, const float*
           if (j0 + j < cpp) acc[j] = fmaf(gv, s_patch[t * cpp + j0 + j], acc[j]);
       }
 #pragma unroll
-      for (int j = 0; j < 16; ++j)
-        if (j0 + j < cpp) atomicAdd(gW + static_cast<size_t>(d) * cpp + j0 + j, acc[j]);
+      for (int j = 0; j < 16; ++j) {
+        if (j0 + j >= cpp) continue;
+        if (kStore) gW[static_cast<size_t>(d) * cpp + j0 + j] = acc[j];
+        else atomicAdd(gW + static_cast<size_t>(d) * cpp + j0 + j, acc[j]);
+      }
     }
-    atomicAdd(gb + d, sb);
+    if (kStore) gb[d] = sb;
+    else atomicAdd(gb + d, sb);
   }
+}
+template <int kPebTok>
+__global__ void patch_embed_bwd_kernel(const float* __restrict__ x, const float* __restrict__ sigma,
+                                       float sigma_data, const int64_t* __restrict__ ids_keep,
+                                       const float* __restrict__ g, float* __restrict__ gW, float* __restrict__ gb,
+                                       int C, int R, int p, int D, int T) {
+  patch_embed_bwd_body<kPebTok, false>(x, sigma, sigma_data, ids_keep, g, gW, gb, C, R, p, D, T);
+}
+template <int kPebTok>
+__global__ void patch_embed_bwd_partial_kernel(const float* __restrict__ x, const float* __restrict__ sigma,
+                                               float sigma_data, const int64_t* __restrict__ ids_keep,
+                                               const float* __restrict__ g, float* __restrict__ pW,
+                                               float* __restrict__ pb, int C, int R, int p, int D, int T) {
+  patch_embed_bwd_body<kPebTok, true>(x, sigma, sigma_data, ids_keep, g, pW, pb, C, R, p, D, T);
 }
 
 // =========================================================================================================
@@ -214,6 +239,56 @@ __global__ void colsum_f32_kernel(const float* __restrict__ in, int M, int N, in
   float s = 0.f;
   for (int r = r0; r < r1; ++r) s += in[static_cast<size_t>(r) * ld + c];
   atomicAdd(out + c, s);
+}
+
+// Column sums in a fixed order (deterministic mode).  Block = one strip of kCoCols columns and ALL rows: row lane w
+// sums rows w, w + kCoLanes, ... in ascending order, then one thread per column adds the lanes' sums in lane order and
+// adds the total to out[c] (the address's only write in the launch).  The order depends on M alone.
+constexpr int kCoCols = 32, kCoLanes = 32, kCoUnroll = 8;
+MDT_DEVINL float load_f32(const float* p) { return __ldg(p); }
+MDT_DEVINL float load_f32(const __nv_bfloat16* p) { return __bfloat162float(*p); }
+template <typename T>
+__global__ void __launch_bounds__(kCoCols * kCoLanes)
+colsum_ordered_kernel(const T* __restrict__ in, int M, int N, long long ld, float* __restrict__ out) {
+  __shared__ float s_part[kCoLanes][kCoCols + 1];
+  const int tx = threadIdx.x % kCoCols, lane = threadIdx.x / kCoCols;
+  const int c = blockIdx.x * kCoCols + tx;
+  float s = 0.f;
+  if (c < N) {
+    const T* col = in + c;
+    int r = lane;
+    // kCoUnroll independent loads in flight, added in row order
+    for (; r + (kCoUnroll - 1) * kCoLanes < M; r += kCoUnroll * kCoLanes) {
+      float v[kCoUnroll];
+#pragma unroll
+      for (int u = 0; u < kCoUnroll; ++u) v[u] = load_f32(col + static_cast<long long>(r + u * kCoLanes) * ld);
+#pragma unroll
+      for (int u = 0; u < kCoUnroll; ++u) s += v[u];
+    }
+    for (; r < M; r += kCoLanes) s += load_f32(col + static_cast<long long>(r) * ld);
+  }
+  s_part[lane][tx] = s;
+  __syncthreads();
+  if (lane == 0 && c < N) {
+    float t = s_part[0][tx];
+    for (int w = 1; w < kCoLanes; ++w) t += s_part[w][tx];
+    out[c] += t;
+  }
+}
+
+// =========================================================================================================
+// Deterministic mode (mdt_set_deterministic): the process-wide setting and the ordered reduction every variant ends in
+// =========================================================================================================
+int g_deterministic = 0;
+
+int colsum_ordered(const void* in, int in_bf16, int M, int N, long long ld, float* out, cudaStream_t stream) {
+  if (M <= 0 || N <= 0) return MDT_OK;
+  const int grid = (N + kCoCols - 1) / kCoCols;
+  if (in_bf16)
+    colsum_ordered_kernel<<<grid, kCoCols * kCoLanes, 0, stream>>>(static_cast<const __nv_bfloat16*>(in), M, N, ld, out);
+  else
+    colsum_ordered_kernel<<<grid, kCoCols * kCoLanes, 0, stream>>>(static_cast<const float*>(in), M, N, ld, out);
+  return cudaGetLastError() == cudaSuccess ? MDT_OK : MDT_ERR_CUDA;
 }
 
 // =========================================================================================================
@@ -407,15 +482,15 @@ __global__ void gate_bwd_kernel(const float* __restrict__ g, const __nv_bfloat16
 // =========================================================================================================
 constexpr int kLgBatch = 4;
 constexpr int kLgMaxThreads = 320;  // D <= 1280
-template <bool GATE>
-__global__ void __launch_bounds__(kLgMaxThreads, 2)
-ln_bwd_gate_kernel(const __nv_bfloat16* __restrict__ dxmod, const float* __restrict__ x,
-                   const float* __restrict__ mean, const float* __restrict__ rstd, const float* __restrict__ scale,
-                   int ld_mod, int rows_per_group, float* __restrict__ g, int accumulate, float* __restrict__ dshift,
-                   float* __restrict__ dscale, int ld_dmod, const __nv_bfloat16* __restrict__ y,
-                   const float* __restrict__ gate, int ld_gate, __nv_bfloat16* __restrict__ dy,
-                   float* __restrict__ dgate, int ld_dgate, float* __restrict__ dbias, int M, int D,
-                   int rows_per_block) {
+// kBiasRows (deterministic mode, one block per sample): the block's bias-gradient sum is stored into row b of dbias
+// ([samples, D] scratch) instead of being added to dbias[:]; colsum_ordered reduces the rows afterwards.
+template <bool GATE, bool kBiasRows>
+__device__ __forceinline__ void ln_bwd_gate_body(
+    const __nv_bfloat16* __restrict__ dxmod, const float* __restrict__ x, const float* __restrict__ mean,
+    const float* __restrict__ rstd, const float* __restrict__ scale, int ld_mod, int rows_per_group,
+    float* __restrict__ g, int accumulate, float* __restrict__ dshift, float* __restrict__ dscale, int ld_dmod,
+    const __nv_bfloat16* __restrict__ y, const float* __restrict__ gate, int ld_gate, __nv_bfloat16* __restrict__ dy,
+    float* __restrict__ dgate, int ld_dgate, float* __restrict__ dbias, int M, int D, int rows_per_block) {
   __shared__ float4 s_part[2][kLgMaxThreads / 32][2];  // [parity][warp][{s1 x4}, {s2 x4}]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
   const int c = tid * 4;
@@ -499,8 +574,32 @@ ln_bwd_gate_kernel(const __nv_bfloat16* __restrict__ dxmod, const float* __restr
   red_add_v4(gaddr(dscale + static_cast<size_t>(b) * ld_dmod + c), a_sc);
   if (GATE) {
     red_add_v4(gaddr(dgate + static_cast<size_t>(b) * ld_dgate + c), ag);
-    if (dbias) red_add_v4(gaddr(dbias + c), ab);
+    if (kBiasRows) stg128(gaddr(dbias + static_cast<size_t>(b) * D + c), ab);
+    else if (dbias) red_add_v4(gaddr(dbias + c), ab);
   }
+}
+template <bool GATE>
+__global__ void __launch_bounds__(kLgMaxThreads, 2)
+ln_bwd_gate_kernel(const __nv_bfloat16* __restrict__ dxmod, const float* __restrict__ x,
+                   const float* __restrict__ mean, const float* __restrict__ rstd, const float* __restrict__ scale,
+                   int ld_mod, int rows_per_group, float* __restrict__ g, int accumulate, float* __restrict__ dshift,
+                   float* __restrict__ dscale, int ld_dmod, const __nv_bfloat16* __restrict__ y,
+                   const float* __restrict__ gate, int ld_gate, __nv_bfloat16* __restrict__ dy,
+                   float* __restrict__ dgate, int ld_dgate, float* __restrict__ dbias, int M, int D,
+                   int rows_per_block) {
+  ln_bwd_gate_body<GATE, false>(dxmod, x, mean, rstd, scale, ld_mod, rows_per_group, g, accumulate, dshift, dscale,
+                                ld_dmod, y, gate, ld_gate, dy, dgate, ld_dgate, dbias, M, D, rows_per_block);
+}
+__global__ void __launch_bounds__(kLgMaxThreads, 2)
+ln_bwd_gate_bias_rows_kernel(const __nv_bfloat16* __restrict__ dxmod, const float* __restrict__ x,
+                             const float* __restrict__ mean, const float* __restrict__ rstd,
+                             const float* __restrict__ scale, int ld_mod, int rows_per_group, float* __restrict__ g,
+                             int accumulate, float* __restrict__ dshift, float* __restrict__ dscale, int ld_dmod,
+                             const __nv_bfloat16* __restrict__ y, const float* __restrict__ gate, int ld_gate,
+                             __nv_bfloat16* __restrict__ dy, float* __restrict__ dgate, int ld_dgate,
+                             float* __restrict__ dbias_rows, int M, int D, int rows_per_block) {
+  ln_bwd_gate_body<true, true>(dxmod, x, mean, rstd, scale, ld_mod, rows_per_group, g, accumulate, dshift, dscale,
+                               ld_dmod, y, gate, ld_gate, dy, dgate, ld_dgate, dbias_rows, M, D, rows_per_block);
 }
 
 // =========================================================================================================
@@ -536,9 +635,12 @@ __global__ void unmask_kernel(const float* __restrict__ u, const float* __restri
     }
   }
 }
-__global__ void unmask_bwd_kernel(const float* __restrict__ g, const int64_t* __restrict__ ids_restore,
-                                  __nv_bfloat16* __restrict__ du, float* __restrict__ dmask_token, int T, int L,
-                                  int D) {
+// kStore (deterministic mode): the block's mask-token sum is stored into its own row of dmask_token ([blocks, D]
+// scratch, block = blockIdx.y * gridDim.x + blockIdx.x); colsum_ordered reduces the rows afterwards.
+template <bool kStore>
+__device__ __forceinline__ void unmask_bwd_body(const float* __restrict__ g, const int64_t* __restrict__ ids_restore,
+                                                __nv_bfloat16* __restrict__ du, float* __restrict__ dmask_token, int T,
+                                                int L, int D) {
   const int c = threadIdx.x * 4;
   if (c >= D) return;
   const int b = blockIdx.y, l0 = blockIdx.x * kUmPos, l1 = min(L, l0 + kUmPos);
@@ -563,11 +665,24 @@ __global__ void unmask_bwd_kernel(const float* __restrict__ g, const int64_t* __
       }
     }
   }
-  if (dmask_token) {  // one 16-byte reduction per thread and block (64 positions): [B * L / 64] per address
+  if (kStore) {
+    const size_t blk = static_cast<size_t>(blockIdx.y) * gridDim.x + blockIdx.x;
+    *reinterpret_cast<float4*>(dmask_token + blk * D + c) = acc;
+  } else if (dmask_token) {  // one 16-byte reduction per thread and block (64 positions): [B * L / 64] per address
     asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dmask_token + c), "f"(acc.x), "f"(acc.y),
                  "f"(acc.z), "f"(acc.w)
                  : "memory");
   }
+}
+__global__ void unmask_bwd_kernel(const float* __restrict__ g, const int64_t* __restrict__ ids_restore,
+                                  __nv_bfloat16* __restrict__ du, float* __restrict__ dmask_token, int T, int L,
+                                  int D) {
+  unmask_bwd_body<false>(g, ids_restore, du, dmask_token, T, L, D);
+}
+__global__ void unmask_bwd_rows_kernel(const float* __restrict__ g, const int64_t* __restrict__ ids_restore,
+                                       __nv_bfloat16* __restrict__ du, float* __restrict__ dmask_rows, int T, int L,
+                                       int D) {
+  unmask_bwd_body<true>(g, ids_restore, du, dmask_rows, T, L, D);
 }
 
 
@@ -581,6 +696,102 @@ __global__ void gather_rows_bf16_kernel(const uint2* __restrict__ in, const int6
     const long long b = row / T;
     out[i] = in[(b * L + idx[row]) * D4 + c];
   }
+}
+
+long long det_scratch_floats(int B, int T, int L, int D, int Dd, int cpp, int has_mask_token) {
+  const long long tok = 128 * cpp * sizeof(float) <= 48 * 1024 ? 128 : 32;
+  const long long pe = static_cast<long long>(B) * ((T + tok - 1) / tok) * D * (cpp + 1);
+  const long long um = has_mask_token ? static_cast<long long>(B) * ((L + kUmPos - 1) / kUmPos) * Dd : 0;
+  const long long ln = static_cast<long long>(B) * (D > Dd ? D : Dd);
+  return pe > um ? (pe > ln ? pe : ln) : (um > ln ? um : ln);
+}
+
+int patch_embed_bwd_s(const float* x, const float* sigma, float sigma_data, const int64_t* ids_keep, const float* g,
+                      float* gW, float* gb, int B, int C, int R, int p, int D, int T, float* scratch,
+                      cudaStream_t stream) {
+  if (!x || !g || !gW || !gb || B <= 0 || T <= 0 || R % p) return MDT_ERR_ARG;
+  const int cpp = C * p * p;
+  if (cpp > kPebMaxCpp) return MDT_ERR_UNSUPPORTED;
+  const int tok = 128 * cpp * sizeof(float) <= 48 * 1024 ? 128 : 32;
+  const dim3 grid((T + tok - 1) / tok, B);
+  const size_t smem = tok * cpp * sizeof(float);
+  if (!g_deterministic) {
+    if (tok == 128)
+      patch_embed_bwd_kernel<128><<<grid, 384, smem, stream>>>(x, sigma, sigma_data, ids_keep, g, gW, gb, C, R, p, D, T);
+    else
+      patch_embed_bwd_kernel<32><<<grid, 384, smem, stream>>>(x, sigma, sigma_data, ids_keep, g, gW, gb, C, R, p, D, T);
+    return launch_status();
+  }
+  if (!scratch) return MDT_ERR_UNSUPPORTED;
+  const long long blocks = static_cast<long long>(grid.x) * grid.y;
+  float* pW = scratch;
+  float* pb = scratch + blocks * D * cpp;
+  if (tok == 128)
+    patch_embed_bwd_partial_kernel<128><<<grid, 384, smem, stream>>>(x, sigma, sigma_data, ids_keep, g, pW, pb, C, R,
+                                                                     p, D, T);
+  else
+    patch_embed_bwd_partial_kernel<32><<<grid, 384, smem, stream>>>(x, sigma, sigma_data, ids_keep, g, pW, pb, C, R,
+                                                                    p, D, T);
+  int rc = launch_status();
+  if (rc == MDT_OK) rc = colsum_ordered(pW, 0, static_cast<int>(blocks), D * cpp, D * cpp, gW, stream);
+  if (rc == MDT_OK) rc = colsum_ordered(pb, 0, static_cast<int>(blocks), D, D, gb, stream);
+  return rc;
+}
+
+int ln_modulate_bwd_gate_s(const void* dxmod_bf16, const float* x, const float* mean, const float* rstd,
+                           const float* scale, int ld_mod, int rows_per_group, float* g, int accumulate, float* dshift,
+                           float* dscale, int ld_dmod, const void* y_bf16, const float* gate, int ld_gate,
+                           void* dy_bf16, float* dgate, int ld_dgate, float* dbias, int M, int D, float* scratch,
+                           cudaStream_t stream) {
+  if (!dxmod_bf16 || !x || !mean || !rstd || !scale || !g || !dshift || !dscale || M <= 0) return MDT_ERR_ARG;
+  if (rows_per_group <= 0 || M % rows_per_group || (ld_mod & 3) || (ld_dmod & 3)) return MDT_ERR_ARG;
+  if (y_bf16 && (!gate || !dy_bf16 || !dgate || (ld_gate & 3) || (ld_dgate & 3))) return MDT_ERR_ARG;
+  if ((reinterpret_cast<uintptr_t>(scale) | reinterpret_cast<uintptr_t>(dshift) | reinterpret_cast<uintptr_t>(dscale) |
+       reinterpret_cast<uintptr_t>(gate) | reinterpret_cast<uintptr_t>(dgate) | reinterpret_cast<uintptr_t>(dbias)) & 15)
+    return MDT_ERR_ARG;
+  if (D % 128 || D / 4 > kLgMaxThreads) return MDT_ERR_UNSUPPORTED;  // D <= 1280, as the LN kernels
+  // deterministic: one block per sample (rows_per_group rows), so the per-sample sums have one writer each; the bias
+  // gradient, a sum over samples, goes through per-sample rows in `scratch`
+  const bool bias_rows = g_deterministic && y_bf16 && dbias;
+  if (bias_rows && (!scratch || (reinterpret_cast<uintptr_t>(scratch) & 15))) return MDT_ERR_UNSUPPORTED;
+  const int rpb = g_deterministic ? rows_per_group : gcd_int(rows_per_group, 32);
+  const int grid = M / rpb;
+  const __nv_bfloat16* dx = static_cast<const __nv_bfloat16*>(dxmod_bf16);
+  const __nv_bfloat16* y = static_cast<const __nv_bfloat16*>(y_bf16);
+  __nv_bfloat16* dy = static_cast<__nv_bfloat16*>(dy_bf16);
+  if (bias_rows) {
+    ln_bwd_gate_bias_rows_kernel<<<grid, D / 4, 0, stream>>>(dx, x, mean, rstd, scale, ld_mod, rows_per_group, g,
+                                                             accumulate, dshift, dscale, ld_dmod, y, gate, ld_gate, dy,
+                                                             dgate, ld_dgate, scratch, M, D, rpb);
+    const int rc = launch_status();
+    return rc == MDT_OK ? colsum_ordered(scratch, 0, grid, D, D, dbias, stream) : rc;
+  }
+  if (y_bf16)
+    ln_bwd_gate_kernel<true><<<grid, D / 4, 0, stream>>>(dx, x, mean, rstd, scale, ld_mod, rows_per_group, g,
+                                                         accumulate, dshift, dscale, ld_dmod, y, gate, ld_gate, dy,
+                                                         dgate, ld_dgate, dbias, M, D, rpb);
+  else
+    ln_bwd_gate_kernel<false><<<grid, D / 4, 0, stream>>>(dx, x, mean, rstd, scale, ld_mod, rows_per_group, g,
+                                                          accumulate, dshift, dscale, ld_dmod, nullptr, nullptr, 0,
+                                                          nullptr, nullptr, 0, nullptr, M, D, rpb);
+  return launch_status();
+}
+
+int unmask_tokens_bwd_s(const float* g, const int64_t* ids_restore, void* du_bf16, float* dmask_token, int B, int T,
+                        int L, int D, float* scratch, cudaStream_t stream) {
+  if (!g || !du_bf16 || B <= 0 || T <= 0 || L <= 0 || D % 4 || D > 4096) return MDT_ERR_ARG;
+  if (!ids_restore && T != L) return MDT_ERR_ARG;
+  const dim3 grid((L + kUmPos - 1) / kUmPos, B);
+  const int threads = ((D / 4 + 31) / 32) * 32;
+  __nv_bfloat16* du = static_cast<__nv_bfloat16*>(du_bf16);
+  if (!g_deterministic || !dmask_token) {
+    unmask_bwd_kernel<<<grid, threads, 0, stream>>>(g, ids_restore, du, dmask_token, T, L, D);
+    return launch_status();
+  }
+  if (!scratch || (reinterpret_cast<uintptr_t>(scratch) & 15)) return MDT_ERR_UNSUPPORTED;
+  unmask_bwd_rows_kernel<<<grid, threads, 0, stream>>>(g, ids_restore, du, scratch, T, L, D);
+  const int rc = launch_status();
+  return rc == MDT_OK ? colsum_ordered(scratch, 0, static_cast<int>(grid.x * grid.y), D, D, dmask_token, stream) : rc;
 }
 
 }  // namespace mdt
@@ -616,19 +827,7 @@ int mdt_patch_embed(const float* x, const float* sigma, float sigma_data, const 
 
 int mdt_patch_embed_bwd(const float* x, const float* sigma, float sigma_data, const int64_t* ids_keep,
                         const float* g, float* gW, float* gb, int B, int C, int R, int p, int D, int T, void* stream) {
-  if (!x || !g || !gW || !gb || B <= 0 || T <= 0 || R % p) return MDT_ERR_ARG;
-  const int cpp = C * p * p;
-  if (cpp > kPebMaxCpp) return MDT_ERR_UNSUPPORTED;
-  if (128 * cpp * sizeof(float) <= 48 * 1024) {
-    dim3 grid((T + 127) / 128, B);
-    patch_embed_bwd_kernel<128><<<grid, 384, 128 * cpp * sizeof(float), S(stream)>>>(x, sigma, sigma_data, ids_keep,
-                                                                                      g, gW, gb, C, R, p, D, T);
-  } else {
-    dim3 grid((T + 31) / 32, B);
-    patch_embed_bwd_kernel<32><<<grid, 384, 32 * cpp * sizeof(float), S(stream)>>>(x, sigma, sigma_data, ids_keep, g,
-                                                                                    gW, gb, C, R, p, D, T);
-  }
-  return launch_status();
+  return patch_embed_bwd_s(x, sigma, sigma_data, ids_keep, g, gW, gb, B, C, R, p, D, T, nullptr, S(stream));
 }
 
 int mdt_timestep_freq(const float* sigma, int B, int dim, void* out_bf16, void* stream) {
@@ -664,12 +863,14 @@ int mdt_cast_f32_bf16(const float* in, void* out_bf16, long long n, void* stream
 }
 int mdt_colsum_bf16(const void* in_bf16, int M, int N, int ld, float* out, void* stream) {
   if (!in_bf16 || !out || M <= 0 || N <= 0 || (ld & 1)) return MDT_ERR_ARG;
+  if (g_deterministic) return colsum_ordered(in_bf16, 1, M, N, ld, out, S(stream));
   dim3 grid((N + 255) / 256, (M + kCsRows - 1) / kCsRows);
   colsum_bf16_kernel<<<grid, 128, 0, S(stream)>>>(static_cast<const __nv_bfloat16*>(in_bf16), M, N, ld, out);
   return launch_status();
 }
 int mdt_colsum_f32(const float* in, int M, int N, int ld, float* out, void* stream) {
   if (!in || !out || M <= 0 || N <= 0) return MDT_ERR_ARG;
+  if (g_deterministic) return colsum_ordered(in, 0, M, N, ld, out, S(stream));
   dim3 grid((N + 127) / 128, (M + kCsRows - 1) / kCsRows);
   colsum_f32_kernel<<<grid, 128, 0, S(stream)>>>(in, M, N, ld, out);
   return launch_status();
@@ -705,6 +906,14 @@ int mdt_ln_modulate_bwd(const void* dxmod_bf16, const float* x, const float* mea
     return MDT_ERR_ARG;
   if (rows_per_group <= 0 || M % rows_per_group || (ld_mod & 3)) return MDT_ERR_ARG;
   if (reinterpret_cast<uintptr_t>(scale) & 15) return MDT_ERR_ARG;
+  if (g_deterministic) {  // the fused kernel with one block per sample: each dshift / dscale address has one writer
+    if (D / 4 > kLgMaxThreads || (ld_dmod & 3) ||
+        ((reinterpret_cast<uintptr_t>(dshift) | reinterpret_cast<uintptr_t>(dscale)) & 15))
+      return MDT_ERR_UNSUPPORTED;
+    return ln_modulate_bwd_gate_s(dxmod_bf16, x, mean, rstd, scale, ld_mod, rows_per_group, g, accumulate, dshift,
+                                  dscale, ld_dmod, nullptr, nullptr, 0, nullptr, nullptr, 0, nullptr, M, D, nullptr,
+                                  S(stream));
+  }
   const int rpb = gcd_int(rows_per_group, kLnbRowsMax);
   const int grid = M / rpb;
   MDT_LN_DISPATCH(D / 128, ln_modulate_bwd_kernel<kNV><<<grid, 128, 0, S(stream)>>>(
@@ -719,7 +928,10 @@ int mdt_gate_bwd(const float* g, const void* y_bf16, const float* gate, int ld_g
   if (rows_per_group <= 0 || M % rows_per_group || (ld_gate & 3)) return MDT_ERR_ARG;
   if (reinterpret_cast<uintptr_t>(gate) & 15) return MDT_ERR_ARG;
   const int threads = ((D / 4 + 31) / 32) * 32;
-  const int rpb = gcd_int(rows_per_group, kGbRowsMax);
+  // deterministic: one block per sample (one writer per dgate address); the bias gradient sums over samples and this
+  // entry point has no scratch for per-sample rows
+  if (g_deterministic && dbias) return MDT_ERR_UNSUPPORTED;
+  const int rpb = g_deterministic ? rows_per_group : gcd_int(rows_per_group, kGbRowsMax);
   gate_bwd_kernel<<<M / rpb, threads, 0, S(stream)>>>(g, static_cast<const __nv_bfloat16*>(y_bf16), gate, ld_gate,
                                                       rows_per_group, static_cast<__nv_bfloat16*>(dy_bf16), dgate,
                                                       ld_dgate, dbias, M, D, rpb);
@@ -733,25 +945,9 @@ int mdt_ln_modulate_bwd_gate(const void* dxmod_bf16, const float* x, const float
                              float* dshift, float* dscale, int ld_dmod, const void* y_bf16, const float* gate,
                              int ld_gate, void* dy_bf16, float* dgate, int ld_dgate, float* dbias, int M, int D,
                              void* stream) {
-  if (!dxmod_bf16 || !x || !mean || !rstd || !scale || !g || !dshift || !dscale || M <= 0) return MDT_ERR_ARG;
-  if (rows_per_group <= 0 || M % rows_per_group || (ld_mod & 3) || (ld_dmod & 3)) return MDT_ERR_ARG;
-  if (y_bf16 && (!gate || !dy_bf16 || !dgate || (ld_gate & 3) || (ld_dgate & 3))) return MDT_ERR_ARG;
-  if ((reinterpret_cast<uintptr_t>(scale) | reinterpret_cast<uintptr_t>(dshift) | reinterpret_cast<uintptr_t>(dscale) |
-       reinterpret_cast<uintptr_t>(gate) | reinterpret_cast<uintptr_t>(dgate) | reinterpret_cast<uintptr_t>(dbias)) & 15)
-    return MDT_ERR_ARG;
-  if (D % 128 || D / 4 > kLgMaxThreads) return MDT_ERR_UNSUPPORTED;  // D <= 1280, as the LN kernels
-  const int rpb = gcd_int(rows_per_group, 32);
-  const int grid = M / rpb;
-  if (y_bf16)
-    ln_bwd_gate_kernel<true><<<grid, D / 4, 0, S(stream)>>>(
-        static_cast<const __nv_bfloat16*>(dxmod_bf16), x, mean, rstd, scale, ld_mod, rows_per_group, g, accumulate,
-        dshift, dscale, ld_dmod, static_cast<const __nv_bfloat16*>(y_bf16), gate, ld_gate,
-        static_cast<__nv_bfloat16*>(dy_bf16), dgate, ld_dgate, dbias, M, D, rpb);
-  else
-    ln_bwd_gate_kernel<false><<<grid, D / 4, 0, S(stream)>>>(
-        static_cast<const __nv_bfloat16*>(dxmod_bf16), x, mean, rstd, scale, ld_mod, rows_per_group, g, accumulate,
-        dshift, dscale, ld_dmod, nullptr, nullptr, 0, nullptr, nullptr, 0, nullptr, M, D, rpb);
-  return launch_status();
+  return ln_modulate_bwd_gate_s(dxmod_bf16, x, mean, rstd, scale, ld_mod, rows_per_group, g, accumulate, dshift, dscale,
+                                ld_dmod, y_bf16, gate, ld_gate, dy_bf16, dgate, ld_dgate, dbias, M, D, nullptr,
+                                S(stream));
 }
 
 int mdt_unmask_tokens(const float* u, const float* mask_token, const float* pos, const int64_t* ids_restore,
@@ -770,12 +966,7 @@ int mdt_unmask_tokens(const float* u, const float* mask_token, const float* pos,
 int mdt_unmask_tokens_bwd(const float* g, const int64_t* ids_keep, const int64_t* ids_restore, void* du_bf16,
                           float* dmask_token, int B, int T, int L, int D, void* stream) {
   (void)ids_keep;
-  if (!g || !du_bf16 || B <= 0 || T <= 0 || L <= 0 || D % 4 || D > 4096) return MDT_ERR_ARG;
-  if (!ids_restore && T != L) return MDT_ERR_ARG;
-  dim3 grid((L + kUmPos - 1) / kUmPos, B);
-  unmask_bwd_kernel<<<grid, ((D / 4 + 31) / 32) * 32, 0, S(stream)>>>(
-      g, ids_restore, static_cast<__nv_bfloat16*>(du_bf16), dmask_token, T, L, D);
-  return launch_status();
+  return unmask_tokens_bwd_s(g, ids_restore, du_bf16, dmask_token, B, T, L, D, nullptr, S(stream));
 }
 
 int mdt_gather_rows_bf16(const void* in_bf16, const int64_t* idx, void* out_bf16, int B, int T, int L, int D,

@@ -23,6 +23,7 @@
 // Reference ops this replaces: every nn.Linear of models/maskdit.py (timm Attention.qkv/proj, Mlp.fc1/fc2,
 // adaLN_modulation, DecoderLayer.linear, TimestepEmbedder.mlp, LabelEmbedder) and their autograd backward.
 #include "common.cuh"
+#include "deterministic.h"
 #include "gemm.h"
 #include "unit_sched.h"
 #include "wgmma.cuh"
@@ -503,9 +504,10 @@ static int launch(const mdt_gemm_args& a, cudaStream_t stream) {
   // k-slices: only for the accumulate epilogue (fp32 red.add).  Units = tiles x slices are dealt round robin to the
   // CTAs, so a launch lasts ceil(units / CTAs) unit-times; a unit costs its k-blocks plus a fixed part (pipeline fill,
   // the tile's reduction epilogue: ~4 k-blocks' worth).  Pick the slice count that minimises
-  // waves x (num_kb / slices + 4).
+  // waves x (num_kb / slices + 4).  Deterministic mode (mdt_set_deterministic): one slice, so every output element
+  // receives exactly one fp32 reduction per launch and its k order is fixed by the shape, whatever the SM count.
   int splits = 1;
-  if (a.epi == EPI_ATOMIC) {
+  if (a.epi == EPI_ATOMIC && !g_deterministic) {
     double best = 0.0;
     for (int c = 1; c <= 32 && c <= p.num_kb; ++c) {
       const long long u = static_cast<long long>(tiles) * c;

@@ -31,6 +31,11 @@ class BlockSpec:
 
 
 class Engine:
+    """Kernel-by-kernel reference of the step driver's launch sequence, for the default mode only: under
+    `mdt_set_deterministic(1)` the per-kernel entry points it calls for the patch-embedding, mask-token and fused
+    LN/gate bias gradients need scratch and return MDT_ERR_UNSUPPORTED (raised here), since only the step driver
+    (`CEngine`) carries that scratch in its workspace."""
+
     def __init__(self, cfg, store):
         self.cfg, self.store = cfg, store
         # dec_hidden == 0: the decoder-less DiT (use_decoder=False), final layer on the encoder width
@@ -407,6 +412,7 @@ class CEngine:
         T = ids_keep.shape[1] if ids_keep is not None else L
         for t, dt in ((x_in, f32), (sigma, f32), (labels, f32), (ids_keep, torch.int64), (ids_restore, torch.int64)):
             ops._c(t, dt)
+        ops.L.sync_deterministic()   # the workspace size and the backward's reductions follow the torch flag
         nbytes = self.workspace_bytes(B, T, save)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=x_in.device)   # ONE allocation per pass
         Fo = torch.empty(B * L, cfg.patch_dim, dtype=f32, device=x_in.device)
@@ -425,7 +431,8 @@ class CEngine:
         st = self.store
         st.ensure_grad()
         ops._c(dF16, bf16)
-        cb = ops.L.GRAD_READY_FN(lambda user, lo, hi: on_ready(lo, hi)) if on_ready is not None \
+        ops.L.sync_deterministic()
+        cb =ops.L.GRAD_READY_FN(lambda user, lo, hi: on_ready(lo, hi)) if on_ready is not None \
             else ops.L.GRAD_READY_FN()
         ops.check(self._L.mdt_backward(self._h, ops.ptr(st.w32), ops.ptr(st.w16), ops.ptr(st.grad), ops.ptr(ctx["x_in"]),
                                        ops.ptr(ctx["sigma"]), ops.ptr(ctx["ids_keep"]), ops.ptr(ctx["ids_restore"]),

@@ -294,8 +294,9 @@ class TrainStep:
         # keyed on the kept-token count (what shapes the launches), not on the float ratio: a schedule such as cos4
         # (configs/finetune/imagenet256-latent-cos.yaml) revisits few distinct T; at most 2 graphs are kept.
         L = self.net.model.num_patches
+        # the deterministic mode is part of the key: a captured graph replays the reductions it was captured with
         key = (tuple(images.shape), tuple(labels.shape), int(L * (1 - mask_ratio)) if mask_ratio > 0 else -1,
-               float(mae_loss_coef), bool(moments))
+               float(mae_loss_coef), bool(moments), ops.L.sync_deterministic())
         ent = self._graphs.get(key)
         if ent is None:
             while len(self._graphs) >= 2:
@@ -333,8 +334,11 @@ class TrainStep:
         (train.py:211-227 under accelerate's `gradient_accumulation_steps`): the wgrad kernels accumulate into the
         flat buffer anyway, so the rounds simply run back to back and 1/rounds is folded into the optimizer kernel.
         `moments=True`: `images` are VAE moments [B,2C,R,R] straight from the dataset; the latent sampling, the label
-        dropout (`class_dropout_prob`) and the noise injection run as the fused step-front kernel (EDMLoss.from_moments)."""
+        dropout (`class_dropout_prob`) and the noise injection run as the fused step-front kernel (EDMLoss.from_moments).
+        Under `torch.use_deterministic_algorithms(True)` the library's deterministic mode is on for the step
+        (`mdt_set_deterministic`): the gradients, and so the weights, moments and EMA, repeat bit for bit."""
         st = self.st
+        ops.L.sync_deterministic()
         if moments:
             base_loss = self.loss_fn
             pre = {}
