@@ -251,6 +251,34 @@ int mdt_adamw_ema_g16(float* w, const void* g_bf16, float* m, float* v, float* e
                       float lr, float beta1, float beta2, float eps, float weight_decay, int step, float ema_decay,
                       float grad_scale, int max_blocks, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Non-finite gradient guard: accelerate's GradScaler skips an optimizer step whose gradients hold an inf or NaN
+ * (train.py:39-48) while update_ema still runs (train.py:230).  The decision lives on the device, so a step needs
+ * no host synchronisation:
+ *   flag    one fp32 word, 0 = every checked element finite, 1 (or any non-zero) = skip.  The checks only ever store
+ *           1.0f, so repeated calls over chunks accumulate, and a SUM all-reduce of the ranks' flags is their OR.
+ *   counts  two int64 words {applied steps, skipped steps}, 8-byte aligned.
+ * mdt_nonfinite_check: flag = 1 if any of g[0, n) is inf or NaN (g 16-byte aligned; one read of g).
+ * mdt_cast_f32_bf16_check: mdt_cast_f32_bf16 (bit-identical output) that also sets the flag if a STORED bf16 value
+ *   is inf or NaN, i.e. also for a finite fp32 value beyond bf16's range (|x| >= 3.3961e38 rounds to inf).
+ * mdt_adamw_ema_guarded(_g16): with *flag == 0, mdt_adamw_ema(_g16) at step = counts[0] + 1 (the bias corrections are
+ *   computed on the device from the counter), bit for bit; with *flag != 0 only ema = d*ema + (1-d)*w, and w, m, v,
+ *   w_bf16 are not written.  Same arguments, alignment rules and grid as mdt_adamw_ema(_g16).  Neither reads or
+ *   writes the counters' values beyond counts[0], so every chunk of a step sees the same step number.
+ * mdt_optim_guard_advance: counts[*flag != 0] += 1 (one thread), enqueued once per step after its last guarded pass.
+ *   The flag is not cleared: the caller zeroes it before the next step's checks.
+ * ------------------------------------------------------------------------------------------------------------ */
+int mdt_nonfinite_check(const float* g, long long n, float* flag, void* stream);
+int mdt_cast_f32_bf16_check(const float* in, void* out_bf16, long long n, float* flag, void* stream);
+int mdt_adamw_ema_guarded(float* w, const float* g, float* m, float* v, float* ema, void* w_bf16, long long n,
+                          float lr, float beta1, float beta2, float eps, float weight_decay, float ema_decay,
+                          float grad_scale, const float* flag, const long long* counts, int max_blocks, void* stream);
+int mdt_adamw_ema_guarded_g16(float* w, const void* g_bf16, float* m, float* v, float* ema, void* w_bf16, long long n,
+                              float lr, float beta1, float beta2, float eps, float weight_decay, float ema_decay,
+                              float grad_scale, const float* flag, const long long* counts, int max_blocks,
+                              void* stream);
+int mdt_optim_guard_advance(const float* flag, long long* counts, void* stream);
+
 /* Cap on the SMs the persistent kernels (the wgmma GEMM) occupy: n > 0 sizes their grids
  * for n SMs instead of the device's count, leaving the rest to a concurrently running collective (the gradient
  * all-reduce overlapped with the backward); 0 = whole device.  Host-side setting, read at launch.                  */

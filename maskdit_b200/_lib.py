@@ -116,6 +116,12 @@ _SIGS = {
     "mdt_set_deterministic": [_I],
     "mdt_get_deterministic": [],
     "mdt_adamw_ema": [_P, _P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _F, _I, _F, _F, _I, _P],
+    # non-finite gradient guard (csrc/loss_optim.cu)
+    "mdt_nonfinite_check": [_P, _LL, _P, _P],
+    "mdt_cast_f32_bf16_check": [_P, _P, _LL, _P, _P],
+    "mdt_adamw_ema_guarded": [_P, _P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _F, _F, _F, _P, _P, _I, _P],
+    "mdt_adamw_ema_guarded_g16": [_P, _P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _F, _F, _F, _P, _P, _I, _P],
+    "mdt_optim_guard_advance": [_P, _P, _P],
 }
 
 

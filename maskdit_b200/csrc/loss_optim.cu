@@ -199,12 +199,13 @@ __global__ void to_uint8_nhwc_kernel(const float* __restrict__ img, unsigned cha
   out[i] = static_cast<unsigned char>(v);  // truncation, as .to(torch.uint8)
 }
 
-// Fused AdamW + EMA + bf16 shadow, float4-vectorised over flat buffers.
+// Fused AdamW + EMA + bf16 shadow, float4-vectorised over flat buffers.  One pass of the grid-stride loop; the
+// unguarded and the guarded kernel share it, so a guarded step with a clear flag computes the same bits.
 template <bool G16>  // G16: the gradient operand is bf16 (the buffer a bf16 all-reduce produced), else fp32
-__global__ void __launch_bounds__(256)
-adamw_ema_kernel(float* __restrict__ w, const void* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
-                 float* __restrict__ ema, __nv_bfloat16* __restrict__ w16, long long n, float lr, float b1, float b2,
-                 float eps, float wd, float inv_bc1, float inv_bc2, float ema_decay, float gscale) {
+MDT_DEVINL void adamw_ema_pass(float* __restrict__ w, const void* __restrict__ g, float* __restrict__ m,
+                               float* __restrict__ v, float* __restrict__ ema, __nv_bfloat16* __restrict__ w16,
+                               long long n, float lr, float b1, float b2, float eps, float wd, float inv_bc1,
+                               float inv_bc2, float ema_decay, float gscale) {
   const long long n4 = n >> 2;
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n4; i += stride) {
@@ -241,6 +242,98 @@ adamw_ema_kernel(float* __restrict__ w, const void* __restrict__ g, float* __res
     }
     if (w16) reinterpret_cast<uint2*>(w16)[i] = make_uint2(pack_bf16(wv.x, wv.y), pack_bf16(wv.z, wv.w));
   }
+}
+
+template <bool G16>
+__global__ void __launch_bounds__(256)
+adamw_ema_kernel(float* __restrict__ w, const void* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+                 float* __restrict__ ema, __nv_bfloat16* __restrict__ w16, long long n, float lr, float b1, float b2,
+                 float eps, float wd, float inv_bc1, float inv_bc2, float ema_decay, float gscale) {
+  adamw_ema_pass<G16>(w, g, m, v, ema, w16, n, lr, b1, b2, eps, wd, inv_bc1, inv_bc2, ema_decay, gscale);
+}
+
+// ---- Non-finite gradient guard (GradScaler's inf-skip, train.py:39-48,230) --------------------------------------------
+MDT_DEVINL bool nonfinite_f32(float x) { return (__float_as_uint(x) & 0x7f800000u) == 0x7f800000u; }
+MDT_DEVINL bool nonfinite_bf16x2(uint32_t u) {   // either bf16 half of the word has an all-ones exponent
+  return (u & 0x7f800000u) == 0x7f800000u || (u & 0x7f80u) == 0x7f80u;
+}
+// One warp vote per warp; lanes that saw a non-finite element set the flag (every writer stores the same 1.0f, so the
+// unordered stores are an OR).  The flag is fp32 so that a SUM all-reduce of the per-rank flags is their OR.
+MDT_DEVINL void flag_or(bool bad, float* flag) {
+  if (__any_sync(0xffffffffu, bad) && (threadIdx.x & 31) == 0) *flag = 1.f;
+}
+
+__global__ void __launch_bounds__(256) nonfinite_check_kernel(const float* __restrict__ g, long long n,
+                                                              float* __restrict__ flag) {
+  const long long n4 = n >> 2;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  const long long t = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  bool bad = false;
+  for (long long i = t; i < n4; i += stride) {
+    const float4 v = reinterpret_cast<const float4*>(g)[i];
+    bad |= nonfinite_f32(v.x) | nonfinite_f32(v.y) | nonfinite_f32(v.z) | nonfinite_f32(v.w);
+  }
+  for (long long i = (n4 << 2) + t; i < n; i += stride) bad |= nonfinite_f32(g[i]);
+  flag_or(bad, flag);
+}
+
+// mdt_cast_f32_bf16's arithmetic (same rounding, same output bits) plus the check, on the bf16 values it stores.
+__global__ void __launch_bounds__(256) cast_f32_bf16_check_kernel(const float* __restrict__ in,
+                                                                  __nv_bfloat16* __restrict__ out, long long n,
+                                                                  float* __restrict__ flag) {
+  const long long n4 = n >> 2;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  const long long t = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  const float4* in4 = reinterpret_cast<const float4*>(in);
+  uint2* out2 = reinterpret_cast<uint2*>(out);
+  bool bad = false;
+  for (long long i = t; i < n4; i += stride) {
+    float4 v = in4[i];
+    const uint2 o = make_uint2(pack_bf16(v.x, v.y), pack_bf16(v.z, v.w));
+    out2[i] = o;
+    bad |= nonfinite_bf16x2(o.x) | nonfinite_bf16x2(o.y);
+  }
+  for (long long i = (n4 << 2) + t; i < n; i += stride) {
+    const __nv_bfloat16 b = __float2bfloat16_rn(in[i]);
+    out[i] = b;
+    bad |= nonfinite_f32(__bfloat162float(b));
+  }
+  flag_or(bad, flag);
+}
+
+// Adam's step number of this step: the applied-step counter + 1, as the bias corrections of adamw_launch compute it.
+template <bool G16>
+__global__ void __launch_bounds__(256)
+adamw_ema_guarded_kernel(float* __restrict__ w, const void* __restrict__ g, float* __restrict__ m,
+                         float* __restrict__ v, float* __restrict__ ema, __nv_bfloat16* __restrict__ w16, long long n,
+                         float lr, float b1, float b2, float eps, float wd, float ema_decay, float gscale,
+                         const float* __restrict__ flag, const long long* __restrict__ counts) {
+  if (*flag != 0.f) {   // skipped step: only the EMA moves, toward the unchanged weights
+    if (!ema) return;
+    const long long n4 = n >> 2;
+    const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n4; i += stride) {
+      const float4 wv = reinterpret_cast<const float4*>(w)[i];
+      float4 ev = reinterpret_cast<float4*>(ema)[i];
+      ev.x = ema_decay * ev.x + (1.f - ema_decay) * wv.x, ev.y = ema_decay * ev.y + (1.f - ema_decay) * wv.y;
+      ev.z = ema_decay * ev.z + (1.f - ema_decay) * wv.z, ev.w = ema_decay * ev.w + (1.f - ema_decay) * wv.w;
+      reinterpret_cast<float4*>(ema)[i] = ev;
+    }
+    return;
+  }
+  __shared__ float s_bc[2];
+  if (threadIdx.x == 0) {
+    const double step = static_cast<double>(counts[0] + 1);
+    s_bc[0] = static_cast<float>(1.0 / (1.0 - pow(static_cast<double>(b1), step)));
+    s_bc[1] = static_cast<float>(1.0 / (1.0 - pow(static_cast<double>(b2), step)));
+  }
+  __syncthreads();
+  adamw_ema_pass<G16>(w, g, m, v, ema, w16, n, lr, b1, b2, eps, wd, s_bc[0], s_bc[1], ema_decay, gscale);
+}
+
+// counts = {applied steps, skipped steps}: one of them advances per optimizer step, after its last guarded pass.
+__global__ void optim_guard_advance_kernel(const float* __restrict__ flag, long long* __restrict__ counts) {
+  counts[*flag != 0.f ? 1 : 0] += 1;
 }
 
 
@@ -397,6 +490,70 @@ int mdt_adamw_ema_g16(float* w, const void* g_bf16, float* m, float* v, float* e
                       float grad_scale, int max_blocks, void* stream) {
   return adamw_launch(true, w, g_bf16, m, v, ema, w_bf16, n, lr, beta1, beta2, eps, weight_decay, step, ema_decay,
                       grad_scale, max_blocks, stream);
+}
+
+static int check_grid(long long n) {   // the grid of mdt_cast_f32_bf16: 4 elements per thread, <= 16 CTAs per SM
+  long long blocks = (n / 4 + 255) / 256;
+  if (blocks < 1) blocks = 1;
+  if (blocks > kNumSMsDefault * 16) blocks = kNumSMsDefault * 16;
+  return static_cast<int>(blocks);
+}
+
+int mdt_nonfinite_check(const float* g, long long n, float* flag, void* stream) {
+  if (!g || !flag || n <= 0 || (reinterpret_cast<uintptr_t>(g) & 15)) return MDT_ERR_ARG;
+  nonfinite_check_kernel<<<check_grid(n), 256, 0, S(stream)>>>(g, n, flag);
+  return launch_status();
+}
+
+int mdt_cast_f32_bf16_check(const float* in, void* out_bf16, long long n, float* flag, void* stream) {
+  if (!in || !out_bf16 || !flag || n <= 0) return MDT_ERR_ARG;
+  if ((reinterpret_cast<uintptr_t>(in) & 15) || (reinterpret_cast<uintptr_t>(out_bf16) & 7)) return MDT_ERR_ARG;
+  cast_f32_bf16_check_kernel<<<check_grid(n), 256, 0, S(stream)>>>(in, static_cast<__nv_bfloat16*>(out_bf16), n,
+                                                                    flag);
+  return launch_status();
+}
+
+static int adamw_guarded_launch(bool g16, float* w, const void* g, float* m, float* v, float* ema, void* w_bf16,
+                                long long n, float lr, float beta1, float beta2, float eps, float weight_decay,
+                                float ema_decay, float grad_scale, const float* flag, const long long* counts,
+                                int max_blocks, void* stream) {
+  if (!w || !g || !m || !v || !flag || !counts || n <= 0 || (n & 3)) return MDT_ERR_ARG;
+  const uintptr_t a16 = reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(m) |
+                        reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(ema) |
+                        (g16 ? 0 : reinterpret_cast<uintptr_t>(g));
+  const uintptr_t a8 = reinterpret_cast<uintptr_t>(w_bf16) | (g16 ? reinterpret_cast<uintptr_t>(g) : 0) |
+                       reinterpret_cast<uintptr_t>(counts);
+  if ((a16 & 15) || (a8 & 7) || (reinterpret_cast<uintptr_t>(flag) & 3)) return MDT_ERR_ARG;
+  long long blocks = (n / 4 + 255) / 256;
+  if (blocks > kNumSMsDefault * 8) blocks = kNumSMsDefault * 8;
+  if (max_blocks > 0 && blocks > max_blocks) blocks = max_blocks;
+  auto kern = g16 ? adamw_ema_guarded_kernel<true> : adamw_ema_guarded_kernel<false>;
+  kern<<<static_cast<int>(blocks), 256, 0, S(stream)>>>(w, g, m, v, ema, static_cast<__nv_bfloat16*>(w_bf16), n, lr,
+                                                        beta1, beta2, eps, weight_decay, ema_decay, grad_scale, flag,
+                                                        counts);
+  return launch_status();
+}
+
+int mdt_adamw_ema_guarded(float* w, const float* g, float* m, float* v, float* ema, void* w_bf16, long long n,
+                          float lr, float beta1, float beta2, float eps, float weight_decay, float ema_decay,
+                          float grad_scale, const float* flag, const long long* counts, int max_blocks, void* stream) {
+  return adamw_guarded_launch(false, w, g, m, v, ema, w_bf16, n, lr, beta1, beta2, eps, weight_decay, ema_decay,
+                              grad_scale, flag, counts, max_blocks, stream);
+}
+
+int mdt_adamw_ema_guarded_g16(float* w, const void* g_bf16, float* m, float* v, float* ema, void* w_bf16, long long n,
+                              float lr, float beta1, float beta2, float eps, float weight_decay, float ema_decay,
+                              float grad_scale, const float* flag, const long long* counts, int max_blocks,
+                              void* stream) {
+  return adamw_guarded_launch(true, w, g_bf16, m, v, ema, w_bf16, n, lr, beta1, beta2, eps, weight_decay, ema_decay,
+                              grad_scale, flag, counts, max_blocks, stream);
+}
+
+int mdt_optim_guard_advance(const float* flag, long long* counts, void* stream) {
+  if (!flag || !counts || (reinterpret_cast<uintptr_t>(counts) & 7) || (reinterpret_cast<uintptr_t>(flag) & 3))
+    return MDT_ERR_ARG;
+  optim_guard_advance_kernel<<<1, 1, 0, S(stream)>>>(flag, counts);
+  return launch_status();
 }
 
 int mdt_step_front(const float* moments, const float* eps, const float* rnd_normal, const float* noise_unit,

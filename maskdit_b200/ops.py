@@ -248,3 +248,35 @@ def adamw_ema(w, g, m, v, ema, w16, n, lr, step, beta1=0.9, beta2=0.999, eps=1e-
     fn = lib().mdt_adamw_ema_g16 if g.dtype == bf16 else lib().mdt_adamw_ema   # bf16: all-reduced bf16 gradients
     check(fn(ptr(w), ptr(g), ptr(m), ptr(v), ptr(ema), ptr(w16), n, lr, beta1, beta2, eps, weight_decay, step,
              ema_decay, grad_scale, max_blocks, stream_ptr()), "mdt_adamw_ema")
+
+
+# -- non-finite gradient guard: `flag` is one fp32 word (0 = finite), `counts` int64 {applied steps, skipped steps} --
+def nonfinite_check(g, flag):
+    """flag = 1 if any element of the fp32 tensor g is inf or NaN; leaves it alone otherwise (calls accumulate)."""
+    _c(g, f32), _c(flag, f32)
+    check(lib().mdt_nonfinite_check(ptr(g), g.numel(), ptr(flag), stream_ptr()), "mdt_nonfinite_check")
+
+
+def cast_bf16_check(x, flag, out=None):
+    """`cast_bf16` (same bits) that also sets `flag` if a stored bf16 value is inf or NaN."""
+    _c(x, f32), _c(flag, f32), _c(out, bf16)
+    if out is None:
+        out = torch.empty(x.shape, dtype=bf16, device=x.device)
+    check(lib().mdt_cast_f32_bf16_check(ptr(x), ptr(out), x.numel(), ptr(flag), stream_ptr()),
+          "mdt_cast_f32_bf16_check")
+    return out
+
+
+def adamw_ema_guarded(w, g, m, v, ema, w16, n, lr, flag, counts, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0,
+                      ema_decay=0.9999, grad_scale=1.0, max_blocks=0):
+    """`adamw_ema` at step counts[0] + 1 when flag == 0; only the EMA update when flag != 0."""
+    _c(flag, f32), _c(counts, torch.int64)
+    fn = lib().mdt_adamw_ema_guarded_g16 if g.dtype == bf16 else lib().mdt_adamw_ema_guarded
+    check(fn(ptr(w), ptr(g), ptr(m), ptr(v), ptr(ema), ptr(w16), n, lr, beta1, beta2, eps, weight_decay, ema_decay,
+             grad_scale, ptr(flag), ptr(counts), max_blocks, stream_ptr()), "mdt_adamw_ema_guarded")
+
+
+def optim_guard_advance(flag, counts):
+    """counts[1 if flag else 0] += 1: once per step, after its last guarded optimizer pass."""
+    _c(flag, f32), _c(counts, torch.int64)
+    check(lib().mdt_optim_guard_advance(ptr(flag), ptr(counts), stream_ptr()), "mdt_optim_guard_advance")

@@ -106,8 +106,16 @@ class TrainStep:
     def __init__(self, net: EDMPrecond, ema: EDMPrecond | None = None, lr=1e-4, betas=(0.9, 0.999), eps=1e-8,
                  weight_decay=0.0, ema_decay=0.9999, loss_fn: EDMLoss | None = None, process_group=None,
                  lr_rampup_kimg=0.0, global_batch=None, device=None, overlap=False, graph=None,
-                 reference_lr_schedule=False, collective=None, grad_dtype=None, comm_ctas=None):
-        """Multi-GPU options (world > 1; SURVEY 8e: the step's ONLY collective is the sum of the flat gradient buffer):
+                 reference_lr_schedule=False, collective=None, grad_dtype=None, comm_ctas=None, skip_nonfinite=False):
+        """skip_nonfinite: skip every optimizer step whose gradient holds an inf or NaN, as the reference's fp16
+        GradScaler does (train.py:39-48): the weights, the bf16 shadow, the moments and Adam's step count stay as they
+        are, the EMA still moves toward the unchanged weights (train.py:230), and the lr schedule's counter
+        (`step_count`) advances as for any attempted step.  The gradient checked is the one the optimizer consumes
+        (the summed one at world > 1; with bf16 exchange the bf16 values, checked while they are cast).  The decision
+        is a device flag that every rank ORs in (no host synchronisation); Adam's step count lives on the device
+        (`applied_steps()`), the number of skipped steps in `skipped_steps`.  Off by default: the step is then
+        exactly the unguarded one.
+        Multi-GPU options (world > 1; SURVEY 8e: the step's ONLY collective is the sum of the flat gradient buffer):
           collective  'mdt' (default with an NCCL process group): our own communicator behind the C ABI (`GradComm`);
                       'torch': `torch.distributed.all_reduce` on the process group (gloo tests, A/B).
           grad_dtype  'bf16' (default, SURVEY 8e): the fp32 gradient buffer is cast to a bf16 exchange buffer, 1.46 GB cross
@@ -174,6 +182,21 @@ class TrainStep:
         self._done = []          # [lo, hi) ranges already handled in the current step
         self._lr_now = lr
         net._grad_ready_hook = self._on_grads_ready if (self.overlap and self.world > 1) else None
+        # non-finite guard: flag (fp32, 0 = finite; a SUM over the ranks is their OR), counts {applied, skipped}
+        self.skip_nonfinite = bool(skip_nonfinite)
+        self._flag = torch.zeros(1, dtype=torch.float32, device=dev) if self.skip_nonfinite else None
+        self._counts = torch.zeros(2, dtype=torch.int64, device=dev) if self.skip_nonfinite else None
+
+    @property
+    def skipped_steps(self):
+        """Device tensor (int64, 0-dim): optimizer steps skipped for non-finite gradients since this object was built
+        (None without `skip_nonfinite`).  Reading its value synchronises; the step itself never does."""
+        return self._counts[1] if self._counts is not None else None
+
+    def applied_steps(self) -> int:
+        """Adam's step count: the steps whose update was applied (a host read of the device counter under
+        `skip_nonfinite`, i.e. one synchronisation; `step_count` otherwise)."""
+        return int(self._counts[0]) if self._counts is not None else self.step_count
 
     # -- optimizer state for checkpoints (reference: train.py:259-270 stores optimizer.state_dict() under 'opt') ------
     def state_dict(self):
@@ -182,19 +205,21 @@ class TrainStep:
         (pos_embed = 0, decoder_pos_embed = 1) keep their index but own no state, so the first key is 2 (1 for the
         decoder-less DiT, whose only frozen tensor is pos_embed) — with
         `exp_avg` / `exp_avg_sq` and a per-parameter `step` (torch layout); the step count is also stored in the
-        param_group (apex layout).  Tensors are copies on the current device."""
+        param_group (apex layout).  Tensors are copies on the current device.  The step count is Adam's
+        (`applied_steps()`): under `skip_nonfinite` it leaves out the skipped steps."""
         state, n_all = {}, 0
+        adam_step = self.applied_steps()
         for i, (k, p) in enumerate(self.net.named_parameters()):
             n_all = i + 1
             if not p.requires_grad:
                 continue
             lo, _, shape = self.st.offsets[k]
             n = p.numel()
-            state[i] = {"step": torch.tensor(float(self.step_count)), "exp_avg": self.m[lo:lo + n].view(shape).clone(),
+            state[i] = {"step": torch.tensor(float(adam_step)), "exp_avg": self.m[lo:lo + n].view(shape).clone(),
                         "exp_avg_sq": self.v[lo:lo + n].view(shape).clone()}
         return {"state": state,
                 "param_groups": [{"lr": self.lr, "betas": self.betas, "eps": self.eps, "weight_decay": self.wd,
-                                  "step": self.step_count, "params": list(range(n_all))}]}
+                                  "step": adam_step, "params": list(range(n_all))}]}
 
     def load_state_dict(self, sd):
         """Accepts (a) this class's own layout, (b) `torch.optim.AdamW(model.parameters()).state_dict()`, (c) apex
@@ -230,6 +255,8 @@ class TrainStep:
         if step is None:
             raise ValueError("optimizer state carries no step count (neither per parameter nor in the param_group)")
         self.step_count = int(float(step))
+        if self._counts is not None:   # Adam continues from the stored count; the skip tally is this object's own
+            self._counts[0].fill_(self.step_count)
         self.lr, self.betas, self.eps, self.wd = group["lr"], tuple(group["betas"]), group["eps"], \
             group["weight_decay"]
 
@@ -252,26 +279,40 @@ class TrainStep:
             if self.ar_chunks > 1 else "one flat call after the backward")
         return f"{self.grad_dtype} sum-all-reduce of the flat gradient buffer, {how}, {when}"
 
-    def _exchange(self, lo, hi, background=False):
-        """Sum gradient elements [lo, hi) over the ranks on the current stream (in `grad`, or in the bf16 buffer)."""
-        if hi <= lo or self.world == 1:
-            return
-        st = self.st
-        buf = st.grad[lo:hi]
-        if self.g16 is not None:
-            buf = ops.cast_bf16(buf, out=self.g16[lo:hi])
+    def _cast(self, lo, hi):
+        """fp32 gradient [lo, hi) -> the bf16 exchange buffer; under the guard the cast also checks what it stores."""
+        if self._flag is not None:
+            return ops.cast_bf16_check(self.st.grad[lo:hi], self._flag, out=self.g16[lo:hi])
+        return ops.cast_bf16(self.st.grad[lo:hi], out=self.g16[lo:hi])
+
+    def _all_reduce(self, buf, background=False):
         if self.comm is not None:
             (self.comm_bg if (background and self.comm_bg is not None) else self.comm).all_reduce(buf)
         else:
             dist.all_reduce(buf, op=dist.ReduceOp.SUM, group=self.pg)
+
+    def _exchange(self, lo, hi, background=False, cast=True):
+        """Sum gradient elements [lo, hi) over the ranks on the current stream (in `grad`, or in the bf16 buffer;
+        cast=False: the bf16 buffer already holds this range's cast)."""
+        if hi <= lo or self.world == 1:
+            return
+        buf = self.st.grad[lo:hi]
+        if self.g16 is not None:
+            buf = self._cast(lo, hi) if cast else self.g16[lo:hi]
+        self._all_reduce(buf, background)
 
     def _step_range(self, lo, hi, max_blocks=0):
         st, n = self.st, hi - lo
         if n <= 0:
             return
         g = self.g16[lo:hi] if (self.g16 is not None and self.world > 1) else st.grad[lo:hi]
-        ops.adamw_ema(st.w32[lo:hi], g, self.m[lo:hi], self.v[lo:hi],
-                      self.ema_st.w32[lo:hi] if self.ema_st is not None else None, st.w16[lo:hi], n, self._lr_now,
+        ema = self.ema_st.w32[lo:hi] if self.ema_st is not None else None
+        if self._flag is not None:   # Adam's step number comes from the device counter, the skip from the flag
+            ops.adamw_ema_guarded(st.w32[lo:hi], g, self.m[lo:hi], self.v[lo:hi], ema, st.w16[lo:hi], n, self._lr_now,
+                                  self._flag, self._counts, self.betas[0], self.betas[1], self.eps, self.wd,
+                                  self.ema_decay, self._grad_scale, max_blocks)
+            return
+        ops.adamw_ema(st.w32[lo:hi], g, self.m[lo:hi], self.v[lo:hi], ema, st.w16[lo:hi], n, self._lr_now,
                       self.step_count, self.betas[0], self.betas[1], self.eps, self.wd, self.ema_decay,
                       self._grad_scale, max_blocks)
 
@@ -362,6 +403,9 @@ class TrainStep:
         self._lr_now = lr_at(self.step_count + self.lr_step_offset, self.lr, gb, self.rampup) \
             if self.reference_lr_schedule else self.lr
         self.step_count += 1
+        guard = self._flag is not None
+        if guard:
+            self._flag.zero_()
         self._done = []
         self._grad_scale = 1.0 / (self.world * grad_accum)
         if grad_accum > 1:
@@ -385,28 +429,45 @@ class TrainStep:
             loss = loss_call(self.net, images, labels, mask_ratio, mae_loss_coef)
             loss.mean().backward()   # engine backward; with overlap=True block ranges are already being reduced/stepped
         main = torch.cuda.current_stream()
+        n = st.n_train
+        # Under the guard the flag must be final before the first optimizer pass.  bf16 exchange: the casts check the
+        # local values and one word is then summed over the ranks.  fp32 exchange: the summed buffer is checked,
+        # except in the chunked pipeline, which checks the local gradients up front and sums the flag.
         if self.overlap and self._done:
             ops.check(ops.lib().mdt_set_sm_budget(0), "mdt_set_sm_budget", 0)
             self.side.wait_stream(main)
             with torch.cuda.stream(self.side):
                 cur = 0
-                for lo, hi in sorted(self._done) + [(st.n_train, st.n_train)]:   # the complement of the block ranges
+                for lo, hi in sorted(self._done) + [(n, n)]:   # the complement of the block ranges
                     self._exchange(cur, lo)
                     cur = max(cur, hi)
+                if guard and self.g16 is not None:
+                    self._all_reduce(self._flag)
             main.wait_stream(self.side)
-            self._step_range(0, st.n_train)          # ONE optimizer pass over the whole (reduced) buffer
+            if guard and self.g16 is None:
+                ops.nonfinite_check(st.grad[:n], self._flag)
+            self._step_range(0, n)                   # ONE optimizer pass over the whole (reduced) buffer
         elif self.world == 1:
-            self._step_range(0, st.n_train)
+            if guard:
+                ops.nonfinite_check(st.grad[:n], self._flag)
+            self._step_range(0, n)
         elif self.ar_chunks > 1:
             # pipeline the exposed all-reduce against the optimizer pass: chunk k is stepped while k+1 is on the wire
             if self.side is None:
                 self.side = torch.cuda.Stream(device=st.grad.device)
-            bounds = ar_chunk_bounds(st.n_train, self.ar_chunks)
+            bounds = ar_chunk_bounds(n, self.ar_chunks)
             self.side.wait_stream(main)
             evs = []
             with torch.cuda.stream(self.side):
+                if guard:   # chunk 0's optimizer pass needs the decision: check every local chunk first
+                    if self.g16 is not None:
+                        for lo, hi in bounds:
+                            self._cast(lo, hi)
+                    else:
+                        ops.nonfinite_check(st.grad[:n], self._flag)
+                    self._all_reduce(self._flag)
                 for lo, hi in bounds:
-                    self._exchange(lo, hi)
+                    self._exchange(lo, hi, cast=not guard)
                     ev = torch.cuda.Event()
                     ev.record(self.side)
                     evs.append(ev)
@@ -414,8 +475,15 @@ class TrainStep:
                 main.wait_event(ev)
                 self._step_range(lo, hi)
         else:
-            self._exchange(0, st.n_train)            # one flat all-reduce ...
-            self._step_range(0, st.n_train)          # ... + one optimizer pass
+            self._exchange(0, n)                     # one flat all-reduce ...
+            if guard:
+                if self.g16 is not None:
+                    self._all_reduce(self._flag)
+                else:
+                    ops.nonfinite_check(st.grad[:n], self._flag)
+            self._step_range(0, n)                   # ... + one optimizer pass
+        if guard:
+            ops.optim_guard_advance(self._flag, self._counts)
         st.mark_shadow_fresh(self.net._params())   # the kernel refreshed the bf16 shadow itself
         if self.ema_st is not None:
             self.ema_st._versions = None           # EMA weights changed behind PyTorch's back: shadow is stale

@@ -5,8 +5,9 @@ the H100 engine.  Launch one process per GPU:
     torchrun --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 train.py --config <yaml> [--synthetic]
 
 Differences from the reference driver, all outside the arithmetic: PyYAML instead of OmegaConf; torchrun instead of
-`accelerate launch`; bf16 GEMM operands instead of fp16 AMP + GradScaler (`--no_amp` is accepted and ignored: there
-is one precision recipe); the DDP wrapper + apex FusedAdam + EMA loop are replaced by `TrainStep` (single flat
+`accelerate launch`; bf16 GEMM operands instead of fp16 AMP + GradScaler (there is one precision recipe and no loss
+scaling, but GradScaler's skip of steps with inf / NaN gradients is kept: `TrainStep(skip_nonfinite=True)` unless
+`--no_amp` is given, where the reference has no GradScaler either); the DDP wrapper + apex FusedAdam + EMA loop are replaced by `TrainStep` (single flat
 all-reduce, fused AdamW+EMA); wandb / FID-during-training are not wired (SURVEY.md §2: out of scope).
 Data: the reference's LMDB latent dataset (`data.root`/train: keys z-{i} / y-{i} / length, train_utils/datasets.py:
 240-304) through `maskdit_b200.data` (liblmdb when the `lmdb` module exists, otherwise a read-only page walker of
@@ -45,7 +46,13 @@ def synthetic_loader(cfg, batch, device, seed):
         yield moments, labels
 
 
-def main():
+def skip_nonfinite(args):
+    """The reference wraps every optimizer step in GradScaler unless --no_amp is given (train.py:39-42); its skip of
+    steps with non-finite gradients follows the same switch."""
+    return not args.no_amp
+
+
+def build_parser():
     ap = argparse.ArgumentParser("training parameters")
     ap.add_argument("--config", required=True)
     ap.add_argument("--results_dir", default="results")
@@ -65,7 +72,11 @@ def main():
     ap.add_argument("--wds", action="store_true",
                     help="data.root holds WebDataset .tar shards (the reference's train_wds.py twin: lmdb2wds.py layout)")
     ap.add_argument("--max_steps", type=int, default=None, help="stop after this many steps (smoke runs)")
-    args, _ = ap.parse_known_args()
+    return ap
+
+
+def main():
+    args, _ = build_parser().parse_known_args()
     cfg = load_config(args.config)
 
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
@@ -95,7 +106,8 @@ def main():
         ema.load_state_dict({k.replace("_orig_mod.", ""): v for k, v in sd["ema"].items()}, strict=strict)
         step0 = int(os.path.basename(ck)[:-3]) if os.path.basename(ck)[:-3].isdigit() else 0
     ts = TrainStep(net, ema, lr=cfg.train.lr, lr_rampup_kimg=cfg.train.lr_rampup_kimg, global_batch=global_batch,
-                   loss_fn=Losses[cfg.model.precond](), reference_lr_schedule=True)
+                   loss_fn=Losses[cfg.model.precond](), reference_lr_schedule=True,
+                   skip_nonfinite=skip_nonfinite(args))
     if ck and strict and "opt" in sd:                      # train.py:150: optimizer state only under strict loading
         ts.load_state_dict(sd["opt"])
     ts.lr_step_offset = step0 - ts.step_count              # lr follows the run's step counter (train.py:223)
@@ -140,8 +152,10 @@ def main():
                 avg = avg / world
             torch.cuda.synchronize()
             if rank == 0:
+                # every rank takes the same skip decisions, so rank 0's tally is the run's
+                skipped = f", Skipped Steps: {int(ts.skipped_steps)}" if ts.skipped_steps is not None else ""
                 print(f"(step={step:07d}) Train Loss: {float(avg):.4f}, Train Steps/Sec: "
-                      f"{log_steps / (time.time() - t0):.2f}", flush=True)
+                      f"{log_steps / (time.time() - t0):.2f}{skipped}", flush=True)
             running, log_steps, t0 = 0.0, 0, time.time()
         if step % cfg.log.ckpt_every == 0 and step > step0:
             if rank == 0:
