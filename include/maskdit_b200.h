@@ -336,8 +336,22 @@ int mdt_model_num_tensors(const mdt_model* m);
 int mdt_model_param_info(const mdt_model* m, int i, char* name, int name_cap, long long* offset, long long* numel);
 int mdt_model_mod_width(const mdt_model* m); /* columns of the concatenated adaLN modulation vector                   */
 
+/* Activation recomputation (gradient checkpointing) of the training pass: the first r blocks in forward order (encoder
+ * blocks 0..depth-1, then decoder blocks) keep only their output residual (4 bytes per row and channel instead of about
+ * 42); their other activations share one recompute slot sized for the largest of them, and mdt_backward re-runs each
+ * such block's forward into the slot from its stored input (the adaLN modulation stays resident) before reading them.
+ * The forward kernels neither split K nor use atomics, so the gradients are those of r = 0 bit for bit under the
+ * deterministic mode.  0 <= r <= depth + dec_depth (MDT_ERR_ARG otherwise), default 0 (nothing recomputed, the plan
+ * and launches of a handle without this setting).  Host-side setting of the handle, read by mdt_workspace_bytes
+ * (training), mdt_forward (save = 1) and mdt_backward; the inference plan ignores it.  mdt_backward refuses
+ * (MDT_ERR_ARG) a workspace laid out for another count: at r > 0 anything but the workspace of the handle's last
+ * mdt_forward(save = 1) at the same r, at r = 0 the workspace of a last saving forward that recomputed.              */
+int mdt_model_set_recompute(mdt_model* m, int r);
+int mdt_model_get_recompute(const mdt_model* m); /* -1 for a NULL handle */
+
 /* Workspace bytes for batch B with T kept tokens per sample (T <= 0: no token dropping, T = L).
- * training != 0: every activation the backward needs stays resident (+ the backward's scratch); else inference.       */
+ * training != 0: every activation the backward needs stays resident (+ the backward's scratch; with recomputation only
+ * the recomputed blocks' output residuals and the slot); else inference.                                              */
 long long mdt_workspace_bytes(const mdt_model* m, int B, int T, int training);
 
 /* F [B*L, p*p*C] f32 = DiT.forward on x_in [B,C,R,R] (UNscaled network input, c_in applied inside), sigma [B],

@@ -96,6 +96,8 @@ _SIGS = {
     "mdt_model_num_tensors": [_P],
     "mdt_model_param_info": [_P, _I, c_char_p, _I, POINTER(c_longlong), POINTER(c_longlong)],
     "mdt_model_mod_width": [_P],
+    "mdt_model_set_recompute": [_P, _I],
+    "mdt_model_get_recompute": [_P],
     "mdt_forward": [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _LL, _P, _P],
     "mdt_backward": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _P, _LL, GRAD_READY_FN, _P, _P],
     "mdt_nccl_unique_id": [_P],

@@ -66,6 +66,11 @@ struct mdt_model {
   i64 n_train, n_total;
   std::vector<NamedTensor> named;  // registration order
   std::vector<int> order;          // blob order (indices into named)
+  int recompute = 0;               // blocks whose activations the backward recomputes (mdt_model_set_recompute)
+  // the workspace of the last mdt_forward(save = 1) and the recompute count it was laid out for: mdt_backward refuses
+  // to read a workspace with another count's plan
+  mutable const void* fwd_ws = nullptr;
+  mutable int fwd_r = 0;
 };
 
 namespace {
@@ -186,10 +191,18 @@ struct Plan {
   i64 total;
 };
 
+// Training plan with recomputation (mdt_model_set_recompute, r > 0): the first r blocks in forward order (encoder blocks
+// first, then decoder blocks) keep only their output residual X2, the next block's input.  Their other slices all point
+// into ONE recompute slot, laid out after the final layer's slices, as large per slice as the largest recomputed block's
+// (plus a second mean1 / rstd1, see mdt_backward).  mdt_forward writes a recomputed block's activations into the slot;
+// mdt_backward re-runs the block's forward there from its stored input before reading them.
 Plan make_plan(const mdt_model* m, int B, int T, bool save, bool with_backward) {
   Plan p;
   Arena a;
   const int D = m->D, Dd = m->Dd, L = m->L, NA = m->NA;
+  const int r = save ? m->recompute : 0;
+  i64 need_md = 0, need_m = 0, need_mh = 0, need_lse = 0;  // slot: largest M * dim, M, M * mlp hidden, lse bytes
+  auto grow = [](i64& n, i64 v) { n = v > n ? v : n; };
   const i64 Me = static_cast<i64>(B) * T, Md = static_cast<i64>(B) * L;
   p.X0 = a.take(Me * D * 4);
   p.tf = a.take(B * 256ll * 2);
@@ -202,13 +215,18 @@ Plan make_plan(const mdt_model* m, int B, int T, bool save, bool with_backward) 
   p.wyp = a.take(static_cast<i64>(D) * m->Kp * 2 + 16);
   p.sc = a.take(static_cast<i64>(B) * D * 2);
   p.mod = a.take(static_cast<i64>(B) * NA * 4);
-  auto plan_blocks = [&](const std::vector<BlockP>& bl, std::vector<BlockBuf>& out, i64 M, int tokens) {
+  auto plan_blocks = [&](const std::vector<BlockP>& bl, std::vector<BlockBuf>& out, i64 M, int tokens, int first) {
     out.resize(bl.size());
     const i64 scratch0 = a.off;
     for (size_t i = 0; i < bl.size(); ++i) {
       if (!save) a.off = scratch0;  // inference: every block reuses one set of temporaries, residual in place
       const int d = bl[i].dim, h4 = bl[i].h4;
       BlockBuf& b = out[i];
+      if (first + static_cast<int>(i) < r) {  // recomputed: only the output residual stays, the rest is in the slot
+        grow(need_md, M * d), grow(need_m, M), grow(need_mh, M * h4), grow(need_lse, 2ll * B * bl[i].heads * tokens * 4);
+        b.X2 = a.take(M * d * 4);
+        continue;
+      }
       b.xm1 = a.take(M * d * 2);
       b.mean1 = save ? a.take(M * 4) : -1;
       b.rstd1 = save ? a.take(M * 4) : -1;
@@ -226,7 +244,7 @@ Plan make_plan(const mdt_model* m, int B, int T, bool save, bool with_backward) 
       b.y2 = save ? a.take(M * d * 2) : -1;
     }
   };
-  plan_blocks(m->enc, p.enc, Me, T);
+  plan_blocks(m->enc, p.enc, Me, T, 0);
   p.xmd = p.mean_d = p.rstd_d = p.u = p.Z = p.fk = p.Gz = p.du = p.dxmd = -1;
   if (m->has_dec) {
     p.xmd = a.take(Me * D * 2);
@@ -234,13 +252,38 @@ Plan make_plan(const mdt_model* m, int B, int T, bool save, bool with_backward) 
     p.rstd_d = a.take(Me * 4);
     p.u = a.take(Me * Dd * 4);
     p.Z = a.take(Md * Dd * 4);
-    plan_blocks(m->dec, p.dec, Md, L);
+    plan_blocks(m->dec, p.dec, Md, L, static_cast<int>(m->enc.size()));
   }
   const i64 Mf = m->has_dec ? Md : Me;  // final-layer rows
   p.xf = a.take(Mf * m->Df * 2);
   p.mean_f = a.take(Mf * 4);
   p.rstd_f = a.take(Mf * 4);
   if (!m->has_dec) p.fk = a.take(Me * m->pd * 4);
+  if (r > 0) {  // the recompute slot, in BlockBuf order (no X2), then the second mean1 / rstd1
+    BlockBuf s;
+    s.xm1 = a.take(need_md * 2);
+    s.mean1 = a.take(need_m * 4);
+    s.rstd1 = a.take(need_m * 4);
+    s.qkv = a.take(need_md * 3 * 2);
+    s.O = a.take(need_md * 2);
+    s.lse = a.take(need_lse);
+    s.X1 = a.take(need_md * 4);
+    s.y1 = a.take(need_md * 2);
+    s.xm2 = a.take(need_md * 2);
+    s.mean2 = a.take(need_m * 4);
+    s.rstd2 = a.take(need_m * 4);
+    s.a = a.take(need_mh * 2);
+    s.hpre = a.take(need_mh * 2);
+    s.y2 = a.take(need_md * 2);
+    const i64 mean1b = a.take(need_m * 4), rstd1b = a.take(need_m * 4);
+    const int ne = static_cast<int>(p.enc.size());
+    for (int g = 0; g < r; ++g) {
+      BlockBuf& b = g < ne ? p.enc[g] : p.dec[g - ne];
+      s.X2 = b.X2;
+      b = s;
+      if (g % 2) b.mean1 = mean1b, b.rstd1 = rstd1b;
+    }
+  }
   if (with_backward) {
     const i64 Mmax_d = Me * D > Md * Dd ? Me * D : Md * Dd;                    // max over (enc, dec) of M * dim
     const i64 Mmax_h = Me * m->H4e > Md * m->H4d ? Me * m->H4e : Md * m->H4d;  // M * mlp hidden
@@ -380,11 +423,23 @@ GateNext mlp_gate(Ctx& c, const BlockP& s, const BlockBuf& b, const float* mod, 
   return GateNext{c.at<void>(b.y2), mod + o, dmod + o, c.Gd(s.fc2_b), dy};
 }
 
+struct Refwd {  // a recomputed block: its forward is re-run into the recompute slot from its stored input X
+  const BlockP* s;
+  const BlockBuf* b;
+  float* X;
+  int T;
+};
+
+void refwd(Ctx& c, const Refwd* r, const float* mod, int B) {
+  if (r) block_fwd(c, *r->s, *r->b, r->X, mod, B, r->T, true);
+}
+
 // Backward of one DiTBlock.  Gr [M, d] f32 = residual-stream gradient, updated in place; dy2 = gradient of this
 // block's MLP-branch output (produced by the caller's LN backward).  `next` = the MLP gate of the block processed
-// next (fused into this block's last LN backward, which writes its dy into next->dy).
+// next (fused into this block's last LN backward, which writes its dy into next->dy).  `pre`: the block processed next
+// when it is recomputed; its forward is re-run just before that last LN backward, which reads its y2.
 void block_bwd(Ctx& c, const Plan& p, const BlockP& s, const BlockBuf& b, const float* X, float* Gr, const float* mod,
-               float* dmod, int B, int T, const void* dy2, const GateNext* next) {
+               float* dmod, int B, int T, const void* dy2, const GateNext* next, const Refwd* pre) {
   const int d = s.dim, h4 = s.h4;
   const i64 M = static_cast<i64>(B) * T, o = s.mod_off;
   void* st = c.stream;
@@ -409,6 +464,7 @@ void block_bwd(Ctx& c, const Plan& p, const BlockP& s, const BlockBuf& b, const 
   c.ck(mdt_colsum_bf16(dqkv, static_cast<int>(M), 3 * d, 3 * d, c.Gd(s.qkv_b), st));
   Gemm(dqkv, c.W16(s.qkv_w), M, d, 3 * d, false, true).out16(dxm).run(c);
   wgrad(c, dqkv, c.at<void>(b.xm1), 3 * d, d, M, c.Gd(s.qkv_w));
+  refwd(c, pre, mod, B);
   ln_bwd_gate(c, dxm, X, c.at<float>(b.mean1), c.at<float>(b.rstd1), mod + o + d, T, Gr, 1, dmod + o, dmod + o + d, M,
               d, next);
 }
@@ -457,6 +513,14 @@ int mdt_model_param_info(const mdt_model* m, int i, char* name, int name_cap, lo
 
 int mdt_model_mod_width(const mdt_model* m) { return m ? m->NA : -1; }
 
+int mdt_model_set_recompute(mdt_model* m, int r) {
+  if (!m || r < 0 || r > static_cast<int>(m->enc.size() + m->dec.size())) return MDT_ERR_ARG;
+  m->recompute = r;
+  return MDT_OK;
+}
+
+int mdt_model_get_recompute(const mdt_model* m) { return m ? m->recompute : -1; }
+
 long long mdt_workspace_bytes(const mdt_model* m, int B, int T, int training) {
   if (!m || B <= 0) return -1;
   if (T <= 0) T = m->L;
@@ -472,6 +536,7 @@ int mdt_forward(const mdt_model* m, const float* w32, const void* w16, const flo
   if (m->cfg.num_classes > 0 && !labels) return MDT_ERR_ARG;
   const Plan p = make_plan(m, B, T, save != 0, save != 0);
   if (p.total > workspace_bytes || (reinterpret_cast<uintptr_t>(workspace) & 255)) return MDT_ERR_ARG;
+  if (save) m->fwd_ws = workspace, m->fwd_r = m->recompute;
   Ctx c{m, w32, static_cast<const __nv_bfloat16*>(w16), nullptr, static_cast<char*>(workspace), stream};
   const mdt_model_cfg& cf = m->cfg;
   const int D = m->D, Dd = m->Dd, L = m->L, NA = m->NA, nc = cf.num_classes;
@@ -553,6 +618,10 @@ int mdt_backward(const mdt_model* m, const float* w32, const void* w16, float* g
   if ((ids_keep == nullptr) != (ids_restore == nullptr) || (!ids_keep && T != m->L)) return MDT_ERR_ARG;
   const Plan p = make_plan(m, B, T, true, true);
   if (p.total > workspace_bytes || (reinterpret_cast<uintptr_t>(workspace) & 255)) return MDT_ERR_ARG;
+  // the workspace must be laid out for this recompute count: at r > 0 it is the last saving forward's, at r = 0 it is
+  // not the last saving forward's if that one recomputed
+  const int r = m->recompute;
+  if (r ? (m->fwd_ws != workspace || m->fwd_r != r) : (m->fwd_ws == workspace && m->fwd_r != 0)) return MDT_ERR_ARG;
   Ctx c{m, w32, static_cast<const __nv_bfloat16*>(w16), grad, static_cast<char*>(workspace), stream};
   c.scratch = c.at<float>(p.det);
   const mdt_model_cfg& cf = m->cfg;
@@ -565,6 +634,18 @@ int mdt_backward(const mdt_model* m, const float* w32, const void* w16, float* g
 
   const int ne = static_cast<int>(m->enc.size());
   void* dyA = c.at<void>(p.dyA);
+  // Recomputation (r > 0).  The LN backward that ends block i's backward (or the final / decoder layer's) also runs the
+  // MLP-gate backward of block i-1 (the block processed next), which reads block i-1's y2.  So a recomputed block's
+  // forward is re-run into the slot right before that LN backward; only block i's mean1 / rstd1 are still read after
+  // the re-run, and consecutive recomputed blocks keep those in different copies (make_plan).
+  Refwd rf;
+  auto recomputed = [&](bool dec, int i) -> const Refwd* {
+    if ((dec ? ne + i : i) >= r) return nullptr;
+    const std::vector<BlockBuf>& bufs = dec ? p.dec : p.enc;
+    rf = Refwd{dec ? &m->dec[i] : &m->enc[i], &bufs[i],
+               c.at<float>(i > 0 ? bufs[i - 1].X2 : (dec ? p.Z : p.X0)), dec ? L : T};
+    return &rf;
+  };
   // the LN backward that starts the encoder's residual-stream gradient: of the decoder layer, or of the final layer
   // when there is no decoder (its adaLN offset, input gradient and saved statistics)
   i64 o = m->off_final;
@@ -592,7 +673,7 @@ int mdt_backward(const mdt_model* m, const float* w32, const void* w16, float* g
     // every LN backward finishes the residual-stream gradient that the NEXT gate backward consumes: one fused pass
     {
       GateNext gn;
-      if (nd) gn = mlp_gate(c, m->dec[nd - 1], p.dec[nd - 1], mod, dmod, dyA);
+      if (nd) gn = mlp_gate(c, m->dec[nd - 1], p.dec[nd - 1], mod, dmod, dyA), refwd(c, recomputed(true, nd - 1), mod, B);
       ln_bwd_gate(c, c.at<void>(p.dxf), Z_out, c.at<float>(p.mean_f), c.at<float>(p.rstd_f), mod + o + Dd, L, Gz, 0,
                   dmod + o, dmod + o + Dd, Md, Dd, nd ? &gn : nullptr);
     }
@@ -601,7 +682,8 @@ int mdt_backward(const mdt_model* m, const float* w32, const void* w16, float* g
       const float* Xin = i > 0 ? c.at<float>(p.dec[i - 1].X2) : c.at<float>(p.Z);
       GateNext gn;
       if (i > 0) gn = mlp_gate(c, m->dec[i - 1], p.dec[i - 1], mod, dmod, dyA);
-      block_bwd(c, p, m->dec[i], p.dec[i], Xin, Gz, mod, dmod, B, L, dyA, i > 0 ? &gn : nullptr);
+      block_bwd(c, p, m->dec[i], p.dec[i], Xin, Gz, mod, dmod, B, L, dyA, i > 0 ? &gn : nullptr,
+                i > 0 ? recomputed(true, i - 1) : nullptr);
       if (on_ready && c.rc == MDT_OK) on_ready(user, m->dec[i].lo, m->dec[i].hi);
     }
     // ---- unmask + decoder layer
@@ -617,7 +699,7 @@ int mdt_backward(const mdt_model* m, const float* w32, const void* w16, float* g
   const float* X_enc = ne ? c.at<float>(p.enc[ne - 1].X2) : c.at<float>(p.X0);
   {
     GateNext gn;
-    if (ne) gn = mlp_gate(c, m->enc[ne - 1], p.enc[ne - 1], mod, dmod, dyA);
+    if (ne) gn = mlp_gate(c, m->enc[ne - 1], p.enc[ne - 1], mod, dmod, dyA), refwd(c, recomputed(false, ne - 1), mod, B);
     ln_bwd_gate(c, dx_top, X_enc, mean_top, rstd_top, mod + o + D, T, Ge, 0, dmod + o, dmod + o + D, Me, D,
                 ne ? &gn : nullptr);
   }
@@ -626,7 +708,8 @@ int mdt_backward(const mdt_model* m, const float* w32, const void* w16, float* g
     const float* Xin = i > 0 ? c.at<float>(p.enc[i - 1].X2) : c.at<float>(p.X0);
     GateNext gn;
     if (i > 0) gn = mlp_gate(c, m->enc[i - 1], p.enc[i - 1], mod, dmod, dyA);
-    block_bwd(c, p, m->enc[i], p.enc[i], Xin, Ge, mod, dmod, B, T, dyA, i > 0 ? &gn : nullptr);
+    block_bwd(c, p, m->enc[i], p.enc[i], Xin, Ge, mod, dmod, B, T, dyA, i > 0 ? &gn : nullptr,
+              i > 0 ? recomputed(false, i - 1) : nullptr);
     if (on_ready && c.rc == MDT_OK) on_ready(user, m->enc[i].lo, m->enc[i].hi);
   }
   // ---- patch embedding (no input gradient needed)

@@ -345,6 +345,21 @@ class Engine:
                                         dmod[:, o:], dmod[:, o + D:], NA, M, D, gate_next=gate_next)
 
 
+RECOMPUTE_MARGIN = 256 << 20   # bytes kept free when the recompute count is chosen from the memory left
+
+
+def pick_recompute(sizes, budget):
+    """The smallest recompute count r whose training workspace `sizes[r]` (bytes, r = 0 .. depth + dec_depth) fits into
+    `budget` bytes.  Raises torch.OutOfMemoryError naming the smallest workspace and the budget when none fits."""
+    for r, n in enumerate(sizes):
+        if n <= budget:
+            return r
+    r = min(range(len(sizes)), key=lambda i: sizes[i])
+    raise torch.OutOfMemoryError(
+        f"the training workspace does not fit: it needs {sizes[r] / 2**30:.2f} GiB even with {r} of "
+        f"{len(sizes) - 1} blocks recomputed, and {max(budget, 0) / 2**30:.2f} GiB of device memory is available")
+
+
 class CEngine:
     """The same forward / backward issued by the C++ step driver (csrc/driver.cu: `mdt_forward`, `mdt_backward`): ONE
     C-ABI call each over the packed parameter blob and one workspace buffer, instead of ~780 ctypes calls and a
@@ -365,6 +380,13 @@ class CEngine:
         ops.check(L.mdt_model_create(ctypes.byref(mc), ctypes.byref(h)), "mdt_model_create", 0)
         self._h, self._L = h, L
         self.NA = L.mdt_model_mod_width(h)   # width of the modulation vector = rows of the adaLN weight matrix
+        # Activation recomputation (`mdt_model_set_recompute`) of the training pass.  `recompute` None: automatic, i.e.
+        # nothing is recomputed unless the workspace allocation runs out of memory, then the smallest count that fits
+        # (remembered per batch shape); an int forces that count.  `recompute_blocks`: the count of the last training
+        # forward.
+        self.recompute = None
+        self.recompute_blocks = 0
+        self._auto_recompute = {}
 
     def __del__(self):
         try:
@@ -386,23 +408,62 @@ class CEngine:
         """Elements of the trainable region, or of the whole blob (`mdt_model_param_count`)."""
         return self._L.mdt_model_param_count(self._h, int(trainable_only))
 
-    def workspace_bytes(self, B, T, training):
-        n = self._L.mdt_workspace_bytes(self._h, B, T, int(training))
+    @property
+    def num_blocks(self):
+        return self.cfg.depth + self.cfg.dec_depth
+
+    def set_recompute(self, r):
+        """Set the handle's recompute count (blocks 0 .. r-1 in forward order, encoder first)."""
+        ops.check(self._L.mdt_model_set_recompute(self._h, int(r)), "mdt_model_set_recompute", 0)
+
+    def workspace_bytes(self, B, T, training, recompute=None):
+        """`mdt_workspace_bytes`; `recompute` (training only): at that count instead of the handle's current one."""
+        cur = self._L.mdt_model_get_recompute(self._h)
+        if recompute is not None:
+            self.set_recompute(recompute)
+        try:
+            n = self._L.mdt_workspace_bytes(self._h, B, T, int(training))
+        finally:
+            if recompute is not None:
+                self.set_recompute(cur)
         if n <= 0:
             raise ops.L.MdtError("mdt_workspace_bytes failed")
         return n
 
-    def _count(self, masked):
-        """Kernel launches of one forward / backward (for bench.py's gpu_launches claim): same sequence as `Engine`."""
+    def _count(self, masked, recompute=0):
+        """Kernel launches of one forward / backward (for bench.py's gpu_launches claim): same sequence as `Engine`,
+        plus the 7 forward launches of each recomputed block in the backward."""
         c = self.cfg
         nb = c.depth + c.dec_depth
         if c.dec_hidden == 0:   # no decoder: final 2 (+ zero-filled scatter) / final 4 (+ kept-row gather of dF)
             fwd = 9 + (2 if c.num_classes else 0) + 7 * nb + int(masked)          # embed/conditioning 7
             bwd = 16 + 13 * nb + (1 if c.num_classes else 0) + int(masked)        # patch-embed 1, conditioning 11
-            return fwd, bwd
+            return fwd, bwd + 7 * recompute
         fwd = 12 + (2 if c.num_classes else 0) + 7 * nb          # embed/conditioning 7, decoder layer 3, final 2
         bwd = 21 + 13 * nb + (1 if c.num_classes else 0)         # final 4, transition 5, patch-embed 1, conditioning 11
-        return fwd, bwd
+        return fwd, bwd + 7 * recompute
+
+    def _training_workspace(self, B, T, device):
+        """The recompute count and the workspace of a training pass.  Forced count: that plan.  Automatic: the count
+        chosen earlier for this batch shape, else r = 0; only when that allocation runs out of memory, the smallest
+        count whose workspace fits into the free device memory plus the caching allocator's reserved-but-unused bytes,
+        less RECOMPUTE_MARGIN."""
+        key = (B, T, self._L.mdt_get_deterministic())   # the deterministic mode's scratch is part of the workspace
+        r =self.recompute if self.recompute is not None else self._auto_recompute.get(key, 0)
+        self.set_recompute(r)
+        nbytes = self.workspace_bytes(B, T, True)
+        try:
+            return r, torch.empty(nbytes, dtype=torch.uint8, device=device), nbytes
+        except torch.OutOfMemoryError:
+            if self.recompute is not None or r > 0:
+                raise
+        free, _ = torch.cuda.mem_get_info(device)
+        budget = free + torch.cuda.memory_reserved(device) - torch.cuda.memory_allocated(device) - RECOMPUTE_MARGIN
+        r = pick_recompute([self.workspace_bytes(B, T, True, k) for k in range(self.num_blocks + 1)], budget)
+        self._auto_recompute[key] = r
+        self.set_recompute(r)
+        nbytes = self.workspace_bytes(B, T, True)
+        return r, torch.empty(nbytes, dtype=torch.uint8, device=device), nbytes
 
     def forward(self, x_in, sigma, labels, mask_dict, save):
         cfg = self.cfg
@@ -413,8 +474,12 @@ class CEngine:
         for t, dt in ((x_in, f32), (sigma, f32), (labels, f32), (ids_keep, torch.int64), (ids_restore, torch.int64)):
             ops._c(t, dt)
         ops.L.sync_deterministic()   # the workspace size and the backward's reductions follow the torch flag
-        nbytes = self.workspace_bytes(B, T, save)
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=x_in.device)   # ONE allocation per pass
+        if save:   # ONE allocation per pass
+            r, ws, nbytes = self._training_workspace(B, T, x_in.device)
+            self.recompute_blocks = r
+        else:
+            nbytes = self.workspace_bytes(B, T, False)
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=x_in.device)
         Fo = torch.empty(B * L, cfg.patch_dim, dtype=f32, device=x_in.device)
         st = self.store
         ops.check(self._L.mdt_forward(self._h, ops.ptr(st.w32), ops.ptr(st.w16), ops.ptr(x_in), ops.ptr(sigma),
@@ -424,7 +489,7 @@ class CEngine:
         ctx = None
         if save:
             ctx = dict(ws=ws, nbytes=nbytes, x_in=x_in, sigma=sigma, ids_keep=ids_keep, ids_restore=ids_restore, B=B,
-                       T=T)
+                       T=T, recompute=r)
         return Fo, ctx
 
     def backward(self, ctx, dF16, on_ready=None):
@@ -432,10 +497,11 @@ class CEngine:
         st.ensure_grad()
         ops._c(dF16, bf16)
         ops.L.sync_deterministic()
+        self.set_recompute(ctx["recompute"])   # the plan the forward laid the workspace out with
         cb =ops.L.GRAD_READY_FN(lambda user, lo, hi: on_ready(lo, hi)) if on_ready is not None \
             else ops.L.GRAD_READY_FN()
         ops.check(self._L.mdt_backward(self._h, ops.ptr(st.w32), ops.ptr(st.w16), ops.ptr(st.grad), ops.ptr(ctx["x_in"]),
                                        ops.ptr(ctx["sigma"]), ops.ptr(ctx["ids_keep"]), ops.ptr(ctx["ids_restore"]),
                                        ops.ptr(dF16), ctx["B"], ctx["T"], ops.ptr(ctx["ws"]), ctx["nbytes"], cb, None,
                                        ops.stream_ptr()), "mdt_backward",
-                  self._count(ctx["ids_restore"] is not None)[1])
+                  self._count(ctx["ids_restore"] is not None, ctx["recompute"])[1])

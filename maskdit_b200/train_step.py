@@ -106,8 +106,15 @@ class TrainStep:
     def __init__(self, net: EDMPrecond, ema: EDMPrecond | None = None, lr=1e-4, betas=(0.9, 0.999), eps=1e-8,
                  weight_decay=0.0, ema_decay=0.9999, loss_fn: EDMLoss | None = None, process_group=None,
                  lr_rampup_kimg=0.0, global_batch=None, device=None, overlap=False, graph=None,
-                 reference_lr_schedule=False, collective=None, grad_dtype=None, comm_ctas=None, skip_nonfinite=False):
-        """skip_nonfinite: skip every optimizer step whose gradient holds an inf or NaN, as the reference's fp16
+                 reference_lr_schedule=False, collective=None, grad_dtype=None, comm_ctas=None, skip_nonfinite=False,
+                 recompute_blocks=None):
+        """recompute_blocks: how many blocks (in forward order, encoder first) keep only their output and have their
+        forward re-run in the backward (activation recomputation, `mdt_model_set_recompute`).  None: automatic, i.e.
+        none unless the training workspace of a micro-batch does not fit into device memory, then the fewest that
+        make it fit; an int in [0, depth + dec_depth] forces that count.  The count in use is `self.recompute_blocks`.
+        The gradients do not depend on it beyond the default mode's summation-order noise (bit for bit under
+        `torch.use_deterministic_algorithms(True)`).
+        skip_nonfinite:skip every optimizer step whose gradient holds an inf or NaN, as the reference's fp16
         GradScaler does (train.py:39-48): the weights, the bf16 shadow, the moments and Adam's step count stay as they
         are, the EMA still moves toward the unchanged weights (train.py:230), and the lr schedule's counter
         (`step_count`) advances as for any attempted step.  The gradient checked is the one the optimizer consumes
@@ -142,6 +149,12 @@ class TrainStep:
         dev = device or next(net.parameters()).device
         self.st = net.prepare(dev)
         self.st.ensure_grad()
+        self._engine = net._engine
+        if recompute_blocks is not None and not 0 <= int(recompute_blocks) <= self._engine.num_blocks:
+            raise ValueError(f"recompute_blocks {recompute_blocks} outside [0, {self._engine.num_blocks}]")
+        self._engine.recompute = None if recompute_blocks is None else int(recompute_blocks)
+        if recompute_blocks is not None:
+            self._engine.recompute_blocks = int(recompute_blocks)
         n = self.st.n_train
         self.m = torch.zeros(n, dtype=torch.float32, device=dev)
         self.v = torch.zeros(n, dtype=torch.float32, device=dev)
@@ -186,6 +199,11 @@ class TrainStep:
         self.skip_nonfinite = bool(skip_nonfinite)
         self._flag = torch.zeros(1, dtype=torch.float32, device=dev) if self.skip_nonfinite else None
         self._counts = torch.zeros(2, dtype=torch.int64, device=dev) if self.skip_nonfinite else None
+
+    @property
+    def recompute_blocks(self) -> int:
+        """Blocks recomputed by the last training forward (before the first step: the forced count, or 0)."""
+        return self._engine.recompute_blocks
 
     @property
     def skipped_steps(self):

@@ -133,6 +133,7 @@ def main():
         loader = batches(ds, batch, rank, world, start=step0)
     log_every = cfg.log.log_every
     running, log_steps, t0, step = 0.0, 0, time.time(), step0
+    recompute_shown = 0
     for moments, labels in loader:
         moments = moments.to(device, non_blocking=True)
         labels = labels.to(device, non_blocking=True)
@@ -141,6 +142,11 @@ def main():
         loss = ts.step(moments, labels, ratio, cfg.model.mae_loss_coef, grad_accum=rounds, moments=True,
                        class_dropout_prob=drop)
         running = running + loss.mean()
+        if rank == 0 and ts.recompute_blocks and not recompute_shown:
+            recompute_shown = ts.recompute_blocks
+            print(f"Activation recomputation: the training workspace of a micro-batch does not fit in device memory, "
+                  f"{recompute_shown} of {net.model.depth + net.model.decoder_depth} blocks recompute their forward "
+                  f"in the backward", flush=True)
         log_steps += 1
         step += 1
         if step - step0 > max_steps:
