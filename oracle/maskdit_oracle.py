@@ -245,7 +245,9 @@ def dit_forward(sd, cfg: Cfg, x, t, y, mask_dict=None, training=True):
         idx = mask_dict["ids_keep"].unsqueeze(-1).expand(-1, -1, D)
         h = torch.gather(h, 1, idx)
     # conditioning (:491-495): t-MLP (:34-38) + label table (:75,80)
-    te = F.linear(timestep_embedding(t, 256), sd["model.t_embedder.mlp.0.weight"], sd["model.t_embedder.mlp.0.bias"])
+    # the frequency embedding is computed in float32 as the reference does; a float64 run casts it up
+    te = F.linear(timestep_embedding(t, 256).to(x.dtype), sd["model.t_embedder.mlp.0.weight"],
+                  sd["model.t_embedder.mlp.0.bias"])
     c = F.linear(F.silu(te), sd["model.t_embedder.mlp.2.weight"], sd["model.t_embedder.mlp.2.bias"])
     if cfg.num_classes:
         c = c + F.linear(y, sd["model.y_embedder.embedding_table.weight"])

@@ -190,7 +190,10 @@ def run_attention(ops, qkv, B, T, H, dh):
     (ref * dout.to(f64)).sum().backward()
     dqkv = ops.attention_bwd(qkv, out, dout, lse, B, T, H, dh)
     impl_bwd = ops.lib().mdt_attention_last_impl(1)
-    close(dqkv, qr.grad, 2 ** -7, "attention bwd")
+    # dq, dk and dv each against its own scale: an error in the smallest cannot hide under the largest
+    got, want = dqkv.view(B * T, 3, H * dh), qr.grad.view(B * T, 3, H * dh)
+    for i, name in enumerate("qkv"):
+        close(got[:, i], want[:, i], 2 ** -7, f"attention bwd d{name}")
     return impl_fwd, impl_bwd
 
 
@@ -223,8 +226,9 @@ def test_attention_large_logits(ops, B, T, H, dh, family):
 
 
 # ---- LayerNorm + modulate, gate backward -----------------------------------------------------------------------------
-@pytest.mark.parametrize("D", [768, 1024, 1280])
-@pytest.mark.parametrize("T", [8, 16, 32, 44, 128])
+# T = 130, 179 and 192: backward blocks of gcd(T, 32) = 2, 1 and 32 rows of one sample in the default mode
+@pytest.mark.parametrize("D", [768, 1024, 1152, 1280])
+@pytest.mark.parametrize("T", [8, 16, 32, 44, 128, 130, 179, 192])
 def test_ln_modulate_and_gate_kernels(ops, D, T):
     torch.manual_seed(70 + D + T)
     B = 3

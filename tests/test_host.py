@@ -201,6 +201,18 @@ def test_config_schema_and_mask_schedule():
     with pytest.raises(ValueError):
         mask_ratio_schedule("bogus")
     assert parse_int_list("1,2,5-8") == [1, 2, 5, 6, 7, 8] and parse_float_none("None") is None
+    # The finetune recipe (cos4, mask_ratio 0.5, 100 000 steps) changes the kept-token count T = int(L * (1 - r))
+    # almost every step: every count from L / 2 to L, and T = L with masking on (r < 1e-16) for the last steps.
+    import numpy as np
+    f = mask_ratio_schedule("cos4", 0.5, 0.0)
+    n = 100000
+    x = np.arange(n) / n
+    r_ref = (0.5 - 0.0) * np.cos(np.pi * x / 2) ** 4 + 0.0      # get_mask_ratio_fn('cosine4', 0.5, 0.0)
+    for L in (256, 1024):
+        T = [int(L * (1 - f(s / n))) for s in range(n)]
+        assert T == [int(L * (1 - r)) for r in r_ref]
+        assert set(T) == set(range(L // 2, L + 1))
+        assert T[-6:] == [L] * 6 and T[-7] == L - 1 and all(0 < f(s / n) < 1e-16 for s in range(n - 6, n))
 
 
 def test_model_handle_and_flat_store_refuse_mismatches():

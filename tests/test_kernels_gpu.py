@@ -1,5 +1,5 @@
-"""Per-kernel parity (GPU): every C-ABI kernel against a plain PyTorch fp32 reference of the same op fed the SAME
-bf16-rounded inputs.  Tolerances are stated per test: fp32-accumulate kernels 1e-3 relative to the output scale,
+"""Per-kernel parity (GPU): every C-ABI kernel against a plain PyTorch fp32 reference (float64 for the attention) of
+the same op fed the SAME bf16-rounded inputs.  Tolerances are stated per test: fp32-accumulate kernels 1e-3 relative to the output scale,
 bf16-output kernels 1 bf16 ulp (2^-8) relative; the integer mask path is bit-exact."""
 import math
 import os
@@ -277,30 +277,43 @@ def test_gate_bwd(ops, D, T, B):
 
 
 def attn_ref(qkv, B, T, H, dh):
-    q, k, v = qkv.float().view(B, T, 3, H, dh).permute(2, 0, 3, 1, 4).unbind(0)
+    q, k, v = qkv.double().view(B, T, 3, H, dh).permute(2, 0, 3, 1, 4).unbind(0)
     att = torch.softmax(q @ k.transpose(-1, -2) * dh ** -0.5, -1)
     return (att @ v).transpose(1, 2).reshape(B * T, H * dh)
+
+
+def close_qkv(got, ref, B, T, H, dh, tol, what=""):
+    """dq, dk and dv each against its own scale: an error in the smallest of the three cannot hide under the largest."""
+    got, ref = got.view(B * T, 3, H * dh), ref.view(B * T, 3, H * dh)
+    for i, name in enumerate("qkv"):
+        close(got[:, i], ref[:, i], tol, f"{what} d{name}")
 
 
 @pytest.mark.parametrize("B,T,H,dh", [(2, 128, 16, 72), (2, 256, 16, 32), (3, 8, 6, 64), (1, 200, 4, 72),
                                       (1, 512, 16, 72), (1, 1024, 2, 32), (2, 256, 16, 72), (3, 128, 6, 64),
                                       (5, 128, 16, 32), (2, 512, 4, 32), (1, 512, 6, 64), (1, 1024, 3, 64),
-                                      (1, 1024, 2, 72), (3, 256, 5, 64)])
+                                      (1, 1024, 2, 72), (3, 256, 5, 64),
+                                      # the wgmma kernels at one and three 64-row blocks (XL and S/B/L encoders at
+                                      # mask ratio 0.75 / 0.25 and 256 px) and at odd block counts at 512 px
+                                      (2, 64, 16, 72), (2, 192, 16, 72), (2, 192, 6, 64), (1, 576, 16, 72),
+                                      (1, 960, 16, 72),
+                                      # mma.sync with one valid key in the last tile (T = 1 mod 64) and with 63
+                                      (2, 129, 16, 72), (2, 193, 6, 64), (2, 255, 16, 72)])
 def test_attention_fwd_bwd(ops, B, T, H, dh):
     torch.manual_seed(8)
     qkv = rb(B * T, 3 * H * dh)
     out, lse = ops.attention_fwd(qkv, B, T, H, dh)
     impl_fwd = ops.lib().mdt_attention_last_impl(0)
-    qr = qkv.float().requires_grad_(True)
+    qr = qkv.double().requires_grad_(True)
     ref = attn_ref(qr, B, T, H, dh)
     close(out, ref, 2 ** -7, "attention fwd")
-    q, k = qkv.float().view(B, T, 3, H, dh)[:, :, 0].transpose(1, 2), qkv.float().view(B, T, 3, H, dh)[:, :, 1].transpose(1, 2)
+    q, k = qkv.double().view(B, T, 3, H, dh)[:, :, 0].transpose(1, 2), qkv.double().view(B, T, 3, H, dh)[:, :, 1].transpose(1, 2)
     close(lse[0], torch.logsumexp(q @ k.transpose(-1, -2) * dh ** -0.5, -1), 1e-3, "lse")
     dout = rb(B * T, H * dh)
-    (ref * dout.float()).sum().backward()
+    (ref * dout.double()).sum().backward()
     dqkv = ops.attention_bwd(qkv, out, dout, lse, B, T, H, dh)
     impl_bwd = ops.lib().mdt_attention_last_impl(1)
-    close(dqkv, qr.grad, 2 ** -7, "attention bwd")
+    close_qkv(dqkv, qr.grad, B, T, H, dh, 2 ** -7, "attention bwd")
     # which kernel family ran (include/maskdit_b200.h): the wgmma + TMA kernels for every T that is a multiple of 64,
     # the mma.sync kernels otherwise - a silently broken wgmma path cannot hide behind the general kernels
     print("attention impl", (B, T, H, dh), impl_fwd, impl_bwd)
