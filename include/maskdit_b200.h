@@ -279,6 +279,18 @@ int mdt_adamw_ema_guarded_g16(float* w, const void* g_bf16, float* m, float* v, 
                               void* stream);
 int mdt_optim_guard_advance(const float* flag, long long* counts, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Power-function EMA profiles (post-hoc EMA, Karras et al., CVPR 2024, §3): k <= 4 fp32 profiles advanced from ONE
+ * read of w[0, n):
+ *   ema[j][i] += one_minus_beta[j] * (w[i] - ema[j][i])        (fp32, one fused multiply-add; c == 1 stores w exactly)
+ * `ema` (k device pointers) and `one_minus_beta` (k coefficients in [0, 1], computed in float64 by the caller and
+ * rounded) are HOST arrays, read at the call.  Any n > 0 and any 4-byte aligned slices: when every buffer reaches a
+ * 16-byte boundary after the same number of elements the body moves float4s, otherwise every element is scalar.
+ * Traffic: (4 + 8k) bytes per element.  MDT_ERR_ARG for a NULL pointer, k outside [1, 4], n <= 0, a pointer not 4-byte
+ * aligned or a coefficient outside [0, 1] (NaN included).
+ * ------------------------------------------------------------------------------------------------------------ */
+int mdt_power_ema(const float* w, float* const* ema, const float* one_minus_beta, int k, long long n, void* stream);
+
 /* Cap on the SMs the persistent kernels (the wgmma GEMM) occupy: n > 0 sizes their grids
  * for n SMs instead of the device's count, leaving the rest to a concurrently running collective (the gradient
  * all-reduce overlapped with the backward); 0 = whole device.  Host-side setting, read at launch.                  */

@@ -1,4 +1,5 @@
-// EDM preconditioning output, EDM + MAE loss (forward + gradient seed), CFG combine, Heun update, fused AdamW+EMA.
+// EDM preconditioning output, EDM + MAE loss (forward + gradient seed), CFG combine, Heun update, fused AdamW+EMA,
+// power-function EMA profiles (post-hoc EMA).
 #include <math.h>
 
 #include "common.cuh"
@@ -336,6 +337,44 @@ __global__ void optim_guard_advance_kernel(const float* __restrict__ flag, long 
   counts[*flag != 0.f ? 1 : 0] += 1;
 }
 
+// ---- Power-function EMA profiles (post-hoc EMA, Karras et al. CVPR 2024 §3) ---------------------------------------------
+// K profiles advanced from one read of w:  e += c_j * (w - e).  c_j == 1 (a profile's first step) stores w exactly.
+constexpr int kMaxPowerEma = 4;
+struct PowerEmaArgs {
+  float* e[kMaxPowerEma];
+  float c[kMaxPowerEma];
+};
+
+MDT_DEVINL float power_ema_one(float w, float e, float c) { return c == 1.f ? w : fmaf(c, w - e, e); }
+
+// [0, head): scalar head up to the 16-byte boundary all buffers share; then n4 float4 groups; then the scalar tail.
+template <int K>
+__global__ void __launch_bounds__(256) power_ema_kernel(const float* __restrict__ w, PowerEmaArgs a, long long n,
+                                                        long long head, long long n4) {
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  const long long t = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  const float4* w4 = reinterpret_cast<const float4*>(w + head);
+  for (long long i = t; i < n4; i += stride) {
+    const float4 wv = w4[i];
+#pragma unroll
+    for (int j = 0; j < K; ++j) {
+      float4* e4 = reinterpret_cast<float4*>(a.e[j] + head);
+      float4 ev = e4[i];
+      ev.x = power_ema_one(wv.x, ev.x, a.c[j]), ev.y = power_ema_one(wv.y, ev.y, a.c[j]);
+      ev.z = power_ema_one(wv.z, ev.z, a.c[j]), ev.w = power_ema_one(wv.w, ev.w, a.c[j]);
+      e4[i] = ev;
+    }
+  }
+  const long long body_end = head + (n4 << 2);
+  const long long n_scalar = head + (n - body_end);
+  for (long long s = t; s < n_scalar; s += stride) {
+    const long long i = s < head ? s : body_end + (s - head);
+    const float wv = w[i];
+#pragma unroll
+    for (int j = 0; j < K; ++j) a.e[j][i] = power_ema_one(wv, a.e[j][i], a.c[j]);
+  }
+}
+
 
 // Step front (SURVEY 8(f)2): VAE moments -> latent (utils.py:59-65), label dropout (train.py:209), sigma draw and
 // noise injection (train_utils/loss.py:35-39) in ONE pass over the batch, given the pre-drawn normals / uniforms
@@ -553,6 +592,35 @@ int mdt_optim_guard_advance(const float* flag, long long* counts, void* stream) 
   if (!flag || !counts || (reinterpret_cast<uintptr_t>(counts) & 7) || (reinterpret_cast<uintptr_t>(flag) & 3))
     return MDT_ERR_ARG;
   optim_guard_advance_kernel<<<1, 1, 0, S(stream)>>>(flag, counts);
+  return launch_status();
+}
+
+int mdt_power_ema(const float* w, float* const* ema, const float* one_minus_beta, int k, long long n, void* stream) {
+  if (!w || !ema || !one_minus_beta || k < 1 || k > kMaxPowerEma || n <= 0) return MDT_ERR_ARG;
+  const uintptr_t phase = reinterpret_cast<uintptr_t>(w) & 15;
+  if (phase & 3) return MDT_ERR_ARG;
+  PowerEmaArgs a{};
+  bool same_phase = true;
+  for (int j = 0; j < k; ++j) {
+    const float c = one_minus_beta[j];
+    if (!ema[j] || (reinterpret_cast<uintptr_t>(ema[j]) & 3) || !(c >= 0.f && c <= 1.f)) return MDT_ERR_ARG;
+    same_phase &= (reinterpret_cast<uintptr_t>(ema[j]) & 15) == phase;
+    a.e[j] = ema[j], a.c[j] = c;
+  }
+  // float4 body when every buffer reaches a 16-byte boundary after the same number of elements; else all scalar
+  long long head = n, n4 = 0;
+  if (same_phase) {
+    head = static_cast<long long>((16 - phase) & 15) / 4;
+    if (head > n) head = n;
+    n4 = (n - head) >> 2;
+  }
+  const int blocks = check_grid(n);
+  switch (k) {
+    case 1: power_ema_kernel<1><<<blocks, 256, 0, S(stream)>>>(w, a, n, head, n4); break;
+    case 2: power_ema_kernel<2><<<blocks, 256, 0, S(stream)>>>(w, a, n, head, n4); break;
+    case 3: power_ema_kernel<3><<<blocks, 256, 0, S(stream)>>>(w, a, n, head, n4); break;
+    default: power_ema_kernel<4><<<blocks, 256, 0, S(stream)>>>(w, a, n, head, n4); break;
+  }
   return launch_status();
 }
 

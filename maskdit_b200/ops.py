@@ -280,3 +280,20 @@ def optim_guard_advance(flag, counts):
     """counts[1 if flag else 0] += 1: once per step, after its last guarded optimizer pass."""
     _c(flag, f32), _c(counts, torch.int64)
     check(lib().mdt_optim_guard_advance(ptr(flag), ptr(counts), stream_ptr()), "mdt_optim_guard_advance")
+
+
+def power_ema(w, emas, coeffs):
+    """Power-function EMA profiles: emas[j] += coeffs[j] * (w - emas[j]) for up to 4 fp32 tensors of w's size, from one
+    read of w.  `coeffs` are host floats (1 - beta_j), rounded to fp32 at the call."""
+    import ctypes
+    _c(w, f32)
+    k = len(emas)
+    if k != len(coeffs):
+        raise L.MdtError(f"{k} profiles but {len(coeffs)} coefficients")
+    for e in emas:
+        _c(e, f32)
+        if e.numel() != w.numel() or e.device != w.device:
+            raise L.MdtError("every profile must have w's size and device")
+    check(lib().mdt_power_ema(ptr(w), (ctypes.c_void_p * max(k, 1))(*[e.data_ptr() for e in emas]),
+                              (ctypes.c_float * max(k, 1))(*[float(c) for c in coeffs]), k, w.numel(), stream_ptr()),
+          "mdt_power_ema")

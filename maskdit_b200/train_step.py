@@ -18,7 +18,7 @@ import os
 import torch
 import torch.distributed as dist
 
-from . import ops
+from . import ops, phema
 from .loss import EDMLoss
 from .maskdit import EDMPrecond
 
@@ -103,12 +103,21 @@ class GradComm:
 
 
 class TrainStep:
+    phema_emas = ()   # no post-hoc EMA profiles unless the constructor is given widths
+
     def __init__(self, net: EDMPrecond, ema: EDMPrecond | None = None, lr=1e-4, betas=(0.9, 0.999), eps=1e-8,
                  weight_decay=0.0, ema_decay=0.9999, loss_fn: EDMLoss | None = None, process_group=None,
                  lr_rampup_kimg=0.0, global_batch=None, device=None, overlap=False, graph=None,
                  reference_lr_schedule=False, collective=None, grad_dtype=None, comm_ctas=None, skip_nonfinite=False,
-                 recompute_blocks=None):
-        """recompute_blocks: how many blocks (in forward order, encoder first) keep only their output and have their
+                 recompute_blocks=None, phema_sigma_rels=()):
+        """phema_sigma_rels: relative widths of power-function EMA profiles to keep for post-hoc EMA (`phema.py`,
+        posthoc_ema.py), e.g. (0.05, 0.10); at most 4.  Each is one fp32 buffer over the trainable region (2.92 GB for XL/2),
+        allocated here and advanced after every optimizer pass over a range, on that pass's stream, by `mdt_power_ema`
+        with 1 - beta(t) from the host's count t of the profiles' steps: exactly one update per optimizer step (also
+        under grad_accum, and toward the unchanged weights when skip_nonfinite skips the step).  The profiles count
+        from `phema_origin`, the run step before their first update (`step_count + lr_step_offset` then).  Empty
+        (default): nothing is allocated and nothing launches.
+        recompute_blocks: how many blocks (in forward order, encoder first) keep only their output and have their
         forward re-run in the backward (activation recomputation, `mdt_model_set_recompute`).  None: automatic, i.e.
         none unless the training workspace of a micro-batch does not fit into device memory, then the fewest that
         make it fit; an int in [0, depth + dec_depth] forces that count.  The count in use is `self.recompute_blocks`.
@@ -199,6 +208,15 @@ class TrainStep:
         self.skip_nonfinite = bool(skip_nonfinite)
         self._flag = torch.zeros(1, dtype=torch.float32, device=dev) if self.skip_nonfinite else None
         self._counts = torch.zeros(2, dtype=torch.int64, device=dev) if self.skip_nonfinite else None
+        # power-function EMA profiles: allocated now, so the recomputation picker sees their memory as used
+        self.phema_sigma_rels = tuple(float(s) for s in phema_sigma_rels)
+        if len(self.phema_sigma_rels) > 4:   # mdt_power_ema advances up to 4 profiles from one read of the weights
+            raise ValueError(f"{len(self.phema_sigma_rels)} post-hoc EMA profiles: at most 4")
+        self.phema_gammas = tuple(phema.sigma_rel_to_gamma(s) for s in self.phema_sigma_rels)
+        self.phema_emas = [torch.zeros(n, dtype=torch.float32, device=dev) for _ in self.phema_sigma_rels]
+        self.phema_origin = None   # run step before the profiles' first update (None: set by the next step)
+        self.phema_steps = 0       # updates since the origin (the profiles' t after the last step)
+        self._phema_c = None
 
     @property
     def recompute_blocks(self) -> int:
@@ -224,7 +242,9 @@ class TrainStep:
         decoder-less DiT, whose only frozen tensor is pos_embed) — with
         `exp_avg` / `exp_avg_sq` and a per-parameter `step` (torch layout); the step count is also stored in the
         param_group (apex layout).  Tensors are copies on the current device.  The step count is Adam's
-        (`applied_steps()`): under `skip_nonfinite` it leaves out the skipped steps."""
+        (`applied_steps()`): under `skip_nonfinite` it leaves out the skipped steps.
+        With power-function EMA profiles, `phema` holds their widths, exponents, origin, step count and flat buffers
+        (host copies: the device keeps no second copy of them)."""
         state, n_all = {}, 0
         adam_step = self.applied_steps()
         for i, (k, p) in enumerate(self.net.named_parameters()):
@@ -235,9 +255,14 @@ class TrainStep:
             n = p.numel()
             state[i] = {"step": torch.tensor(float(adam_step)), "exp_avg": self.m[lo:lo + n].view(shape).clone(),
                         "exp_avg_sq": self.v[lo:lo + n].view(shape).clone()}
-        return {"state": state,
-                "param_groups": [{"lr": self.lr, "betas": self.betas, "eps": self.eps, "weight_decay": self.wd,
-                                  "step": adam_step, "params": list(range(n_all))}]}
+        sd = {"state": state,
+              "param_groups": [{"lr": self.lr, "betas": self.betas, "eps": self.eps, "weight_decay": self.wd,
+                                "step": adam_step, "params": list(range(n_all))}]}
+        if self.phema_emas:
+            sd["phema"] = {"sigma_rels": list(self.phema_sigma_rels), "gammas": list(self.phema_gammas),
+                           "origin": self.phema_origin, "steps": self.phema_steps,
+                           "emas": [e.to("cpu", copy=True) for e in self.phema_emas]}
+        return sd
 
     def load_state_dict(self, sd):
         """Accepts (a) this class's own layout, (b) `torch.optim.AdamW(model.parameters()).state_dict()`, (c) apex
@@ -277,6 +302,50 @@ class TrainStep:
             self._counts[0].fill_(self.step_count)
         self.lr, self.betas, self.eps, self.wd = group["lr"], tuple(group["betas"]), group["eps"], \
             group["weight_decay"]
+        if self.phema_emas:
+            self._load_phema(sd.get("phema"))
+
+    def _load_phema(self, ph):
+        """Continue the stored profiles, or (a state without them, e.g. a reference checkpoint) start new ones whose
+        origin is the run step of the next update."""
+        if ph is None:
+            for e in self.phema_emas:
+                e.zero_()
+            self.phema_origin, self.phema_steps = None, 0
+            return
+        if [round(s, 9) for s in ph["sigma_rels"]] != [round(s, 9) for s in self.phema_sigma_rels]:
+            raise ValueError(f"the state holds post-hoc EMA profiles of sigma_rel {list(ph['sigma_rels'])}, this "
+                             f"TrainStep keeps {list(self.phema_sigma_rels)}")
+        for e, src in zip(self.phema_emas, ph["emas"]):
+            if src.numel() != e.numel():
+                raise ValueError(f"post-hoc EMA profile of {src.numel()} elements, the model trains {e.numel()}")
+            e.copy_(src.reshape(-1))
+        self.phema_origin, self.phema_steps = int(ph["origin"]), int(ph["steps"])
+
+    # -- power-function EMA profiles (post-hoc EMA) ----------------------------------------------------------------
+    def phema_state_dicts(self):
+        """The profiles as model state dicts with the module's keys (host copies; frozen tensors from the weights)."""
+        out = []
+        for e in self.phema_emas:
+            flat = e.to("cpu", copy=True)   # one host storage per profile; the trainable tensors are views into it
+            sd = {}
+            for k, v in self.net.state_dict().items():
+                o, cnt, shape = self.st.offsets.get(k, (None, None, None))
+                if o is not None and o + cnt <= self.st.n_train:
+                    sd[k] = flat[o:o + cnt].view(shape)
+                else:
+                    sd[k] = v.detach().to("cpu", copy=True)
+            out.append(sd)
+        return out
+
+    def phema_snapshot(self):
+        """What post-hoc EMA reconstruction reads: {step, origin, profiles: [{sigma_rel, gamma, ema}]}, where step is
+        the run step of the last update and each ema a state dict."""
+        if self.phema_origin is None:
+            raise ValueError("the post-hoc EMA profiles have not been updated yet")
+        return {"step": self.phema_origin + self.phema_steps, "origin": self.phema_origin,
+                "profiles": [{"sigma_rel": s, "gamma": g, "ema": sd} for s, g, sd in
+                             zip(self.phema_sigma_rels, self.phema_gammas, self.phema_state_dicts())]}
 
     def close(self):
         """Release the communicator (a TrainStep owns one when world > 1 and collective == 'mdt')."""
@@ -329,10 +398,12 @@ class TrainStep:
             ops.adamw_ema_guarded(st.w32[lo:hi], g, self.m[lo:hi], self.v[lo:hi], ema, st.w16[lo:hi], n, self._lr_now,
                                   self._flag, self._counts, self.betas[0], self.betas[1], self.eps, self.wd,
                                   self.ema_decay, self._grad_scale, max_blocks)
-            return
-        ops.adamw_ema(st.w32[lo:hi], g, self.m[lo:hi], self.v[lo:hi], ema, st.w16[lo:hi], n, self._lr_now,
-                      self.step_count, self.betas[0], self.betas[1], self.eps, self.wd, self.ema_decay,
-                      self._grad_scale, max_blocks)
+        else:
+            ops.adamw_ema(st.w32[lo:hi], g, self.m[lo:hi], self.v[lo:hi], ema, st.w16[lo:hi], n, self._lr_now,
+                          self.step_count, self.betas[0], self.betas[1], self.eps, self.wd, self.ema_decay,
+                          self._grad_scale, max_blocks)
+        if self.phema_emas:   # the profiles follow the range's new (or, skipped, unchanged) weights on the same stream
+            ops.power_ema(st.w32[lo:hi], [e[lo:hi] for e in self.phema_emas], self._phema_c)
 
     def _on_grads_ready(self, lo, hi):
         """Called (on the host, from inside mdt_backward) when the kernels finalising gradient elements [lo, hi) of one
@@ -421,6 +492,11 @@ class TrainStep:
         self._lr_now = lr_at(self.step_count + self.lr_step_offset, self.lr, gb, self.rampup) \
             if self.reference_lr_schedule else self.lr
         self.step_count += 1
+        if self.phema_emas:
+            if self.phema_origin is None:
+                self.phema_origin = self.step_count - 1 + self.lr_step_offset
+            self.phema_steps += 1
+            self._phema_c = [phema.one_minus_beta(g, self.phema_steps) for g in self.phema_gammas]
         guard = self._flag is not None
         if guard:
             self._flag.zero_()

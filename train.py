@@ -15,6 +15,9 @@ data.mdb); `--wds` reads WebDataset tar shards instead (the reference's train_wd
 moments of the configured shape (no dataset on the bench boxes).  Either
 way the moments -> latent sampling, label dropout and noise injection run as ONE fused kernel (`ops.step_front`),
 gradient accumulation (`train.grad_accum`) and the lr ramp follow train.py:211-227.
+Post-hoc EMA (not in the reference): `--phema_sigma_rel 0.05,0.10` keeps power-function EMA profiles next to the
+reference-fixed EMA, the checkpoints carry them, and `--phema_every N` writes snapshots that posthoc_ema.py combines
+into the EMA of any width after the run.
 """
 import argparse
 import copy
@@ -52,6 +55,10 @@ def skip_nonfinite(args):
     return not args.no_amp
 
 
+def parse_sigma_rels(s):
+    return tuple(float(v) for v in s.split(",") if v.strip())
+
+
 def build_parser():
     ap = argparse.ArgumentParser("training parameters")
     ap.add_argument("--config", required=True)
@@ -72,6 +79,11 @@ def build_parser():
     ap.add_argument("--wds", action="store_true",
                     help="data.root holds WebDataset .tar shards (the reference's train_wds.py twin: lmdb2wds.py layout)")
     ap.add_argument("--max_steps", type=int, default=None, help="stop after this many steps (smoke runs)")
+    ap.add_argument("--phema_sigma_rel", type=parse_sigma_rels, default=(),
+                    help="keep power-function EMA profiles of these relative widths for post-hoc EMA, e.g. 0.05,0.10")
+    ap.add_argument("--phema_every", type=int, default=0,
+                    help="write a snapshot of the profiles to <results_dir>/phema/phema-<step>.pt every N steps "
+                         "(posthoc_ema.py combines them into any EMA width after the run)")
     return ap
 
 
@@ -107,10 +119,19 @@ def main():
         step0 = int(os.path.basename(ck)[:-3]) if os.path.basename(ck)[:-3].isdigit() else 0
     ts = TrainStep(net, ema, lr=cfg.train.lr, lr_rampup_kimg=cfg.train.lr_rampup_kimg, global_batch=global_batch,
                    loss_fn=Losses[cfg.model.precond](), reference_lr_schedule=True,
-                   skip_nonfinite=skip_nonfinite(args))
+                   skip_nonfinite=skip_nonfinite(args), phema_sigma_rels=args.phema_sigma_rel)
     if ck and strict and "opt" in sd:                      # train.py:150: optimizer state only under strict loading
         ts.load_state_dict(sd["opt"])
     ts.lr_step_offset = step0 - ts.step_count              # lr follows the run's step counter (train.py:223)
+    if args.phema_every and not ts.phema_emas:
+        raise SystemExit("--phema_every needs --phema_sigma_rel")
+    if rank == 0 and ts.phema_emas:
+        if ts.phema_origin is None:   # a fresh run, or a checkpoint without profiles: they start at this step
+            print(f"Post-hoc EMA: new profiles of sigma_rel {list(ts.phema_sigma_rels)} "
+                  f"(gamma {[round(g, 3) for g in ts.phema_gammas]}) from step {step0}", flush=True)
+        else:
+            print(f"Post-hoc EMA: continuing the profiles of sigma_rel {list(ts.phema_sigma_rels)} from step "
+                  f"{ts.phema_origin}", flush=True)
     ratio_fn = mask_ratio_schedule(cfg.model.get("mask_ratio_fn", "constant"), cfg.model.mask_ratio,
                                    cfg.model.get("mask_ratio_min", 0) or 0)
     drop = cfg.model.get("class_dropout_prob", 0) or 0
@@ -171,6 +192,13 @@ def main():
                            os.path.join(d, f"{step:07d}.pt"))
             if world > 1:
                 dist.barrier()
+        if args.phema_every and step % args.phema_every == 0 and step > step0 and rank == 0:
+            # every rank holds the same profiles; rank 0 writes them
+            d = os.path.join(args.results_dir, "phema")
+            os.makedirs(d, exist_ok=True)
+            path = os.path.join(d, f"phema-{step:07d}.pt")
+            torch.save(ts.phema_snapshot(), path)
+            print(f"(step={step:07d}) Post-hoc EMA snapshot (origin {ts.phema_origin}): {path}", flush=True)
     if world > 1:
         dist.destroy_process_group()
 
