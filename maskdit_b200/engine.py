@@ -191,11 +191,8 @@ class Engine:
         return X2, saved
 
     # ------------------------------------------------------------------------------------------------------
-    def backward(self, ctx, dF16, on_ready=None):
-        """Accumulate d(loss)/d(params) into the flat gradient buffer given dF [B*L, pd] bf16.
-        `on_ready(lo, hi)` (optional) is called as soon as the gradient elements [lo, hi) are final, i.e. right after
-        the kernels of a block's backward have been enqueued: the training step uses it to overlap the gradient
-        all-reduce and the optimizer with the rest of the backward (what DDP buckets do in the reference)."""
+    def backward(self, ctx, dF16):
+        """Accumulate d(loss)/d(params) into the flat gradient buffer given dF [B*L, pd] bf16."""
         cfg, st = self.cfg, self.store
         st.ensure_grad()
         G = st.gview
@@ -236,8 +233,6 @@ class Engine:
             for i, (spec, saved) in enumerate(zip(dec, dec_sv)):
                 nxt = self._mlp_gate(dec[i + 1], dec_sv[i + 1], mod, dmod) if i + 1 < len(dec) else None
                 dy2 = self._block_bwd(spec, saved, Gz, mod, dmod, B, L, dy2, nxt)
-                if on_ready is not None:
-                    on_ready(*st.prefix_range(spec.prefix + "."))
             # ---- unmask + decoder layer
             tok_g = G("model.mask_token").view(Dd) if "model.mask_token" in st.offsets and \
                 ctx["ids_restore"] is not None else None
@@ -259,8 +254,6 @@ class Engine:
         for i, (spec, saved) in enumerate(zip(enc, enc_sv)):
             nxt = self._mlp_gate(enc[i + 1], enc_sv[i + 1], mod, dmod) if i + 1 < len(enc) else None
             dy2 = self._block_bwd(spec, saved, Ge, mod, dmod, B, T, dy2, nxt)
-            if on_ready is not None:
-                on_ready(*st.prefix_range(spec.prefix + "."))
         # ---- patch embedding (no input gradient needed)
         ops.patch_embed_bwd(ctx["x_in"], ctx["sigma"], cfg.sigma_data, ctx["ids_keep"], Ge.view(B, T, D),
                             G("model.x_embedder.proj.weight").view(D, -1), G("model.x_embedder.proj.bias"), p)
@@ -492,16 +485,14 @@ class CEngine:
                        T=T, recompute=r)
         return Fo, ctx
 
-    def backward(self, ctx, dF16, on_ready=None):
+    def backward(self, ctx, dF16):
         st = self.store
         st.ensure_grad()
         ops._c(dF16, bf16)
         ops.L.sync_deterministic()
         self.set_recompute(ctx["recompute"])   # the plan the forward laid the workspace out with
-        cb =ops.L.GRAD_READY_FN(lambda user, lo, hi: on_ready(lo, hi)) if on_ready is not None \
-            else ops.L.GRAD_READY_FN()
         ops.check(self._L.mdt_backward(self._h, ops.ptr(st.w32), ops.ptr(st.w16), ops.ptr(st.grad), ops.ptr(ctx["x_in"]),
                                        ops.ptr(ctx["sigma"]), ops.ptr(ctx["ids_keep"]), ops.ptr(ctx["ids_restore"]),
-                                       ops.ptr(dF16), ctx["B"], ctx["T"], ops.ptr(ctx["ws"]), ctx["nbytes"], cb, None,
-                                       ops.stream_ptr()), "mdt_backward",
+                                       ops.ptr(dF16), ctx["B"], ctx["T"], ops.ptr(ctx["ws"]), ctx["nbytes"],
+                                       ops.L.GRAD_READY_FN(), None, ops.stream_ptr()), "mdt_backward",
                   self._count(ctx["ids_restore"] is not None, ctx["recompute"])[1])

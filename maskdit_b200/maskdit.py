@@ -188,7 +188,6 @@ class EDMPrecond(nn.Module):
                                             num_classes=num_classes, **model_kwargs)
         self._store, self._engine, self._anchor = None, None, None
         self._graphs = {}  # CUDA graphs of the eval-mode forward, keyed by input shapes (see _eval_graphed)
-        self._grad_ready_hook = None  # set by TrainStep: called with (lo, hi) when a gradient range is final
 
     # -- engine plumbing ---------------------------------------------------------------------------------------
     def _cfg(self):
@@ -248,7 +247,7 @@ class EDMPrecond(nn.Module):
             for k, p in params.items():
                 if p.requires_grad:
                     p.grad = st.gview(k)
-        self._engine.backward(saved, dF16, on_ready=self._grad_ready_hook)
+        self._engine.backward(saved, dF16)
 
     def __deepcopy__(self, memo):
         new = EDMPrecond(**copy.deepcopy(self._ctor))

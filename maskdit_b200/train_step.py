@@ -5,11 +5,9 @@ One process per GPU.  A step is:
     zero flat grad  ->  fused EDM loss forward/backward (C++ step driver)  ->  sum-all-reduce of the flat gradient
     buffer over NVLink (`GradComm`: our own NCCL communicator behind the C ABI; the 1/world factor is folded into the
     optimizer kernel)  ->  fused AdamW + EMA + bf16-shadow kernel over the flat buffers.
-`overlap=False`: literally one all-reduce after the backward and one optimizer launch.  `overlap=True`: a block's
-gradient range is exchanged on a side stream as soon as its backward is enqueued (the role DDP's bucketed hooks play in
-the reference), through a communicator confined to a few CTAs while the persistent GEMM grids leave those SMs free
-(`mdt_set_sm_budget`), then one optimizer pass.  No other collective is issued in the step (SURVEY.md §8e); the loss is
-returned as a device tensor (no per-step `.item()` host sync as at train.py:227).
+At world > 1 the all-reduce runs after the backward in `ar_chunks` chunks on a side stream, the optimizer pass of chunk
+k running on the main stream while chunk k+1 is on the wire.  No other collective is issued in the step (SURVEY.md
+§8e); the loss is returned as a device tensor (no per-step `.item()` host sync as at train.py:227).
 """
 from __future__ import annotations
 
@@ -73,10 +71,9 @@ def ar_chunk_bounds(n, k):
 class GradComm:
     """The step's gradient exchange behind the C ABI (`mdt_nccl_*`, `mdt_allreduce_grads`, csrc/driver.cu): an NCCL
     communicator of our own, created from a unique id that rank 0 draws and `torch.distributed` merely ships to the
-    other ranks (any backend; it is the bootstrap side channel, nothing else).  `max_ctas` > 0 confines the
-    communicator's kernels to that many CTAs so that they run NEXT TO the backward instead of after it."""
+    other ranks (any backend; it is the bootstrap side channel, nothing else)."""
 
-    def __init__(self, pg=None, max_ctas=0):
+    def __init__(self, pg=None):
         import ctypes
         self.rank, self.world = dist.get_rank(pg), dist.get_world_size(pg)
         L = ops.lib()
@@ -86,9 +83,8 @@ class GradComm:
         box = [bytes(buf.raw)]
         dist.broadcast_object_list(box, src=dist.get_global_rank(pg, 0) if pg is not None else 0, group=pg)
         self._comm = ctypes.c_void_p()
-        ops.check(L.mdt_nccl_comm_create(box[0], self.rank, self.world, int(max_ctas), ctypes.byref(self._comm)),
+        ops.check(L.mdt_nccl_comm_create(box[0], self.rank, self.world, 0, ctypes.byref(self._comm)),
                   "mdt_nccl_comm_create", 0)
-        self.max_ctas = max_ctas
 
     def all_reduce(self, t):
         """In-place SUM over the ranks of a contiguous fp32 / bf16 device tensor, on the current stream."""
@@ -108,7 +104,7 @@ class TrainStep:
     def __init__(self, net: EDMPrecond, ema: EDMPrecond | None = None, lr=1e-4, betas=(0.9, 0.999), eps=1e-8,
                  weight_decay=0.0, ema_decay=0.9999, loss_fn: EDMLoss | None = None, process_group=None,
                  lr_rampup_kimg=0.0, global_batch=None, device=None, overlap=False, graph=None,
-                 reference_lr_schedule=False, collective=None, grad_dtype=None, comm_ctas=None, skip_nonfinite=False,
+                 reference_lr_schedule=False, collective=None, grad_dtype=None, skip_nonfinite=False,
                  recompute_blocks=None, phema_sigma_rels=()):
         """phema_sigma_rels: relative widths of power-function EMA profiles to keep for post-hoc EMA (`phema.py`,
         posthoc_ema.py), e.g. (0.05, 0.10); at most 4.  Each is one fp32 buffer over the trainable region (2.92 GB for XL/2),
@@ -126,9 +122,12 @@ class TrainStep:
         skip_nonfinite:skip every optimizer step whose gradient holds an inf or NaN, as the reference's fp16
         GradScaler does (train.py:39-48): the weights, the bf16 shadow, the moments and Adam's step count stay as they
         are, the EMA still moves toward the unchanged weights (train.py:230), and the lr schedule's counter
-        (`step_count`) advances as for any attempted step.  The gradient checked is the one the optimizer consumes
-        (the summed one at world > 1; with bf16 exchange the bf16 values, checked while they are cast).  The decision
-        is a device flag that every rank ORs in (no host synchronisation); Adam's step count lives on the device
+        (`step_count`) advances as for any attempted step.  At world 1 the flat gradient is checked; at world > 1
+        each rank checks its local values before the exchange (with bf16 exchange the bf16 values, checked while they
+        are cast) and one flag word is summed over the ranks, so a non-finite value on any rank skips the step
+        everywhere (with `MDT_AR_CHUNKS=1` and fp32 exchange this replaces an earlier check of the summed buffer, which
+        could also flag finite values whose sum overflows).  The decision is a device flag (no host
+        synchronisation); Adam's step count lives on the device
         (`applied_steps()`), the number of skipped steps in `skipped_steps`.  Off by default: the step is then
         exactly the unguarded one.
         Multi-GPU options (world > 1; SURVEY 8e: the step's ONLY collective is the sum of the flat gradient buffer):
@@ -138,11 +137,16 @@ class TrainStep:
                       the links instead of 2.92 GB and the optimizer kernel reads the bf16 sums; local
                       accumulation, moments and master weights stay fp32.  2-rank vs 1-GPU gradient rel-L2 2.3e-3.
                       'fp32': the 2.92 GB buffer is reduced as is (DDP's arithmetic; rel-L2 1e-5, order noise).
-          overlap     the exchange of a block's gradients starts as soon as its backward is enqueued, on a side stream,
-                      through a communicator confined to `comm_ctas` CTAs while the persistent GEMM grids are sized
-                      for (SMs - comm_ctas) (`mdt_set_sm_budget`; the other kernels' grids are not budgeted).  Off by
-                      default, kept for A/B.
-        Environment overrides: MDT_COLLECTIVE, MDT_GRAD_AR, MDT_OVERLAP, MDT_COMM_CTAS."""
+          The exchange runs after the backward in `ar_chunks` chunks (MDT_AR_CHUNKS, default 4) on a side stream, the
+          optimizer pass of chunk k on the main stream while chunk k+1 is on the wire.
+          overlap     only False is accepted: the exchange overlapped with the backward was removed (a C caller can
+                      still overlap through `mdt_backward`'s `on_ready` callback).  `self.overlap` stays readable
+                      and is always False, so code that inspects a TrainStep's configuration keeps working.
+        Environment overrides: MDT_COLLECTIVE, MDT_GRAD_AR, MDT_AR_CHUNKS."""
+        if overlap:
+            raise ValueError("overlap=True: the gradient exchange overlapped with the backward was removed; the "
+                             "exchange runs after the backward, chunked and pipelined with the optimizer")
+        self.overlap = False
         self.net, self.ema = net, ema
         self.lr, self.betas, self.eps, self.wd, self.ema_decay = lr, betas, eps, weight_decay, ema_decay
         self.loss_fn = loss_fn or EDMLoss()
@@ -174,36 +178,25 @@ class TrainStep:
         for k, p in net.named_parameters():  # .grad views into the flat buffer (optimizer-compatible)
             if p.requires_grad:
                 p.grad = self.st.gview(k)
-        # Overlap: gradient ranges are exchanged on a side stream as soon as a block's backward is enqueued.
         env = os.environ
-        self.overlap = bool(int(env["MDT_OVERLAP"])) if "MDT_OVERLAP" in env else bool(overlap)
         self.collective = env.get("MDT_COLLECTIVE") or collective or \
             ("mdt" if self.world > 1 and dist.get_backend(process_group) == "nccl" else "torch")
         self.grad_dtype = env.get("MDT_GRAD_AR") or grad_dtype or "bf16"
         assert self.collective in ("mdt", "torch") and self.grad_dtype in ("fp32", "bf16")
-        self.comm_ctas = int(env.get("MDT_COMM_CTAS", comm_ctas if comm_ctas is not None else 8))
         self.comm = None
-        self.comm_bg = None
         self.g16 = None
         if self.world > 1:
             if self.collective == "mdt":
-                self.comm = GradComm(process_group)               # full-width communicator (NVLS, all channels)
-                # a second communicator confined to a few CTAs carries the per-block chunks DURING the backward; the
-                # gradients that only become final at its very end (adaLN projections = 35 % of the volume, embeddings)
-                # go through the full-width one afterwards
-                self.comm_bg = GradComm(process_group, max_ctas=max(1, self.comm_ctas // 2)) if self.overlap else None
+                self.comm = GradComm(process_group)
             if self.grad_dtype == "bf16":
                 self.g16 = torch.empty(n, dtype=torch.bfloat16, device=dev)
-        self._sms = torch.cuda.get_device_properties(dev).multi_processor_count
         self.graph = (os.environ.get("MDT_TRAIN_GRAPH", "0") == "1") if graph is None else bool(graph)
         self._graphs = {}
         # gradient all-reduce in this many chunks on a side stream, the fused AdamW/EMA pass of chunk k running while
         # chunk k+1 is on the wire.
         self.ar_chunks = int(os.environ.get("MDT_AR_CHUNKS", "4"))
-        self.side = torch.cuda.Stream(device=dev, priority=-1) if self.overlap else None
-        self._done = []          # [lo, hi) ranges already handled in the current step
+        self.side = None         # the exchange's stream, created by the first step at world > 1
         self._lr_now = lr
-        net._grad_ready_hook = self._on_grads_ready if (self.overlap and self.world > 1) else None
         # non-finite guard: flag (fp32, 0 = finite; a SUM over the ranks is their OR), counts {applied, skipped}
         self.skip_nonfinite = bool(skip_nonfinite)
         self._flag = torch.zeros(1, dtype=torch.float32, device=dev) if self.skip_nonfinite else None
@@ -349,21 +342,17 @@ class TrainStep:
 
     def close(self):
         """Release the communicator (a TrainStep owns one when world > 1 and collective == 'mdt')."""
-        for c in (self.comm, self.comm_bg):
-            if c is not None:
-                c.close()
-        self.comm = self.comm_bg = None
-        self.net._grad_ready_hook = None
+        if self.comm is not None:
+            self.comm.close()
+        self.comm = None
 
     # -- gradient exchange + optimizer ------------------------------------------------------------------------------------
     def describe_collective(self):
         if self.world == 1:
             return "none (1 GPU)"
         how = "own NCCL communicator behind the C ABI (mdt_allreduce_grads)" if self.comm else "torch.distributed"
-        when = (f"per block during the backward on a side stream ({self.comm_ctas} comm CTAs, persistent grids sized "
-                f"for {self._sms - self.comm_ctas} SMs)") if self.overlap else (
-            f"after the backward in {self.ar_chunks} chunks on a side stream, pipelined with the optimizer pass"
-            if self.ar_chunks > 1 else "one flat call after the backward")
+        when = f"after the backward in {self.ar_chunks} chunks on a side stream, pipelined with the optimizer pass" \
+            if self.ar_chunks > 1 else "one flat call after the backward"
         return f"{self.grad_dtype} sum-all-reduce of the flat gradient buffer, {how}, {when}"
 
     def _cast(self, lo, hi):
@@ -372,23 +361,21 @@ class TrainStep:
             return ops.cast_bf16_check(self.st.grad[lo:hi], self._flag, out=self.g16[lo:hi])
         return ops.cast_bf16(self.st.grad[lo:hi], out=self.g16[lo:hi])
 
-    def _all_reduce(self, buf, background=False):
+    def _all_reduce(self, buf):
         if self.comm is not None:
-            (self.comm_bg if (background and self.comm_bg is not None) else self.comm).all_reduce(buf)
+            self.comm.all_reduce(buf)
         else:
             dist.all_reduce(buf, op=dist.ReduceOp.SUM, group=self.pg)
 
-    def _exchange(self, lo, hi, background=False, cast=True):
+    def _exchange(self, lo, hi, cast=True):
         """Sum gradient elements [lo, hi) over the ranks on the current stream (in `grad`, or in the bf16 buffer;
         cast=False: the bf16 buffer already holds this range's cast)."""
-        if hi <= lo or self.world == 1:
-            return
         buf = self.st.grad[lo:hi]
         if self.g16 is not None:
             buf = self._cast(lo, hi) if cast else self.g16[lo:hi]
-        self._all_reduce(buf, background)
+        self._all_reduce(buf)
 
-    def _step_range(self, lo, hi, max_blocks=0):
+    def _step_range(self, lo, hi):
         st, n = self.st, hi - lo
         if n <= 0:
             return
@@ -397,24 +384,13 @@ class TrainStep:
         if self._flag is not None:   # Adam's step number comes from the device counter, the skip from the flag
             ops.adamw_ema_guarded(st.w32[lo:hi], g, self.m[lo:hi], self.v[lo:hi], ema, st.w16[lo:hi], n, self._lr_now,
                                   self._flag, self._counts, self.betas[0], self.betas[1], self.eps, self.wd,
-                                  self.ema_decay, self._grad_scale, max_blocks)
+                                  self.ema_decay, self._grad_scale)
         else:
             ops.adamw_ema(st.w32[lo:hi], g, self.m[lo:hi], self.v[lo:hi], ema, st.w16[lo:hi], n, self._lr_now,
                           self.step_count, self.betas[0], self.betas[1], self.eps, self.wd, self.ema_decay,
-                          self._grad_scale, max_blocks)
+                          self._grad_scale)
         if self.phema_emas:   # the profiles follow the range's new (or, skipped, unchanged) weights on the same stream
             ops.power_ema(st.w32[lo:hi], [e[lo:hi] for e in self.phema_emas], self._phema_c)
-
-    def _on_grads_ready(self, lo, hi):
-        """Called (on the host, from inside mdt_backward) when the kernels finalising gradient elements [lo, hi) of one
-        block are enqueued: start their exchange behind them on the side stream."""
-        if not self._done:   # first block of this backward: from here on the persistent grids leave SMs to the side stream
-            ops.check(ops.lib().mdt_set_sm_budget(self._sms - self.comm_ctas), "mdt_set_sm_budget", 0)
-        main = torch.cuda.current_stream()
-        self.side.wait_stream(main)
-        with torch.cuda.stream(self.side):
-            self._exchange(lo, hi, background=True)
-        self._done.append((lo, hi))
 
     def _fwd_bwd_graphed(self, images, labels, mask_ratio, mae_loss_coef, loss_call, moments=False):
         """Gradient zeroing + loss forward + engine backward (~770 launches, 70 ms of host time) replayed from a CUDA
@@ -500,13 +476,10 @@ class TrainStep:
         guard = self._flag is not None
         if guard:
             self._flag.zero_()
-        self._done = []
         self._grad_scale = 1.0 / (self.world * grad_accum)
         if grad_accum > 1:
             if images.shape[0] % grad_accum:
                 raise ValueError(f"batch {images.shape[0]} is not divisible by grad_accum {grad_accum}")
-            if self.overlap:
-                raise ValueError("overlap=True steps block ranges during the backward: incompatible with grad_accum > 1")
             mb = images.shape[0] // grad_accum
             st.grad.zero_()
             losses = []
@@ -516,36 +489,21 @@ class TrainStep:
                 lr_.mean().backward()
                 losses.append(lr_.detach())
             loss = torch.cat(losses)
-        elif self.graph and not self.overlap and ops.L.GEMM_PROFILE is None:
+        elif self.graph and ops.L.GEMM_PROFILE is None:
             loss = self._fwd_bwd_graphed(images, labels, mask_ratio, mae_loss_coef, loss_call, moments)
         else:
             st.grad.zero_()
             loss = loss_call(self.net, images, labels, mask_ratio, mae_loss_coef)
-            loss.mean().backward()   # engine backward; with overlap=True block ranges are already being reduced/stepped
+            loss.mean().backward()   # engine backward
         main = torch.cuda.current_stream()
         n = st.n_train
-        # Under the guard the flag must be final before the first optimizer pass.  bf16 exchange: the casts check the
-        # local values and one word is then summed over the ranks.  fp32 exchange: the summed buffer is checked,
-        # except in the chunked pipeline, which checks the local gradients up front and sums the flag.
-        if self.overlap and self._done:
-            ops.check(ops.lib().mdt_set_sm_budget(0), "mdt_set_sm_budget", 0)
-            self.side.wait_stream(main)
-            with torch.cuda.stream(self.side):
-                cur = 0
-                for lo, hi in sorted(self._done) + [(n, n)]:   # the complement of the block ranges
-                    self._exchange(cur, lo)
-                    cur = max(cur, hi)
-                if guard and self.g16 is not None:
-                    self._all_reduce(self._flag)
-            main.wait_stream(self.side)
-            if guard and self.g16 is None:
-                ops.nonfinite_check(st.grad[:n], self._flag)
-            self._step_range(0, n)                   # ONE optimizer pass over the whole (reduced) buffer
-        elif self.world == 1:
+        # Under the guard the flag must be final before the first optimizer pass.  At world > 1 every rank checks its
+        # local values (bf16 exchange: while casting them) and one flag word is summed over the ranks.
+        if self.world == 1:
             if guard:
                 ops.nonfinite_check(st.grad[:n], self._flag)
             self._step_range(0, n)
-        elif self.ar_chunks > 1:
+        else:
             # pipeline the exposed all-reduce against the optimizer pass: chunk k is stepped while k+1 is on the wire
             if self.side is None:
                 self.side = torch.cuda.Stream(device=st.grad.device)
@@ -568,14 +526,6 @@ class TrainStep:
             for (lo, hi), ev in zip(bounds, evs):
                 main.wait_event(ev)
                 self._step_range(lo, hi)
-        else:
-            self._exchange(0, n)                     # one flat all-reduce ...
-            if guard:
-                if self.g16 is not None:
-                    self._all_reduce(self._flag)
-                else:
-                    ops.nonfinite_check(st.grad[:n], self._flag)
-            self._step_range(0, n)                   # ... + one optimizer pass
         if guard:
             ops.optim_guard_advance(self._flag, self._counts)
         st.mark_shadow_fresh(self.net._params())   # the kernel refreshed the bf16 shadow itself

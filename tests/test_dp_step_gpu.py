@@ -6,10 +6,12 @@
     pass, any grid cap).
 (b) The NCCL entry points of the C ABI on a one-rank communicator (plain and CTA-confined): a one-rank SUM is the
     identity, argument errors are statuses.
-(c) `TrainStep`'s world > 1 branches run in process as rank 0 of two ranks holding the same gradient
+(c) `TrainStep`'s world > 1 exchange run in process as rank 0 of two ranks holding the same gradient
     (`TwoIdenticalRanks`): which element ranges are exchanged, on which stream, under which SM budget, that nothing
     writes a range after its exchange started, and that the optimizer pass is exactly one AdamW pass over the summed
     buffer.
+(d) What a C caller that overlaps its own exchange with the backward relies on: `mdt_backward`'s `on_ready` reports
+    each block's range once it is final, and a backward under `mdt_set_sm_budget` computes the plain gradient.
 """
 import copy
 import ctypes
@@ -209,17 +211,15 @@ class Call:
     stream: int
     budget: int
     snap: torch.Tensor
-    background: bool
     rc: int
 
 
 class TwoIdenticalRanks:
     """Stand-in for `GradComm` on rank 0 of two ranks that hold the same gradient: records what it is handed, runs the
-    real one-rank `mdt_allreduce_grads`, then doubles the buffer (the exact sum of the two ranks).  Runs inside the
-    backward's ready callback, so it records and never raises."""
+    real one-rank `mdt_allreduce_grads`, then doubles the buffer (the exact sum of the two ranks)."""
 
-    def __init__(self, ts, comm, log, background):
-        self.ts, self.comm, self.log, self.background = ts, comm, log, background
+    def __init__(self, ts, comm, log):
+        self.ts, self.comm, self.log = ts, comm, log
 
     def all_reduce(self, t):
         from maskdit_b200 import ops
@@ -229,23 +229,20 @@ class TwoIdenticalRanks:
         snap = t.clone()                                # on the current stream: in stream order
         rc = L.mdt_allreduce_grads(self.comm, t.data_ptr(), t.numel(), int(t.dtype == bf16), ops.stream_ptr())
         self.log.append(Call(lo, lo + t.numel(), t.dtype, torch.cuda.current_stream().cuda_stream,
-                             L.mdt_get_sm_budget(), snap, self.background, rc))
+                             L.mdt_get_sm_budget(), snap, rc))
         t.mul_(2)
 
     def close(self):
         pass   # the communicators belong to the module's fixture
 
 
-def make_rank0_of_two(ts, comms, log, ar_chunks):
+def make_rank0_of_two(ts, comm, log, ar_chunks):
     """Turn a world-1 TrainStep into rank 0 of a two-rank job (tools/dp_equivalence.py flips the same fields back)."""
     ts.world = 2
-    ts.comm = TwoIdenticalRanks(ts, comms[0], log, False)
-    ts.comm_bg = TwoIdenticalRanks(ts, comms[4], log, True) if ts.overlap else None
+    ts.comm = TwoIdenticalRanks(ts, comm, log)
     if ts.grad_dtype == "bf16":
         ts.g16 = torch.empty(ts.st.n_train, dtype=bf16, device="cuda")
     ts.ar_chunks = ar_chunks
-    if ts.overlap:
-        ts.net._grad_ready_hook = ts._on_grads_ready
 
 
 R, NCLS, B = 32, 1000, 4
@@ -299,17 +296,15 @@ def _net(use_decoder):
 MODES = {
     "bf16-flat": dict(grad_dtype="bf16", ar_chunks=1),
     "bf16-chunked": dict(grad_dtype="bf16", ar_chunks=4),
-    "bf16-overlap": dict(grad_dtype="bf16", overlap=True),
     "fp32-flat": dict(grad_dtype="fp32", ar_chunks=1),
     "fp32-chunked": dict(grad_dtype="fp32", ar_chunks=4),
-    "fp32-overlap": dict(grad_dtype="fp32", overlap=True),
     "bf16-chunked-graph": dict(grad_dtype="bf16", ar_chunks=4, graph=True),
     "bf16-chunked-accum2": dict(grad_dtype="bf16", ar_chunks=4, grad_accum=2),
     "fp32-flat-lr-schedule": dict(grad_dtype="fp32", ar_chunks=1, reference_lr_schedule=True),
-    "nodecoder-bf16-overlap": dict(grad_dtype="bf16", overlap=True, use_decoder=False),
+    "nodecoder-bf16-chunked": dict(grad_dtype="bf16", ar_chunks=4, use_decoder=False),
     "nodecoder-fp32-chunked": dict(grad_dtype="fp32", ar_chunks=4, use_decoder=False),
 }
-ENV = ("MDT_OVERLAP", "MDT_GRAD_AR", "MDT_COLLECTIVE", "MDT_COMM_CTAS", "MDT_AR_CHUNKS", "MDT_TRAIN_GRAPH")
+ENV = ("MDT_GRAD_AR", "MDT_COLLECTIVE", "MDT_AR_CHUNKS", "MDT_TRAIN_GRAPH")
 
 
 def _block_ranges_backward_order(net, st):
@@ -326,18 +321,16 @@ def test_train_step_world2_exchange(ops, comms, sm_budget, monkeypatch, mode):
         monkeypatch.delenv(k, raising=False)
     kw = dict(MODES[mode])
     use_decoder, ga = kw.pop("use_decoder", True), kw.pop("grad_accum", 1)
-    chunks, overlap = kw.pop("ar_chunks", 4), kw.get("overlap", False)
+    chunks = kw.pop("ar_chunks")
     bf = kw["grad_dtype"] == "bf16"
     images, labels, Draws = _draws()
     net = _net(use_decoder)
     ema = copy.deepcopy(net).eval()
     ts = TrainStep(net, ema, lr=LR, weight_decay=0.01, loss_fn=Draws(), global_batch=2 * B, **kw)
+    assert ts.overlap is False
     log = []
-    make_rank0_of_two(ts, comms, log, chunks)
+    make_rank0_of_two(ts, comms[0], log, chunks)
     st, n, L = ts.st, ts.st.n_train, sm_budget
-    main = torch.cuda.current_stream().cuda_stream
-    blocks = _block_ranges_backward_order(net, st)
-    local_grad_step1 = None
     for step in (1, 2, 3):
         pre = {"w": st.w32[:n].clone(), "m": ts.m.clone(), "v": ts.v.clone(), "ema": ts.ema_st.w32[:n].clone()}
         log.clear()
@@ -346,29 +339,24 @@ def test_train_step_world2_exchange(ops, comms, sm_budget, monkeypatch, mode):
         what = f"{mode} step {step}"
         assert L.mdt_get_sm_budget() == 0, what
         assert log and all(c.rc == 0 for c in log), (what, [c.rc for c in log])
-        # 1. coverage: disjoint ranges that tile [0, n_train) exactly once
-        spans = sorted((c.lo, c.hi) for c in log)
+        # 1. coverage: the chunks, in order, tiling [0, n_train) exactly once
+        spans = [(c.lo, c.hi) for c in log]
         assert spans[0][0] == 0 and spans[-1][1] == n, (what, spans[:2], spans[-2:])
         assert all(a[1] == b[0] for a, b in zip(spans, spans[1:])), (what, spans)
+        assert spans == ar_chunk_bounds(n, chunks), (what, spans)
         assert all(c.dtype == (bf16 if bf else torch.float32) for c in log), what
-        bg = [c for c in log if c.background]
-        if overlap:
-            assert [(c.lo, c.hi) for c in bg] == blocks, what                 # each block, in backward order
-            assert all(c.background for c in log[:len(bg)]) and not any(c.background for c in log[len(bg):]), what
-        else:
-            assert not bg and [(c.lo, c.hi) for c in log] == (ar_chunk_bounds(n, chunks) if chunks > 1 else [(0, n)])
         # 2. finality: nothing writes a range after its exchange started
         for c in log:
             final = st.grad[c.lo:c.hi]
             ok = torch.equal(c.snap, final.to(bf16)) if bf else torch.equal(c.snap * 2, final)
-            assert ok, (what, "range written after its exchange started", c.lo, c.hi, c.background)
+            assert ok, (what, "range written after its exchange started", c.lo, c.hi)
         # 3. the exchange buffer holds the two-rank sum
         if bf:
             assert torch.equal(ts.g16, st.grad.to(bf16) * 2), what
-        # 4. streams and SM budget
+        # 4. streams and SM budget: every exchange on the side stream, the whole device's grids
         for c in log:
-            assert c.stream == (ts.side.cuda_stream if (overlap or chunks > 1) else main), (what, c.lo)
-            assert c.budget == ((ts._sms - ts.comm_ctas) if c.background else 0), (what, c.lo, c.budget)
+            assert c.stream == ts.side.cuda_stream, (what, c.lo)
+            assert c.budget == 0, (what, c.lo, c.budget)
         # 5. the optimizer: exactly one AdamW pass over the summed buffer
         if mode == "fp32-flat-lr-schedule" and step == 1:
             assert ts._lr_now == 0.0
@@ -379,26 +367,69 @@ def test_train_step_world2_exchange(ops, comms, sm_budget, monkeypatch, mode):
         for name, got, want in (("w32", st.w32[:n], pre["w"]), ("m", ts.m, pre["m"]), ("v", ts.v, pre["v"]),
                                 ("ema", ts.ema_st.w32[:n], pre["ema"]), ("w16", st.w16[:n], w16)):
             assert torch.equal(got, want), (what, name, "optimizer pass differs from one AdamW pass over the sum")
-        if step == 1:
-            local_grad_step1 = st.grad.clone() if bf else st.grad / 2
     ts.close()
-    if not overlap:
-        return
-    # 6. the backward under the SM budget computes the same local gradient as a plain one-GPU step
-    images, labels, Draws = _draws()
-    ref_net = _net(use_decoder)
-    ref = TrainStep(ref_net, None, lr=LR, loss_fn=Draws(), grad_dtype=kw["grad_dtype"])
-    ref.step(images, labels, 0.5, 0.1)
+
+
+# ---- (d) what a C caller overlapping its own exchange relies on ---------------------------------------------------------
+@pytest.mark.parametrize("use_decoder", [True, False], ids=["maskdit", "nodecoder"])
+def test_backward_on_ready_reports_each_block_once_final(ops, use_decoder):
+    """`mdt_backward`'s `on_ready(user, lo, hi)` reports each block's gradient range once, in backward order (decoder
+    blocks, then encoder blocks), and nothing writes a range after it was reported: a clone enqueued from the callback
+    on the backward's stream equals the final gradient."""
+    net = _net(use_decoder)
+    st = net.prepare()
+    st.ensure_grad().zero_()
+    ce, Lt = net._engine, net.model.num_patches
+    g = torch.Generator().manual_seed(3)
+    x = (torch.randn(B, 4, R, R, generator=g) * 0.5).cuda()
+    sigma = (torch.rand(B, generator=g) + 0.5).cuda()
+    labels = torch.nn.functional.one_hot(torch.randint(0, NCLS, (B,), generator=g), NCLS).float().cuda()
+    mask = ops.mask_indices(torch.rand(B, Lt, generator=g).cuda(), Lt // 2)
+    dF = (torch.randn(B * Lt, ce.cfg.patch_dim, generator=g) * 0.1).to(bf16).cuda()
+    _, ctx = ce.forward(x, sigma, labels, mask, True)
+    seen = []
+
+    def on_ready(user, lo, hi):   # runs inside mdt_backward: records, never raises
+        seen.append((lo, hi, st.grad[lo:hi].clone()))
+
+    cb, p = ops.L.GRAD_READY_FN(on_ready), ops.ptr
+    rc = ce._L.mdt_backward(ce._h, p(st.w32), p(st.w16), p(st.grad), p(ctx["x_in"]), p(ctx["sigma"]),
+                            p(ctx["ids_keep"]), p(ctx["ids_restore"]), p(dF), ctx["B"], ctx["T"], p(ctx["ws"]),
+                            ctx["nbytes"], cb, None, ops.stream_ptr())
     torch.cuda.synchronize()
-    assert ref.st.offsets == st.offsets
+    assert rc == 0
+    assert [(lo, hi) for lo, hi, _ in seen] == _block_ranges_backward_order(net, st)
+    for lo, hi, snap in seen:
+        assert snap.abs().max().item() > 0, (lo, hi)
+        assert torch.equal(snap, st.grad[lo:hi]), ("range written after it was reported final", lo, hi)
+
+
+@pytest.mark.parametrize("use_decoder", [True, False], ids=["maskdit", "nodecoder"])
+def test_backward_under_sm_budget_matches_plain_step(ops, sm_budget, use_decoder):
+    """A step whose persistent GEMM grids are sized for 8 SMs fewer than the device has (`mdt_set_sm_budget`, which a
+    C caller sets to leave SMs to an exchange running next to the backward) computes the same gradient as a plain one:
+    every block tensor within 5e-5 of its scale, the conditioning path within 1e-2 (default-mode order noise)."""
+    from maskdit_b200.train_step import TrainStep
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    grads = {}
+    for budget in (sms - 8, 0):
+        images, labels, Draws = _draws()
+        ts = TrainStep(_net(use_decoder), None, lr=LR, loss_fn=Draws())
+        assert sm_budget.mdt_set_sm_budget(budget) == 0
+        ts.step(images, labels, 0.5, 0.1)
+        torch.cuda.synchronize()
+        assert sm_budget.mdt_get_sm_budget() == budget
+        grads[budget] = (ts.st, ts.st.grad.clone())
+    (st, budgeted), (ref_st, ref) = grads[sms - 8], grads[0]
+    assert ref_st.offsets == st.offsets
     worst = 0.0
     for k, (o, cnt, _) in st.offsets.items():
-        if o + cnt > n:
+        if o + cnt > st.n_train:
             continue
-        a, b = local_grad_step1[o:o + cnt], ref.st.grad[o:o + cnt]
+        a, b = budgeted[o:o + cnt], ref[o:o + cnt]
         scale = b.abs().max().item()
         err = (a - b).abs().max().item() / scale if scale > 0 else a.abs().max().item()
         cond = any(t in k for t in ("adaLN_modulation", "t_embedder", "y_embedder"))
         worst = max(worst, 0.0 if cond else err)
-        assert err <= (1e-2 if cond else 5e-5), (mode, k, err)
-    print(f"{mode}: budgeted backward vs one-GPU step, worst block-tensor deviation {worst:.2e}")
+        assert err <= (1e-2 if cond else 5e-5), (use_decoder, k, err)
+    print(f"use_decoder={use_decoder}: budgeted backward vs plain step, worst block-tensor deviation {worst:.2e}")

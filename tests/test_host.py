@@ -99,7 +99,7 @@ def test_flat_store_layout_from_driver():
     assert st.offsets["model.pos_embed"][0] >= st.n_train  # frozen tensors sit after the trainable region
     n_train = sum(v[1] for k, v in st.offsets.items() if not k.endswith("pos_embed"))
     assert n_train == 730_115_216  # SURVEY §2.2: trainable parameter count
-    # per-block gradient ranges (overlapped all-reduce/optimizer): contiguous, disjoint, inside the trainable region
+    # per-block gradient ranges (what mdt_backward's on_ready reports): contiguous, disjoint, inside the trainable region
     ranges = [st.prefix_range(f"model.blocks.{i}.") for i in range(28)] + \
              [st.prefix_range(f"model.decoder_blocks.{i}.") for i in range(8)]
     for (a0, a1), (b0, b1) in zip(sorted(ranges), sorted(ranges)[1:]):
@@ -120,6 +120,15 @@ def test_dp_helpers_and_schedule():
         b = ar_chunk_bounds(n, k)
         assert b[0][0] == 0 and b[-1][1] == n and all(x[1] == y[0] for x, y in zip(b, b[1:]))
         assert all(lo % 1024 == 0 for lo, _ in b) and len(b) <= max(k, 1)
+
+
+def test_train_step_refuses_overlap():
+    """The exchange overlapped with the backward was removed: asking for it is an error, not a silent change."""
+    from maskdit_b200.maskdit import Precond_models
+    from maskdit_b200.train_step import TrainStep
+    net = Precond_models["edm"](8, 4, num_classes=10, model_type="DiT-S/2", use_decoder=True, mae_loss_coef=0.1)
+    with pytest.raises(ValueError, match="overlap"):
+        TrainStep(net, None, overlap=True)
 
 
 def _gloo_worker(rank, world, port, q):

@@ -4,7 +4,7 @@
 2. The guarded AdamW entries: bit-identical to the unguarded ones with the flag clear; only the EMA moves with it set.
 3. Exact skip: under the deterministic mode a run that skips a poisoned batch equals, bit for bit, a run that never saw
    it (world 1, CUDA graph, gradient accumulation, and rank 0 of two emulated ranks in the exchange modes).
-4. Consensus: a non-finite contribution of the other rank makes this rank skip (a real two-process run needs two GPUs).
+4. Consensus: the other rank's flag makes this rank skip (a real two-process run needs two GPUs).
 5. Resume after a skip equals an uninterrupted run; the checkpoint carries Adam's applied step count.
 6. train.py end to end with a loader that yields one NaN batch, with and without --no_amp.
 """
@@ -219,25 +219,16 @@ def test_guarded_adamw_flag_set_moves_only_the_ema(ops, fp32_grad):
 
 
 # ---- the emulated second rank ----------------------------------------------------------------------------------------------
-def _one_rank_comm(L, max_ctas):
-    uid = ctypes.create_string_buffer(128)
-    assert L.mdt_nccl_unique_id(uid) == 0
-    comm = ctypes.c_void_p()
-    assert L.mdt_nccl_comm_create(bytes(uid.raw), 0, 1, max_ctas, ctypes.byref(comm)) == 0 and comm.value
-    return comm
-
-
 class Peer:
-    """What the other rank contributes: its flag word, and whether its gradient holds a NaN (element 0)."""
+    """What the other rank contributes to the summed flag word."""
 
-    def __init__(self, flag=0.0, nan_grad=False):
-        self.flag, self.nan_grad = flag, nan_grad
+    def __init__(self, flag=0.0):
+        self.flag = flag
 
 
 class RankZeroOfTwo:
     """`GradComm` stand-in on rank 0 of two ranks: runs the real one-rank `mdt_allreduce_grads`, then adds the other
-    rank's contribution (the same gradient, or the peer's flag word).  Runs inside the backward's ready callback, so it
-    records its statuses and never raises."""
+    rank's contribution (the same gradient, or the peer's flag word).  Records the statuses for the fixture to check."""
 
     def __init__(self, ts, comm, peer, log):
         self.ts, self.comm, self.peer, self.log = ts, comm, peer, log
@@ -251,38 +242,37 @@ class RankZeroOfTwo:
             t.add_(self.peer.flag)
             return
         t.mul_(2)
-        base = self.ts.g16 if t.dtype == bf16 else self.ts.st.grad
-        if self.peer.nan_grad and t.data_ptr() == base.data_ptr():
-            t[0] = NAN
 
     def close(self):
         pass
 
 
 @pytest.fixture(scope="module")
-def comms(ops):
+def comm(ops):
+    """A one-rank communicator."""
     L = ops.lib()
-    cs = {0: _one_rank_comm(L, 0), 4: _one_rank_comm(L, 4)}
-    yield cs
-    for c in cs.values():
-        assert L.mdt_nccl_comm_destroy(c) == 0
+    uid = ctypes.create_string_buffer(128)
+    assert L.mdt_nccl_unique_id(uid) == 0
+    c = ctypes.c_void_p()
+    assert L.mdt_nccl_comm_create(bytes(uid.raw), 0, 1, 0, ctypes.byref(c)) == 0 and c.value
+    yield c
+    assert L.mdt_nccl_comm_destroy(c) == 0
 
 
 @pytest.fixture
-def rank0_of_two(comms):
-    """make(ts, peer): turn a world-1 TrainStep into rank 0 of a two-rank job; the statuses are checked at the end."""
+def rank0_of_two(comm):
+    """make(ts, peer, ar_chunks): turn a world-1 TrainStep into rank 0 of a two-rank job; the statuses are checked at
+    the end."""
     logs = []
 
-    def make(ts, peer):
+    def make(ts, peer, ar_chunks):
         log = []
         logs.append(log)
         ts.world = 2
-        ts.comm = RankZeroOfTwo(ts, comms[0], peer, log)
-        ts.comm_bg = RankZeroOfTwo(ts, comms[4], peer, log) if ts.overlap else None
+        ts.comm = RankZeroOfTwo(ts, comm, peer, log)
         if ts.grad_dtype == "bf16":
             ts.g16 = torch.empty(ts.st.n_train, dtype=bf16, device="cuda")
-        if ts.overlap:
-            ts.net._grad_ready_hook = ts._on_grads_ready
+        ts.ar_chunks = ar_chunks
         return ts
 
     yield make
@@ -297,12 +287,10 @@ MODES = {
     "graph": dict(graph=True),
     "accum2": dict(grad_accum=2),
     "bf16-chunked": dict(world2=True, grad_dtype="bf16", ar_chunks=4),
-    "fp32-flat": dict(world2=True, grad_dtype="fp32", ar_chunks=1),
-    "bf16-overlap": dict(world2=True, grad_dtype="bf16", overlap=True),
-    "fp32-overlap": dict(world2=True, grad_dtype="fp32", overlap=True),
+    "fp32-one-chunk": dict(world2=True, grad_dtype="fp32", ar_chunks=1),
     "fp32-chunked": dict(world2=True, grad_dtype="fp32", ar_chunks=4),
 }
-ENV = ("MDT_OVERLAP", "MDT_GRAD_AR", "MDT_COLLECTIVE", "MDT_COMM_CTAS", "MDT_AR_CHUNKS", "MDT_TRAIN_GRAPH")
+ENV = ("MDT_GRAD_AR", "MDT_COLLECTIVE", "MDT_AR_CHUNKS", "MDT_TRAIN_GRAPH")
 
 
 def _net(model):
@@ -349,8 +337,7 @@ def _trainstep(model, mode, rank0_of_two=None, peer=None, lr_rampup_kimg=0.0):
     ts = TrainStep(net, copy.deepcopy(net).eval(), lr=1e-3, weight_decay=0.01, global_batch=B * (2 if world2 else 1),
                    lr_rampup_kimg=lr_rampup_kimg, reference_lr_schedule=True, skip_nonfinite=True, **kw)
     if world2:
-        rank0_of_two(ts, peer or Peer())
-        ts.ar_chunks = chunks
+        rank0_of_two(ts, peer or Peer(), chunks)
     return ts, ga
 
 
@@ -434,11 +421,10 @@ def test_exact_skip_xl2(det, rank0_of_two, monkeypatch, mode):
 
 
 # ---- 4. consensus ------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("mode,peer", [("bf16-chunked", "flag"), ("bf16-overlap", "flag"), ("fp32-chunked", "flag"),
-                                       ("fp32-flat", "grad"), ("fp32-overlap", "grad")])
-def test_other_rank_nonfinite_makes_this_rank_skip(det, rank0_of_two, monkeypatch, mode, peer):
-    """This rank's gradients are finite; the other rank's flag (bf16 exchange, fp32 chunks: local checks, one summed
-    word) or its gradient (fp32 flat / overlap: the summed buffer is checked) is not."""
+@pytest.mark.parametrize("mode", ["bf16-chunked", "fp32-chunked", "fp32-one-chunk"])
+def test_other_rank_nonfinite_makes_this_rank_skip(det, rank0_of_two, monkeypatch, mode):
+    """This rank's gradients are finite, the other rank's are not: every rank checks its local values and one flag word
+    is summed over the ranks, so the other rank's flag makes this rank skip too."""
     for k in ENV:
         monkeypatch.delenv(k, raising=False)
     data = _batches("S/2", 2)
@@ -446,13 +432,13 @@ def test_other_rank_nonfinite_makes_this_rank_skip(det, rank0_of_two, monkeypatc
     ts, ga = _trainstep("S/2", mode, rank0_of_two, p)
     _step(ts, data[0], ga)
     before = _opt_state(ts)
-    p.flag, p.nan_grad = (1.0, False) if peer == "flag" else (0.0, True)
+    p.flag = 1.0
     loss = _step(ts, data[1], ga)
     torch.cuda.synchronize()
     assert torch.isfinite(loss).all()
     _assert_skip(before, _opt_state(ts), ts.ema_decay)
     assert ts._counts.tolist() == [1, 1] and int(ts.skipped_steps) == 1
-    p.flag, p.nan_grad = 0.0, False
+    p.flag = 0.0
     _step(ts, data[0], ga)
     assert ts._counts.tolist() == [2, 1]
     assert not torch.equal(before["w32"], ts.st.w32[:ts.st.n_train])

@@ -291,21 +291,16 @@ def test_resume_continues_the_profiles_bit_for_bit(det):
 
 
 # ---- 5. world > 1 ------------------------------------------------------------------------------------------------------------
-def _one_rank_comm(L, max_ctas):
+@pytest.fixture(scope="module")
+def comm(ops):
+    """A one-rank communicator."""
+    L = ops.lib()
     uid = ctypes.create_string_buffer(128)
     assert L.mdt_nccl_unique_id(uid) == 0
-    comm = ctypes.c_void_p()
-    assert L.mdt_nccl_comm_create(bytes(uid.raw), 0, 1, max_ctas, ctypes.byref(comm)) == 0 and comm.value
-    return comm
-
-
-@pytest.fixture(scope="module")
-def comms(ops):
-    L = ops.lib()
-    cs = {0: _one_rank_comm(L, 0), 4: _one_rank_comm(L, 4)}
-    yield cs
-    for c in cs.values():
-        assert L.mdt_nccl_comm_destroy(c) == 0
+    c = ctypes.c_void_p()
+    assert L.mdt_nccl_comm_create(bytes(uid.raw), 0, 1, 0, ctypes.byref(c)) == 0 and c.value
+    yield c
+    assert L.mdt_nccl_comm_destroy(c) == 0
 
 
 class TwoIdenticalRanks:
@@ -329,27 +324,23 @@ WORLD2 = {
     "bf16-chunked": dict(grad_dtype="bf16", ar_chunks=4),
     "bf16-flat": dict(grad_dtype="bf16", ar_chunks=1),
     "fp32-chunked": dict(grad_dtype="fp32", ar_chunks=4),
-    "bf16-overlap": dict(grad_dtype="bf16", overlap=True),
     "bf16-chunked-skip": dict(grad_dtype="bf16", ar_chunks=4, skip_nonfinite=True),
 }
 
 
 @pytest.mark.parametrize("mode", list(WORLD2))
-def test_world2_every_element_once_after_its_pass(ops, comms, monkeypatch, mode):
+def test_world2_every_element_once_after_its_pass(ops, comm, monkeypatch, mode):
     from maskdit_b200.train_step import ar_chunk_bounds
-    for k in ("MDT_OVERLAP", "MDT_GRAD_AR", "MDT_COLLECTIVE", "MDT_COMM_CTAS", "MDT_AR_CHUNKS", "MDT_TRAIN_GRAPH"):
+    for k in ("MDT_GRAD_AR", "MDT_COLLECTIVE", "MDT_AR_CHUNKS", "MDT_TRAIN_GRAPH"):
         monkeypatch.delenv(k, raising=False)
     kw = dict(WORLD2[mode])
-    chunks = kw.pop("ar_chunks", 4)
+    chunks = kw.pop("ar_chunks")
     ts = _trainstep(phema_sigma_rels=SIGMAS, **kw)
     ts.world = 2
-    ts.comm = TwoIdenticalRanks(comms[0])
-    ts.comm_bg = TwoIdenticalRanks(comms[4]) if ts.overlap else None
+    ts.comm = TwoIdenticalRanks(comm)
     if ts.grad_dtype == "bf16":
         ts.g16 = torch.empty(ts.st.n_train, dtype=bf16, device="cuda")
     ts.ar_chunks = chunks
-    if ts.overlap:
-        ts.net._grad_ready_hook = ts._on_grads_ready
     n = ts.st.n_train
     log = []
 
@@ -371,8 +362,7 @@ def test_world2_every_element_once_after_its_pass(ops, comms, monkeypatch, mode)
         pe = [(lo, hi, s) for name, lo, hi, s in log if name == "power_ema"]
         spans = sorted((lo, hi) for lo, hi, _ in pe)
         assert spans[0][0] == 0 and spans[-1][1] == n and all(a[1] == b_[0] for a, b_ in zip(spans, spans[1:])), what
-        want = ar_chunk_bounds(n, chunks) if (chunks > 1 and not ts.overlap) else [(0, n)]
-        assert spans == want, what
+        assert spans == ar_chunk_bounds(n, chunks), what
         # each update directly follows the optimizer pass over the same range, on its stream
         for i, (name, lo, hi, s) in enumerate(log):
             if name == "power_ema":
