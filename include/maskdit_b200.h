@@ -280,6 +280,48 @@ int mdt_adamw_ema_guarded_g16(float* w, const void* g_bf16, float* m, float* v, 
 int mdt_optim_guard_advance(const float* flag, long long* counts, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Gradient-norm clipping (torch.nn.utils.clip_grad_norm_; the reference does not clip, train.py:141,211-227).  The
+ * norm and the coefficient live on the device, so a clipped step needs no host synchronisation:
+ * mdt_grad_sumsq_scratch: the number of fp64 scratch slots mdt_grad_sumsq needs for n elements (>= 1; at most 2112
+ *   whatever n), or MDT_ERR_ARG for n <= 0.  Host only, no device.
+ * mdt_grad_sumsq: *out = sum of g[i]^2 over [0, n), g fp32 (bf16 = 0, 16-byte aligned) or bf16 (bf16 != 0, 8-byte
+ *   aligned), accumulated in fp64: per-block partials in `scratch` (8-byte aligned), then one block sums them into
+ *   *out (8-byte aligned) in a fixed order, without atomics.  The grid and the order depend on n alone, so the result
+ *   is bit-reproducible whatever mdt_set_sm_budget and mdt_set_deterministic say.  A fp32 square stays below fp64's
+ *   maximum: *out is finite exactly when every element is.  flag (may be NULL, 4-byte aligned): set to 1 when an
+ *   element is inf or NaN, with mdt_nonfinite_check's convention, so one read of g is both the check and the norm.
+ *   Two launches; calls on one stream may share `scratch`.
+ * mdt_grad_clip_coef (one thread): norm = fp32(grad_scale * sqrt(sum of sumsq[0, k) in index order)), the sum and the
+ *   product in fp64; coef = min(1, max_norm / (norm + 1e-6)) in fp32 as clip_grad_norm_ computes it
+ *   (reciprocal(norm + 1e-6) * max_norm, a NaN staying NaN).  max_norm = +inf measures only: coef = 1.  With a finite
+ *   max_norm and flag != NULL a non-finite norm sets the flag (a sum that overflowed although every rank's values were
+ *   finite).  MDT_ERR_ARG for a NULL sumsq / norm / coef, k < 1, grad_scale <= 0 or NaN, max_norm <= 0 or NaN, sumsq
+ *   not 8-byte or norm / coef / flag not 4-byte aligned.
+ * mdt_adamw_ema_coef(_g16), mdt_adamw_ema_guarded_coef(_g16): mdt_adamw_ema(_g16) / mdt_adamw_ema_guarded(_g16) with
+ *   the gradient scale grad_scale * *coef (coef: one fp32 word on the device, 4-byte aligned, read once
+ *   before the loop).  With *coef == 1 they compute the plain entries' bits.  Same arguments, alignment rules and grid
+ *   otherwise; MDT_ERR_ARG also for a NULL or misaligned coef.
+ * ------------------------------------------------------------------------------------------------------------ */
+int mdt_grad_sumsq_scratch(long long n);
+int mdt_grad_sumsq(const void* g, long long n, int bf16, double* scratch, double* out, float* flag, void* stream);
+int mdt_grad_clip_coef(const double* sumsq, int k, double grad_scale, float max_norm, float* norm, float* coef,
+                       float* flag, void* stream);
+int mdt_adamw_ema_coef(float* w, const float* g, float* m, float* v, float* ema, void* w_bf16, long long n, float lr,
+                       float beta1, float beta2, float eps, float weight_decay, int step, float ema_decay,
+                       float grad_scale, const float* coef, int max_blocks, void* stream);
+int mdt_adamw_ema_coef_g16(float* w, const void* g_bf16, float* m, float* v, float* ema, void* w_bf16, long long n,
+                           float lr, float beta1, float beta2, float eps, float weight_decay, int step, float ema_decay,
+                           float grad_scale, const float* coef, int max_blocks, void* stream);
+int mdt_adamw_ema_guarded_coef(float* w, const float* g, float* m, float* v, float* ema, void* w_bf16, long long n,
+                               float lr, float beta1, float beta2, float eps, float weight_decay, float ema_decay,
+                               float grad_scale, const float* coef, const float* flag, const long long* counts,
+                               int max_blocks, void* stream);
+int mdt_adamw_ema_guarded_coef_g16(float* w, const void* g_bf16, float* m, float* v, float* ema, void* w_bf16,
+                                   long long n, float lr, float beta1, float beta2, float eps, float weight_decay,
+                                   float ema_decay, float grad_scale, const float* coef, const float* flag,
+                                   const long long* counts, int max_blocks, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Power-function EMA profiles (post-hoc EMA, Karras et al., CVPR 2024, §3): k <= 4 fp32 profiles advanced from ONE
  * read of w[0, n):
  *   ema[j][i] += one_minus_beta[j] * (w[i] - ema[j][i])        (fp32, one fused multiply-add; c == 1 stores w exactly)

@@ -124,6 +124,14 @@ _SIGS = {
     "mdt_adamw_ema_guarded": [_P, _P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _F, _F, _F, _P, _P, _I, _P],
     "mdt_adamw_ema_guarded_g16": [_P, _P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _F, _F, _F, _P, _P, _I, _P],
     "mdt_optim_guard_advance": [_P, _P, _P],
+    # gradient-norm clipping (csrc/loss_optim.cu)
+    "mdt_grad_sumsq_scratch": [_LL],
+    "mdt_grad_sumsq": [_P, _LL, _I, _P, _P, _P, _P],
+    "mdt_grad_clip_coef": [_P, _I, _D, _F, _P, _P, _P, _P],
+    "mdt_adamw_ema_coef": [_P, _P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _F, _I, _F, _F, _P, _I, _P],
+    "mdt_adamw_ema_coef_g16": [_P, _P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _F, _I, _F, _F, _P, _I, _P],
+    "mdt_adamw_ema_guarded_coef": [_P, _P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _F, _F, _F, _P, _P, _P, _I, _P],
+    "mdt_adamw_ema_guarded_coef_g16": [_P, _P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _F, _F, _F, _P, _P, _P, _I, _P],
     # power-function EMA profiles (post-hoc EMA, csrc/loss_optim.cu)
     "mdt_power_ema": [_P, POINTER(c_void_p), POINTER(c_float), _I, _LL, _P],
 }

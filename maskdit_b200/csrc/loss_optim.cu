@@ -337,6 +337,124 @@ __global__ void optim_guard_advance_kernel(const float* __restrict__ flag, long 
   counts[*flag != 0.f ? 1 : 0] += 1;
 }
 
+// ---- Gradient-norm clipping (torch.nn.utils.clip_grad_norm_) ------------------------------------------------------------
+// The AdamW passes with the clip coefficient read from device memory: the gradient scale becomes grad_scale * *coef
+// before the loop, so *coef == 1 computes the plain kernels' bits.
+template <bool G16>
+__global__ void __launch_bounds__(256)
+adamw_ema_coef_kernel(float* __restrict__ w, const void* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+                      float* __restrict__ ema, __nv_bfloat16* __restrict__ w16, long long n, float lr, float b1,
+                      float b2, float eps, float wd, float inv_bc1, float inv_bc2, float ema_decay, float gscale,
+                      const float* __restrict__ coef) {
+  adamw_ema_pass<G16>(w, g, m, v, ema, w16, n, lr, b1, b2, eps, wd, inv_bc1, inv_bc2, ema_decay, gscale * *coef);
+}
+
+// adamw_ema_guarded_kernel's two branches with the scaled gradient (a skipped step reads neither g nor the scale).
+template <bool G16>
+__global__ void __launch_bounds__(256)
+adamw_ema_guarded_coef_kernel(float* __restrict__ w, const void* __restrict__ g, float* __restrict__ m,
+                              float* __restrict__ v, float* __restrict__ ema, __nv_bfloat16* __restrict__ w16,
+                              long long n, float lr, float b1, float b2, float eps, float wd, float ema_decay,
+                              float gscale, const float* __restrict__ coef, const float* __restrict__ flag,
+                              const long long* __restrict__ counts) {
+  if (*flag != 0.f) {
+    if (!ema) return;
+    const long long n4 = n >> 2;
+    const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n4; i += stride) {
+      const float4 wv = reinterpret_cast<const float4*>(w)[i];
+      float4 ev = reinterpret_cast<float4*>(ema)[i];
+      ev.x = ema_decay * ev.x + (1.f - ema_decay) * wv.x, ev.y = ema_decay * ev.y + (1.f - ema_decay) * wv.y;
+      ev.z = ema_decay * ev.z + (1.f - ema_decay) * wv.z, ev.w = ema_decay * ev.w + (1.f - ema_decay) * wv.w;
+      reinterpret_cast<float4*>(ema)[i] = ev;
+    }
+    return;
+  }
+  __shared__ float s_bc[3];
+  if (threadIdx.x == 0) {
+    const double step = static_cast<double>(counts[0] + 1);
+    s_bc[0] = static_cast<float>(1.0 / (1.0 - pow(static_cast<double>(b1), step)));
+    s_bc[1] = static_cast<float>(1.0 / (1.0 - pow(static_cast<double>(b2), step)));
+    s_bc[2] = gscale * *coef;
+  }
+  __syncthreads();
+  adamw_ema_pass<G16>(w, g, m, v, ema, w16, n, lr, b1, b2, eps, wd, s_bc[0], s_bc[1], ema_decay, s_bc[2]);
+}
+
+// Fixed-order fp64 block sum (xor-shuffle tree per warp, then warp 0 over the warp sums): the same bits on every run.
+MDT_DEVINL double block_sum_f64(double v, double* s_buf) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) s_buf[warp] = v;
+  __syncthreads();
+  double t = (threadIdx.x < (blockDim.x >> 5)) ? s_buf[threadIdx.x] : 0.0;
+  if (warp == 0) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+  }
+  return t;   // valid in thread 0
+}
+
+MDT_DEVINL double sq64(float x) { return static_cast<double>(x) * static_cast<double>(x); }
+
+// Per-block partial sums of squares of g[0, n) in fp64.  The grid and every thread's visiting order are functions of n
+// alone.  A fp32 square stays below fp64's maximum, so a thread's sum is non-finite exactly when it met an inf or NaN:
+// that is the non-finite check (flag != NULL), with flag_or's convention.
+template <bool G16>
+__global__ void __launch_bounds__(256) grad_sumsq_kernel(const void* __restrict__ g, long long n,
+                                                         double* __restrict__ partials, float* __restrict__ flag) {
+  __shared__ double s_buf[8];
+  const long long n4 = n >> 2;
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  const long long t = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  double acc = 0.0;
+  for (long long i = t; i < n4; i += stride) {
+    float4 x;
+    if constexpr (G16) {
+      const uint2 u = reinterpret_cast<const uint2*>(g)[i];
+      x = make_float4(bf16_lo(u.x), bf16_hi(u.x), bf16_lo(u.y), bf16_hi(u.y));
+    } else {
+      x = reinterpret_cast<const float4*>(g)[i];
+    }
+    acc += (sq64(x.x) + sq64(x.y)) + (sq64(x.z) + sq64(x.w));
+  }
+  for (long long i = (n4 << 2) + t; i < n; i += stride) {
+    if constexpr (G16) acc += sq64(__bfloat162float(reinterpret_cast<const __nv_bfloat16*>(g)[i]));
+    else acc += sq64(reinterpret_cast<const float*>(g)[i]);
+  }
+  if (flag) flag_or(!isfinite(acc), flag);
+  const double s = block_sum_f64(acc, s_buf);
+  if (threadIdx.x == 0) partials[blockIdx.x] = s;
+}
+
+// One block: out = the partials' sum in a fixed order (thread j takes partials j, j + 256, ... in index order).
+__global__ void __launch_bounds__(256) grad_sumsq_final_kernel(const double* __restrict__ partials, int nb,
+                                                               double* __restrict__ out) {
+  __shared__ double s_buf[8];
+  double acc = 0.0;
+  for (int i = threadIdx.x; i < nb; i += blockDim.x) acc += partials[i];
+  const double s = block_sum_f64(acc, s_buf);
+  if (threadIdx.x == 0) *out = s;
+}
+
+// norm = fp32(grad_scale * sqrt(sum of the k slots in index order)); coef as clip_grad_norm_ computes it in fp32:
+// clamp(reciprocal(norm + 1e-6) * max_norm, max = 1), NaN staying NaN; max_norm = inf measures only (coef = 1).
+__global__ void grad_clip_coef_kernel(const double* __restrict__ sumsq, int k, double grad_scale, float max_norm,
+                                      float* __restrict__ norm, float* __restrict__ coef, float* __restrict__ flag) {
+  double s = 0.0;
+  for (int i = 0; i < k; ++i) s += sumsq[i];
+  const float nrm = static_cast<float>(grad_scale * sqrt(s));
+  *norm = nrm;
+  float c = 1.f;
+  if (!isinf(max_norm)) {
+    const float q = (1.f / (nrm + 1e-6f)) * max_norm;
+    c = q > 1.f ? 1.f : q;
+    if (flag && !isfinite(nrm)) *flag = 1.f;
+  }
+  *coef = c;
+}
+
 // ---- Power-function EMA profiles (post-hoc EMA, Karras et al. CVPR 2024 §3) ---------------------------------------------
 // K profiles advanced from one read of w:  e += c_j * (w - e).  c_j == 1 (a profile's first step) stores w exactly.
 constexpr int kMaxPowerEma = 4;
@@ -497,7 +615,7 @@ int mdt_to_uint8_nhwc(const float* img, unsigned char* out, int B, int C, int H,
 
 static int adamw_launch(bool g16, float* w, const void* g, float* m, float* v, float* ema, void* w_bf16, long long n,
                         float lr, float beta1, float beta2, float eps, float weight_decay, int step, float ema_decay,
-                        float grad_scale, int max_blocks, void* stream) {
+                        float grad_scale, int max_blocks, void* stream, const float* coef = nullptr) {
   if (!w || !g || !m || !v || n <= 0 || step < 1 || (n & 3)) return MDT_ERR_ARG;
   // the kernel moves 4 elements per access: float4 for the fp32 buffers, uint2 for the bf16 ones
   const uintptr_t a16 = reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(m) |
@@ -510,6 +628,13 @@ static int adamw_launch(bool g16, float* w, const void* g, float* m, float* v, f
   long long blocks = (n / 4 + 255) / 256;
   if (blocks > kNumSMsDefault * 8) blocks = kNumSMsDefault * 8;
   if (max_blocks > 0 && blocks > max_blocks) blocks = max_blocks;
+  if (coef) {
+    auto kern = g16 ? adamw_ema_coef_kernel<true> : adamw_ema_coef_kernel<false>;
+    kern<<<static_cast<int>(blocks), 256, 0, S(stream)>>>(w, g, m, v, ema, static_cast<__nv_bfloat16*>(w_bf16), n,
+                                                          lr, beta1, beta2, eps, weight_decay, inv_bc1, inv_bc2,
+                                                          ema_decay, grad_scale, coef);
+    return launch_status();
+  }
   auto kern = g16 ? adamw_ema_kernel<true> : adamw_ema_kernel<false>;
   kern<<<static_cast<int>(blocks), 256, 0, S(stream)>>>(w, g, m, v, ema, static_cast<__nv_bfloat16*>(w_bf16), n, lr,
                                                         beta1, beta2, eps, weight_decay, inv_bc1, inv_bc2, ema_decay,
@@ -555,7 +680,7 @@ int mdt_cast_f32_bf16_check(const float* in, void* out_bf16, long long n, float*
 static int adamw_guarded_launch(bool g16, float* w, const void* g, float* m, float* v, float* ema, void* w_bf16,
                                 long long n, float lr, float beta1, float beta2, float eps, float weight_decay,
                                 float ema_decay, float grad_scale, const float* flag, const long long* counts,
-                                int max_blocks, void* stream) {
+                                int max_blocks, void* stream, const float* coef = nullptr) {
   if (!w || !g || !m || !v || !flag || !counts || n <= 0 || (n & 3)) return MDT_ERR_ARG;
   const uintptr_t a16 = reinterpret_cast<uintptr_t>(w) | reinterpret_cast<uintptr_t>(m) |
                         reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(ema) |
@@ -566,6 +691,13 @@ static int adamw_guarded_launch(bool g16, float* w, const void* g, float* m, flo
   long long blocks = (n / 4 + 255) / 256;
   if (blocks > kNumSMsDefault * 8) blocks = kNumSMsDefault * 8;
   if (max_blocks > 0 && blocks > max_blocks) blocks = max_blocks;
+  if (coef) {
+    auto kern = g16 ? adamw_ema_guarded_coef_kernel<true> : adamw_ema_guarded_coef_kernel<false>;
+    kern<<<static_cast<int>(blocks), 256, 0, S(stream)>>>(w, g, m, v, ema, static_cast<__nv_bfloat16*>(w_bf16), n,
+                                                          lr, beta1, beta2, eps, weight_decay, ema_decay, grad_scale,
+                                                          coef, flag, counts);
+    return launch_status();
+  }
   auto kern = g16 ? adamw_ema_guarded_kernel<true> : adamw_ema_guarded_kernel<false>;
   kern<<<static_cast<int>(blocks), 256, 0, S(stream)>>>(w, g, m, v, ema, static_cast<__nv_bfloat16*>(w_bf16), n, lr,
                                                         beta1, beta2, eps, weight_decay, ema_decay, grad_scale, flag,
@@ -593,6 +725,70 @@ int mdt_optim_guard_advance(const float* flag, long long* counts, void* stream) 
     return MDT_ERR_ARG;
   optim_guard_advance_kernel<<<1, 1, 0, S(stream)>>>(flag, counts);
   return launch_status();
+}
+
+// ---- gradient-norm clipping ---------------------------------------------------------------------------------------------
+int mdt_grad_sumsq_scratch(long long n) {
+  if (n <= 0) return MDT_ERR_ARG;
+  return check_grid(n);
+}
+
+int mdt_grad_sumsq(const void* g, long long n, int bf16, double* scratch, double* out, float* flag, void* stream) {
+  if (!g || !scratch || !out || n <= 0) return MDT_ERR_ARG;
+  const uintptr_t ag = reinterpret_cast<uintptr_t>(g);
+  if ((bf16 ? (ag & 7) : (ag & 15)) || ((reinterpret_cast<uintptr_t>(scratch) | reinterpret_cast<uintptr_t>(out)) & 7) ||
+      (reinterpret_cast<uintptr_t>(flag) & 3))
+    return MDT_ERR_ARG;
+  const int blocks = check_grid(n);
+  if (bf16) grad_sumsq_kernel<true><<<blocks, 256, 0, S(stream)>>>(g, n, scratch, flag);
+  else grad_sumsq_kernel<false><<<blocks, 256, 0, S(stream)>>>(g, n, scratch, flag);
+  if (int rc = launch_status()) return rc;
+  grad_sumsq_final_kernel<<<1, 256, 0, S(stream)>>>(scratch, blocks, out);
+  return launch_status();
+}
+
+int mdt_grad_clip_coef(const double* sumsq, int k, double grad_scale, float max_norm, float* norm, float* coef,
+                       float* flag, void* stream) {
+  if (!sumsq || !norm || !coef || k < 1 || !(grad_scale > 0.0) || !(max_norm > 0.f)) return MDT_ERR_ARG;
+  if ((reinterpret_cast<uintptr_t>(sumsq) & 7) ||
+      ((reinterpret_cast<uintptr_t>(norm) | reinterpret_cast<uintptr_t>(coef) | reinterpret_cast<uintptr_t>(flag)) & 3))
+    return MDT_ERR_ARG;
+  grad_clip_coef_kernel<<<1, 1, 0, S(stream)>>>(sumsq, k, grad_scale, max_norm, norm, coef, flag);
+  return launch_status();
+}
+
+int mdt_adamw_ema_coef(float* w, const float* g, float* m, float* v, float* ema, void* w_bf16, long long n, float lr,
+                       float beta1, float beta2, float eps, float weight_decay, int step, float ema_decay,
+                       float grad_scale, const float* coef, int max_blocks, void* stream) {
+  if (!coef || (reinterpret_cast<uintptr_t>(coef) & 3)) return MDT_ERR_ARG;
+  return adamw_launch(false, w, g, m, v, ema, w_bf16, n, lr, beta1, beta2, eps, weight_decay, step, ema_decay,
+                      grad_scale, max_blocks, stream, coef);
+}
+
+int mdt_adamw_ema_coef_g16(float* w, const void* g_bf16, float* m, float* v, float* ema, void* w_bf16, long long n,
+                           float lr, float beta1, float beta2, float eps, float weight_decay, int step, float ema_decay,
+                           float grad_scale, const float* coef, int max_blocks, void* stream) {
+  if (!coef || (reinterpret_cast<uintptr_t>(coef) & 3)) return MDT_ERR_ARG;
+  return adamw_launch(true, w, g_bf16, m, v, ema, w_bf16, n, lr, beta1, beta2, eps, weight_decay, step, ema_decay,
+                      grad_scale, max_blocks, stream, coef);
+}
+
+int mdt_adamw_ema_guarded_coef(float* w, const float* g, float* m, float* v, float* ema, void* w_bf16, long long n,
+                               float lr, float beta1, float beta2, float eps, float weight_decay, float ema_decay,
+                               float grad_scale, const float* coef, const float* flag, const long long* counts,
+                               int max_blocks, void* stream) {
+  if (!coef || (reinterpret_cast<uintptr_t>(coef) & 3)) return MDT_ERR_ARG;
+  return adamw_guarded_launch(false, w, g, m, v, ema, w_bf16, n, lr, beta1, beta2, eps, weight_decay, ema_decay,
+                              grad_scale, flag, counts, max_blocks, stream, coef);
+}
+
+int mdt_adamw_ema_guarded_coef_g16(float* w, const void* g_bf16, float* m, float* v, float* ema, void* w_bf16,
+                                   long long n, float lr, float beta1, float beta2, float eps, float weight_decay,
+                                   float ema_decay, float grad_scale, const float* coef, const float* flag,
+                                   const long long* counts, int max_blocks, void* stream) {
+  if (!coef || (reinterpret_cast<uintptr_t>(coef) & 3)) return MDT_ERR_ARG;
+  return adamw_guarded_launch(true, w, g_bf16, m, v, ema, w_bf16, n, lr, beta1, beta2, eps, weight_decay, ema_decay,
+                              grad_scale, flag, counts, max_blocks, stream, coef);
 }
 
 int mdt_power_ema(const float* w, float* const* ema, const float* one_minus_beta, int k, long long n, void* stream) {

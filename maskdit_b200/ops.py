@@ -244,7 +244,15 @@ def to_uint8_nhwc(img):
 
 
 def adamw_ema(w, g, m, v, ema, w16, n, lr, step, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0,
-              ema_decay=0.9999, grad_scale=1.0, max_blocks=0):
+              ema_decay=0.9999, grad_scale=1.0, max_blocks=0, coef=None):
+    """coef (one fp32 word on the device, or None): the gradient scale becomes grad_scale * coef (a clip
+    coefficient from `grad_clip_coef`)."""
+    if coef is not None:
+        _c(coef, f32)
+        fn = lib().mdt_adamw_ema_coef_g16 if g.dtype == bf16 else lib().mdt_adamw_ema_coef
+        check(fn(ptr(w), ptr(g), ptr(m), ptr(v), ptr(ema), ptr(w16), n, lr, beta1, beta2, eps, weight_decay, step,
+                 ema_decay, grad_scale, ptr(coef), max_blocks, stream_ptr()), "mdt_adamw_ema_coef")
+        return
     fn = lib().mdt_adamw_ema_g16 if g.dtype == bf16 else lib().mdt_adamw_ema   # bf16: all-reduced bf16 gradients
     check(fn(ptr(w), ptr(g), ptr(m), ptr(v), ptr(ema), ptr(w16), n, lr, beta1, beta2, eps, weight_decay, step,
              ema_decay, grad_scale, max_blocks, stream_ptr()), "mdt_adamw_ema")
@@ -268,9 +276,16 @@ def cast_bf16_check(x, flag, out=None):
 
 
 def adamw_ema_guarded(w, g, m, v, ema, w16, n, lr, flag, counts, beta1=0.9, beta2=0.999, eps=1e-8, weight_decay=0.0,
-                      ema_decay=0.9999, grad_scale=1.0, max_blocks=0):
-    """`adamw_ema` at step counts[0] + 1 when flag == 0; only the EMA update when flag != 0."""
+                      ema_decay=0.9999, grad_scale=1.0, max_blocks=0, coef=None):
+    """`adamw_ema` at step counts[0] + 1 when flag == 0; only the EMA update when flag != 0.  coef: as `adamw_ema`'s."""
     _c(flag, f32), _c(counts, torch.int64)
+    if coef is not None:
+        _c(coef, f32)
+        fn = lib().mdt_adamw_ema_guarded_coef_g16 if g.dtype == bf16 else lib().mdt_adamw_ema_guarded_coef
+        check(fn(ptr(w), ptr(g), ptr(m), ptr(v), ptr(ema), ptr(w16), n, lr, beta1, beta2, eps, weight_decay,
+                 ema_decay, grad_scale, ptr(coef), ptr(flag), ptr(counts), max_blocks, stream_ptr()),
+              "mdt_adamw_ema_guarded_coef")
+        return
     fn = lib().mdt_adamw_ema_guarded_g16 if g.dtype == bf16 else lib().mdt_adamw_ema_guarded
     check(fn(ptr(w), ptr(g), ptr(m), ptr(v), ptr(ema), ptr(w16), n, lr, beta1, beta2, eps, weight_decay, ema_decay,
              grad_scale, ptr(flag), ptr(counts), max_blocks, stream_ptr()), "mdt_adamw_ema_guarded")
@@ -280,6 +295,35 @@ def optim_guard_advance(flag, counts):
     """counts[1 if flag else 0] += 1: once per step, after its last guarded optimizer pass."""
     _c(flag, f32), _c(counts, torch.int64)
     check(lib().mdt_optim_guard_advance(ptr(flag), ptr(counts), stream_ptr()), "mdt_optim_guard_advance")
+
+
+# -- gradient-norm clipping: sums of squares in fp64 slots, then the norm and the clip coefficient (fp32 words) ---------
+def grad_sumsq_scratch(n, device):
+    """The fp64 scratch `grad_sumsq` needs for up to n elements (it may be shared by calls on one stream)."""
+    k = lib().mdt_grad_sumsq_scratch(int(n))
+    if k < 1:
+        raise L.MdtError(f"mdt_grad_sumsq_scratch({n}) failed (status {k})")
+    return torch.empty(k, dtype=torch.float64, device=device)
+
+
+def grad_sumsq(g, out, scratch, flag=None):
+    """out[0] = sum of g**2 (fp32 or bf16 g, fp64 sum in an order that depends on g.numel() alone); with `flag`, the
+    non-finite check of `nonfinite_check` from the same read."""
+    _c(g), _c(out, torch.float64), _c(scratch, torch.float64), _c(flag, f32)
+    if g.dtype not in (f32, bf16):
+        raise L.MdtError(f"grad_sumsq: expected float32 or bfloat16, got {g.dtype}")
+    if scratch.numel() < lib().mdt_grad_sumsq_scratch(g.numel()):
+        raise L.MdtError(f"grad_sumsq: {scratch.numel()} scratch slots for {g.numel()} elements (grad_sumsq_scratch)")
+    check(lib().mdt_grad_sumsq(ptr(g), g.numel(), int(g.dtype == bf16), ptr(scratch), ptr(out), ptr(flag),
+                               stream_ptr()), "mdt_grad_sumsq", 2)
+
+
+def grad_clip_coef(sumsq, grad_scale, max_norm, norm, coef, flag=None):
+    """norm = grad_scale * sqrt(sum(sumsq)) (fp64, rounded once), coef = min(1, max_norm / (norm + 1e-6)) as
+    clip_grad_norm_ computes it (max_norm = inf: coef = 1); with `flag` and a finite max_norm a non-finite norm sets it."""
+    _c(sumsq, torch.float64), _c(norm, f32), _c(coef, f32), _c(flag, f32)
+    check(lib().mdt_grad_clip_coef(ptr(sumsq), sumsq.numel(), float(grad_scale), float(max_norm), ptr(norm),
+                                   ptr(coef), ptr(flag), stream_ptr()), "mdt_grad_clip_coef")
 
 
 def power_ema(w, emas, coeffs):

@@ -60,6 +60,16 @@ def lr_at(step: int, base_lr: float, global_batch: int, rampup_kimg: float):
     return base_lr * min(step * global_batch / max(rampup_kimg * 1000, 1e-8), 1)
 
 
+def check_max_grad_norm(c):
+    """The clipping bound `TrainStep(max_grad_norm=)` accepts: None (off), or a float > 0, inf included (measure only)."""
+    if c is None:
+        return None
+    c = float(c)
+    if not c > 0:   # also NaN
+        raise ValueError(f"max_grad_norm must be > 0 (inf: report the norm without clipping), got {c}")
+    return c
+
+
 def ar_chunk_bounds(n, k):
     """[lo, hi) element ranges of the k all-reduce chunks of a flat buffer of n elements (4 KiB aligned starts)."""
     if k <= 1 or n < k * 1024:
@@ -105,8 +115,26 @@ class TrainStep:
                  weight_decay=0.0, ema_decay=0.9999, loss_fn: EDMLoss | None = None, process_group=None,
                  lr_rampup_kimg=0.0, global_batch=None, device=None, overlap=False, graph=None,
                  reference_lr_schedule=False, collective=None, grad_dtype=None, skip_nonfinite=False,
-                 recompute_blocks=None, phema_sigma_rels=()):
-        """phema_sigma_rels: relative widths of power-function EMA profiles to keep for post-hoc EMA (`phema.py`,
+                 recompute_blocks=None, phema_sigma_rels=(), max_grad_norm=None):
+        """max_grad_norm: gradient-norm clipping, torch.nn.utils.clip_grad_norm_'s formula on the device.  None
+        (default): off, nothing is allocated or launched.  A float c > 0: every step measures
+        norm = grad_scale * ||g||_2 over the trainable region, g being the gradient the optimizer reads (the fp32 flat
+        gradient at world 1, the summed exchange buffer at world > 1, bf16 sums under grad_dtype='bf16') and
+        grad_scale = 1/(world * grad_accum), i.e. the norm of the averaged gradient that clip_grad_norm_ returns after
+        a DDP backward.  The sum of squares runs in fp64 in an order that depends only on the size (bit-reproducible in
+        both modes, whatever the SM budget), and the norm is rounded to fp32 once.  The update then uses
+        coef * grad_scale * g with coef = min(1, c / (norm + 1e-6)) in fp32; c = inf only measures (coef = 1, and the
+        update is the unclipped one bit for bit).  `grad_norm` holds the last step's norm before clipping on the
+        device.  Every rank holds the same summed bits, so every rank computes the same norm without a collective.
+        Cost: at world 1 one extra read of the gradient, none under skip_nonfinite (the norm pass replaces the check
+        pass).  At world > 1 each chunk's sum of squares runs on the exchange stream after that chunk's all-reduce; with
+        a finite c every optimizer pass then waits for the last chunk, since clipping needs the global norm, which
+        serialises the optimizer behind the whole exchange (c = inf keeps the pipelined order).  With skip_nonfinite a
+        non-finite element still skips the step, and with a finite c so does a non-finite norm (a sum that overflows
+        although every rank's values were finite).  Without the guard a non-finite norm gives the coefficient the
+        formula gives (NaN or 0), as clip_grad_norm_(error_if_nonfinite=False) does, and that poisons or freezes the
+        weights; skip_nonfinite is how to avoid it.
+        phema_sigma_rels: relative widths of power-function EMA profiles to keep for post-hoc EMA (`phema.py`,
         posthoc_ema.py), e.g. (0.05, 0.10); at most 4.  Each is one fp32 buffer over the trainable region (2.92 GB for XL/2),
         allocated here and advanced after every optimizer pass over a range, on that pass's stream, by `mdt_power_ema`
         with 1 - beta(t) from the host's count t of the profiles' steps: exactly one update per optimizer step (also
@@ -201,6 +229,13 @@ class TrainStep:
         self.skip_nonfinite = bool(skip_nonfinite)
         self._flag = torch.zeros(1, dtype=torch.float32, device=dev) if self.skip_nonfinite else None
         self._counts = torch.zeros(2, dtype=torch.int64, device=dev) if self.skip_nonfinite else None
+        # gradient-norm clipping: fp64 sum-of-squares slots (one per exchange chunk), the norm pass's scratch, norm, coef
+        self.max_grad_norm = check_max_grad_norm(max_grad_norm)
+        if self.max_grad_norm is not None:
+            self._gn_slots = torch.zeros(max(len(ar_chunk_bounds(n, self.ar_chunks)), 1), dtype=torch.float64,
+                                         device=dev)
+            self._gn_scratch = ops.grad_sumsq_scratch(n, dev)
+            self._gn = torch.zeros(2, dtype=torch.float32, device=dev)   # {norm, coef}
         # power-function EMA profiles: allocated now, so the recomputation picker sees their memory as used
         self.phema_sigma_rels = tuple(float(s) for s in phema_sigma_rels)
         if len(self.phema_sigma_rels) > 4:   # mdt_power_ema advances up to 4 profiles from one read of the weights
@@ -221,6 +256,12 @@ class TrainStep:
         """Device tensor (int64, 0-dim): optimizer steps skipped for non-finite gradients since this object was built
         (None without `skip_nonfinite`).  Reading its value synchronises; the step itself never does."""
         return self._counts[1] if self._counts is not None else None
+
+    @property
+    def grad_norm(self):
+        """Device tensor (fp32, 0-dim): the last step's gradient norm before clipping, grad_scale * ||g||_2 (None without
+        `max_grad_norm`).  Reading its value synchronises; the step itself never does."""
+        return self._gn[0] if self.max_grad_norm is not None else None
 
     def applied_steps(self) -> int:
         """Adam's step count: the steps whose update was applied (a host read of the device counter under
@@ -375,20 +416,31 @@ class TrainStep:
             buf = self._cast(lo, hi) if cast else self.g16[lo:hi]
         self._all_reduce(buf)
 
+    def _clips(self):
+        return self.max_grad_norm is not None and self.max_grad_norm != float("inf")
+
+    def _grad_norm_coef(self, k):
+        """norm and coef from the first k sum-of-squares slots; with a finite bound a non-finite norm sets the guard's
+        flag."""
+        ops.grad_clip_coef(self._gn_slots[:k], self._grad_scale, self.max_grad_norm, self._gn[:1], self._gn[1:],
+                           flag=self._flag if self._clips() else None)
+
     def _step_range(self, lo, hi):
         st, n = self.st, hi - lo
         if n <= 0:
             return
         g = self.g16[lo:hi] if (self.g16 is not None and self.world > 1) else st.grad[lo:hi]
         ema = self.ema_st.w32[lo:hi] if self.ema_st is not None else None
+        # a finite clipping bound: the optimizer reads the coefficient (c = inf keeps the plain kernels)
+        coef = self._gn[1:] if self._clips() else None
         if self._flag is not None:   # Adam's step number comes from the device counter, the skip from the flag
             ops.adamw_ema_guarded(st.w32[lo:hi], g, self.m[lo:hi], self.v[lo:hi], ema, st.w16[lo:hi], n, self._lr_now,
                                   self._flag, self._counts, self.betas[0], self.betas[1], self.eps, self.wd,
-                                  self.ema_decay, self._grad_scale)
+                                  self.ema_decay, self._grad_scale, coef=coef)
         else:
             ops.adamw_ema(st.w32[lo:hi], g, self.m[lo:hi], self.v[lo:hi], ema, st.w16[lo:hi], n, self._lr_now,
                           self.step_count, self.betas[0], self.betas[1], self.eps, self.wd, self.ema_decay,
-                          self._grad_scale)
+                          self._grad_scale, coef=coef)
         if self.phema_emas:   # the profiles follow the range's new (or, skipped, unchanged) weights on the same stream
             ops.power_ema(st.w32[lo:hi], [e[lo:hi] for e in self.phema_emas], self._phema_c)
 
@@ -499,8 +551,12 @@ class TrainStep:
         n = st.n_train
         # Under the guard the flag must be final before the first optimizer pass.  At world > 1 every rank checks its
         # local values (bf16 exchange: while casting them) and one flag word is summed over the ranks.
+        measure = self.max_grad_norm is not None
         if self.world == 1:
-            if guard:
+            if measure:   # one read of the gradient: the norm, and under the guard the non-finite check
+                ops.grad_sumsq(st.grad[:n], self._gn_slots[:1], self._gn_scratch, flag=self._flag)
+                self._grad_norm_coef(1)
+            elif guard:
                 ops.nonfinite_check(st.grad[:n], self._flag)
             self._step_range(0, n)
         else:
@@ -508,6 +564,8 @@ class TrainStep:
             if self.side is None:
                 self.side = torch.cuda.Stream(device=st.grad.device)
             bounds = ar_chunk_bounds(n, self.ar_chunks)
+            if measure and self._gn_slots.numel() < len(bounds):
+                self._gn_slots = torch.zeros(len(bounds), dtype=torch.float64, device=st.grad.device)
             self.side.wait_stream(main)
             evs = []
             with torch.cuda.stream(self.side):
@@ -518,14 +576,25 @@ class TrainStep:
                     else:
                         ops.nonfinite_check(st.grad[:n], self._flag)
                     self._all_reduce(self._flag)
-                for lo, hi in bounds:
+                for k, (lo, hi) in enumerate(bounds):
                     self._exchange(lo, hi, cast=not guard)
                     ev = torch.cuda.Event()
                     ev.record(self.side)
                     evs.append(ev)
+                    if measure:   # the chunk's summed values, while the optimizer steps it
+                        g = self.g16[lo:hi] if self.g16 is not None else st.grad[lo:hi]
+                        ops.grad_sumsq(g, self._gn_slots[k:k + 1], self._gn_scratch)
+                if measure:
+                    self._grad_norm_coef(len(bounds))
+            if self._clips():   # clipping needs the global norm: every chunk's pass waits for the coefficient
+                main.wait_stream(self.side)
+                evs = [None] * len(bounds)
             for (lo, hi), ev in zip(bounds, evs):
-                main.wait_event(ev)
+                if ev is not None:
+                    main.wait_event(ev)
                 self._step_range(lo, hi)
+            if measure:   # the norm passes read buffers the next step writes on this stream
+                main.wait_stream(self.side)
         if guard:
             ops.optim_guard_advance(self._flag, self._counts)
         st.mark_shadow_fresh(self.net._params())   # the kernel refreshed the bf16 shadow itself

@@ -18,6 +18,9 @@ gradient accumulation (`train.grad_accum`) and the lr ramp follow train.py:211-2
 Post-hoc EMA (not in the reference): `--phema_sigma_rel 0.05,0.10` keeps power-function EMA profiles next to the
 reference-fixed EMA, the checkpoints carry them, and `--phema_every N` writes snapshots that posthoc_ema.py combines
 into the EMA of any width after the run.
+Gradient-norm clipping (not in the reference): `--max_grad_norm 1.0` clips the global gradient norm as
+torch.nn.utils.clip_grad_norm_ does, `--max_grad_norm inf` only measures it; either way the log line reports the
+window's mean and maximum norm.
 """
 import argparse
 import copy
@@ -29,7 +32,7 @@ import torch.distributed as dist
 
 from maskdit_b200.config import build_net, load_config, mask_ratio_schedule, parse_float_none, parse_int_list
 from maskdit_b200.loss import Losses
-from maskdit_b200.train_step import TrainStep
+from maskdit_b200.train_step import TrainStep, check_max_grad_norm
 
 
 def latest_ckpt(d):
@@ -55,8 +58,26 @@ def skip_nonfinite(args):
     return not args.no_amp
 
 
+def log_line(step, loss, steps_per_sec, skipped=None, grad_norm=None):
+    """The training log line (the reference's format, train.py:247); `skipped` (a count) and `grad_norm` (the
+    window's mean and max) are appended only when given."""
+    line = f"(step={step:07d}) Train Loss: {loss:.4f}, Train Steps/Sec: {steps_per_sec:.2f}"
+    if skipped is not None:
+        line += f", Skipped Steps: {skipped}"
+    if grad_norm is not None:
+        line += f", Grad Norm: {grad_norm[0]:.4g} (max {grad_norm[1]:.4g})"
+    return line
+
+
 def parse_sigma_rels(s):
     return tuple(float(v) for v in s.split(",") if v.strip())
+
+
+def parse_max_grad_norm(s):
+    try:
+        return check_max_grad_norm(s)
+    except ValueError as e:
+        raise argparse.ArgumentTypeError(str(e))
 
 
 def build_parser():
@@ -84,6 +105,9 @@ def build_parser():
     ap.add_argument("--phema_every", type=int, default=0,
                     help="write a snapshot of the profiles to <results_dir>/phema/phema-<step>.pt every N steps "
                          "(posthoc_ema.py combines them into any EMA width after the run)")
+    ap.add_argument("--max_grad_norm", type=parse_max_grad_norm, default=None,
+                    help="clip the global gradient norm to this bound (torch's clip_grad_norm_; 'inf' only measures) "
+                         "and log its mean and max over each logging window")
     return ap
 
 
@@ -119,7 +143,8 @@ def main():
         step0 = int(os.path.basename(ck)[:-3]) if os.path.basename(ck)[:-3].isdigit() else 0
     ts = TrainStep(net, ema, lr=cfg.train.lr, lr_rampup_kimg=cfg.train.lr_rampup_kimg, global_batch=global_batch,
                    loss_fn=Losses[cfg.model.precond](), reference_lr_schedule=True,
-                   skip_nonfinite=skip_nonfinite(args), phema_sigma_rels=args.phema_sigma_rel)
+                   skip_nonfinite=skip_nonfinite(args), phema_sigma_rels=args.phema_sigma_rel,
+                   max_grad_norm=args.max_grad_norm)
     if ck and strict and "opt" in sd:                      # train.py:150: optimizer state only under strict loading
         ts.load_state_dict(sd["opt"])
     ts.lr_step_offset = step0 - ts.step_count              # lr follows the run's step counter (train.py:223)
@@ -154,6 +179,7 @@ def main():
         loader = batches(ds, batch, rank, world, start=step0)
     log_every = cfg.log.log_every
     running, log_steps, t0, step = 0.0, 0, time.time(), step0
+    gn_sum = gn_max = None   # the window's gradient norms, accumulated on the device like `running`
     recompute_shown = 0
     for moments, labels in loader:
         moments = moments.to(device, non_blocking=True)
@@ -163,6 +189,10 @@ def main():
         loss = ts.step(moments, labels, ratio, cfg.model.mae_loss_coef, grad_accum=rounds, moments=True,
                        class_dropout_prob=drop)
         running = running + loss.mean()
+        if ts.grad_norm is not None:
+            gn = ts.grad_norm
+            gn_sum = gn.clone() if gn_sum is None else gn_sum + gn
+            gn_max = gn.clone() if gn_max is None else torch.maximum(gn_max, gn)
         if rank == 0 and ts.recompute_blocks and not recompute_shown:
             recompute_shown = ts.recompute_blocks
             print(f"Activation recomputation: the training workspace of a micro-batch does not fit in device memory, "
@@ -180,10 +210,12 @@ def main():
             torch.cuda.synchronize()
             if rank == 0:
                 # every rank takes the same skip decisions, so rank 0's tally is the run's
-                skipped = f", Skipped Steps: {int(ts.skipped_steps)}" if ts.skipped_steps is not None else ""
-                print(f"(step={step:07d}) Train Loss: {float(avg):.4f}, Train Steps/Sec: "
-                      f"{log_steps / (time.time() - t0):.2f}{skipped}", flush=True)
+                skipped = int(ts.skipped_steps) if ts.skipped_steps is not None else None
+                # every rank computes the same norm from the same summed gradient
+                gnorm = (float(gn_sum) / log_steps, float(gn_max)) if gn_sum is not None else None
+                print(log_line(step, float(avg), log_steps / (time.time() - t0), skipped, gnorm), flush=True)
             running, log_steps, t0 = 0.0, 0, time.time()
+            gn_sum = gn_max = None
         if step % cfg.log.ckpt_every == 0 and step > step0:
             if rank == 0:
                 d = os.path.join(args.results_dir, "checkpoints")
