@@ -18,6 +18,9 @@ gradient accumulation (`train.grad_accum`) and the lr ramp follow train.py:211-2
 Post-hoc EMA (not in the reference): `--phema_sigma_rel 0.05,0.10` keeps power-function EMA profiles next to the
 reference-fixed EMA, the checkpoints carry them, and `--phema_every N` writes snapshots that posthoc_ema.py combines
 into the EMA of any width after the run.
+Held-out validation (not in the reference): `--val_every M` scores the EMA every M steps on the first `--val_count`
+items of the latent LMDB split `data.root`/val (`--synthetic`: moments drawn from a fixed seed) at `--val_levels` fixed
+noise levels (`maskdit_b200/validate.py`), a loss that compares across steps and runs; val_loss.py scores checkpoints.
 Gradient-norm clipping (not in the reference): `--max_grad_norm 1.0` clips the global gradient norm as
 torch.nn.utils.clip_grad_norm_ does, `--max_grad_norm inf` only measures it; either way the log line reports the
 window's mean and maximum norm.
@@ -108,7 +111,27 @@ def build_parser():
     ap.add_argument("--max_grad_norm", type=parse_max_grad_norm, default=None,
                     help="clip the global gradient norm to this bound (torch's clip_grad_norm_; 'inf' only measures) "
                          "and log its mean and max over each logging window")
+    ap.add_argument("--val_every", type=int, default=0,
+                    help="every N steps, print the held-out denoising loss of the EMA (0: off)")
+    ap.add_argument("--val_count", type=int, default=1000,
+                    help="held-out items: the first N of data.root/val (with --synthetic: N moments from a fixed seed)")
+    ap.add_argument("--val_levels", type=int, default=8, help="noise levels per held-out item")
     return ap
+
+
+def val_line(step, res):
+    """The validation log line (rank 0): the mean over levels, then each level's mean loss."""
+    from maskdit_b200.validate import format_levels
+    return f"(step={step:07d}) Val Loss: {format_levels(res)} ({res['count']} items, EMA)"
+
+
+def held_out_set(args, cfg):
+    """The validation items: the first --val_count of data.root/val, or synthetic moments from a fixed seed."""
+    from maskdit_b200.validate import HeldOut
+    m = cfg.model
+    if args.synthetic:
+        return HeldOut.synthetic(args.val_count, m.in_size, m.in_channels, m.num_classes)
+    return HeldOut.from_lmdb(cfg.data.root, args.val_count, cfg.data.resolution, cfg.data.num_channels, m.num_classes)
 
 
 def main():
@@ -177,6 +200,14 @@ def main():
         if rank == 0:
             print(f"Dataset contains {len(ds):,} images ({cfg.data.root})", flush=True)
         loader = batches(ds, batch, rank, world, start=step0)
+    held = None
+    if args.val_every:
+        if args.val_count < 1 or args.val_levels < 1:
+            raise SystemExit("--val_count and --val_levels must be positive")
+        held = held_out_set(args, cfg)
+        if rank == 0:
+            print(f"Validation: {len(held)} held-out items x {args.val_levels} noise levels every {args.val_every} "
+                  f"steps", flush=True)
     log_every = cfg.log.log_every
     running, log_steps, t0, step = 0.0, 0, time.time(), step0
     gn_sum = gn_max = None   # the window's gradient norms, accumulated on the device like `running`
@@ -216,6 +247,12 @@ def main():
                 print(log_line(step, float(avg), log_steps / (time.time() - t0), skipped, gnorm), flush=True)
             running, log_steps, t0 = 0.0, 0, time.time()
             gn_sum = gn_max = None
+        if held is not None and step % args.val_every == 0:
+            from maskdit_b200.validate import validate
+            # eager, fixed draws from their own generators: the training step's RNG stream and memory plan are untouched
+            res = validate(ema, held, levels=args.val_levels, batch=micro_batch)
+            if rank == 0:
+                print(val_line(step, res), flush=True)
         if step % cfg.log.ckpt_every == 0 and step > step0:
             if rank == 0:
                 d = os.path.join(args.results_dir, "checkpoints")
