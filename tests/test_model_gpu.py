@@ -374,10 +374,9 @@ def test_train_step_state_dict_resume():
 
 
 def test_full_size_config2_properties():
-    """BASELINE config 2 at FULL size (XL/2, batch 256, 32x32x4, mask 0.5) through size-independent properties:
-    samples are independent through the whole path, so (i) the first rows of a batch-256 loss equal a batch-4 run on
-    the same rows bit-for-bit in the forward (row results do not depend on the tile a row lands in), (ii) the mask path
-    invariants hold for every row, (iii) the gradient is linear in the upstream loss gradient."""
+    """BASELINE config 2 at FULL size (XL/2, batch 256, 32x32x4, mask 0.5) through the loss interface: the loss is
+    finite and the mask path invariants hold for every row.  Every row and every gradient of this step against
+    batch-2 runs: tests/test_production_batch_gpu.py."""
     from maskdit_b200.loss import EDMLoss
     torch.manual_seed(0)
     net, cfg, _ = build("DiT-XL/2", 32, 1000)
@@ -405,18 +404,7 @@ def test_full_size_config2_properties():
         lf = L(B)
         full = lf(net, images, labels, mask_ratio=0.5, mae_loss_coef=0.1)
         md = lf.last_mask_dict
-        small = L(4)(net, images[:4].contiguous(), labels[:4].contiguous(), mask_ratio=0.5, mae_loss_coef=0.1)
     assert torch.isfinite(full).all()
-    assert torch.equal(full[:4], small), (full[:4], small)
     assert torch.equal(md["mask"].sum(1), torch.full((B,), 128.0, device="cuda"))
     assert torch.equal(torch.gather(md["ids_restore"], 1, md["ids_keep"]),
                        torch.arange(128, device="cuda").expand(B, -1))
-    # linearity of the hand-written backward in the upstream gradient (stream-K / atomics: compare within 1e-3)
-    key = "model.blocks.13.mlp.fc2.weight"
-    grads = []
-    for scale in (1.0, 2.0):
-        net.zero_grad(set_to_none=True)
-        loss = L(8)(net, images[:8].contiguous(), labels[:8].contiguous(), mask_ratio=0.5, mae_loss_coef=0.1)
-        (loss.sum() * scale).backward()
-        grads.append(dict(net.named_parameters())[key].grad.clone())
-    assert rel_l2(grads[1], 2 * grads[0]) < 1e-3

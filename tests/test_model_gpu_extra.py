@@ -381,9 +381,9 @@ def test_unconditional_odd_token_count_vs_reference_golden():
 
 def test_full_size_config4_properties():
     """BASELINE config 4 at the largest per-GPU batch an 80 GB H100 holds (XL/2, 64x64x4 latents, mask 0.5, batch 64:
-    512 kept / 1024 decoder tokens per sample, a 54 GB workspace) through size-independent properties: the forward is
-    row-independent bit for bit (first rows of the batch-64 loss == a batch-2 run on the same rows), the mask path
-    invariants hold for every row, one backward leaves finite gradients everywhere."""
+    512 kept / 1024 decoder tokens per sample, a 54 GB workspace) through the loss interface without recomputation:
+    the mask path invariants hold for every row and one backward leaves finite gradients everywhere.  Every row and
+    every gradient of this step against batch-2 runs: tests/test_production_batch_gpu.py."""
     from maskdit_b200.loss import EDMLoss
     import gc
     gc.collect()
@@ -420,6 +420,3 @@ def test_full_size_config4_properties():
     assert torch.isfinite(st.grad).all() and float(st.grad.abs().sum()) > 0
     del lf, md
     torch.cuda.empty_cache()
-    with torch.no_grad():
-        small = Lz(2)(net, images[:2].contiguous(), labels[:2].contiguous(), mask_ratio=0.5, mae_loss_coef=0.1)
-    assert torch.equal(full[:2].detach(), small), (full[:2], small)
