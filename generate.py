@@ -10,6 +10,12 @@ decode of the reference (sample.py:275) runs on the same kernels (`maskdit_b200/
 FrozenAutoencoderKL checkpoint: images are converted to 8 bit (`ops.to_uint8_nhwc`) and written as `<seed>.png`
 (`sampler.write_png`), exactly the tail of generate_with_net (sample.py:275-296).  The latents are always saved as `.npy`
 per seed as well; without a VAE checkpoint `--png_preview` writes the raw latent channels as a picture.
+
+Guidance beyond the reference's `--cfg_scale`: `--guide_ckpt` (or `--guide_snapshots` + `--guide_sigma_rel`, a post-hoc
+EMA built by `posthoc_ema.reconstruct`) with `--guidance W` guides with a second, weaker network of the same image
+geometry and classes (autoguidance; `--guide_config` when its architecture differs), and `--guidance_interval LO HI`
+applies CFG or the guide only at evaluations with LO < sigma <= HI.  Class-unconditional configs sample with all-zero
+label rows as the reference does (sample.py:261-264).
 """
 import argparse
 import os
@@ -36,7 +42,7 @@ class StackedRandomGenerator:
         return torch.stack([torch.randint(*a, size=size[1:], generator=g, **kw) for g in self.generators])
 
 
-def main():
+def build_parser():
     ap = argparse.ArgumentParser("Sample from a trained model")
     ap.add_argument("--config", required=True)
     ap.add_argument("--results_dir", default="samples")
@@ -58,7 +64,64 @@ def main():
     ap.add_argument("--subdirs", action="store_true", help="<seed - seed % 1000:06d>/ sub-directories (sample.py:289)")
     ap.add_argument("--png_preview", action="store_true",
                     help="also write channels 0-2 of every latent as an 8-bit PNG (no SD-VAE in this repo)")
-    args, _ = ap.parse_known_args()
+    # guidance by a second network (autoguidance) and a noise-level interval for guidance (maskdit_b200/sampler.py)
+    ap.add_argument("--guide_ckpt", default=None,
+                    help="guide network checkpoint (train.py, posthoc_ema.py or the reference's)")
+    ap.add_argument("--guide_key", choices=["ema", "model"], default="ema", help="weights of --guide_ckpt to load")
+    ap.add_argument("--guide_config", default=None, help="YAML of the guide's architecture (default: --config)")
+    ap.add_argument("--guide_snapshots", default=None,
+                    help="build the guide from the post-hoc EMA snapshots in this directory (posthoc_ema.py)")
+    ap.add_argument("--guide_sigma_rel", type=float, default=None, help="relative EMA width of the snapshot guide")
+    ap.add_argument("--guide_step", type=int, default=None,
+                    help="run step of the snapshot guide's EMA (default: the last snapshot's)")
+    ap.add_argument("--guidance", type=float, default=None,
+                    help="guide weight w: D = D_guide + w (D_net - D_guide); 1 is the unguided network")
+    ap.add_argument("--guidance_interval", type=float, nargs=2, default=None, metavar=("LO", "HI"),
+                    help="apply the guidance (--cfg_scale or the guide) only at evaluations with LO < sigma <= HI")
+    return ap
+
+
+def parse_args(argv=None):
+    ap = build_parser()
+    args, _ = ap.parse_known_args(argv)
+    guide = args.guide_ckpt is not None or args.guide_snapshots is not None
+    if args.guide_ckpt is not None and args.guide_snapshots is not None:
+        ap.error("--guide_ckpt and --guide_snapshots are mutually exclusive")
+    if (args.guide_snapshots is None) != (args.guide_sigma_rel is None):
+        ap.error("--guide_snapshots and --guide_sigma_rel go together")
+    if args.guide_step is not None and args.guide_snapshots is None:
+        ap.error("--guide_step needs --guide_snapshots")
+    if args.guide_config is not None and not guide:
+        ap.error("--guide_config needs --guide_ckpt or --guide_snapshots")
+    if guide and args.cfg_scale is not None:
+        ap.error("--cfg_scale and a guide network are mutually exclusive")
+    if guide != (args.guidance is not None):
+        ap.error("--guidance is the weight of a guide network (--guide_ckpt / --guide_snapshots): give both or neither")
+    if args.guidance_interval is not None:
+        lo, hi = args.guidance_interval
+        if not lo < hi:
+            ap.error(f"--guidance_interval needs LO < HI, got {lo:g} {hi:g}")
+        if not guide and args.cfg_scale is None:
+            ap.error("--guidance_interval needs --cfg_scale or a guide network")
+    return args
+
+
+def guide_state_dict(args):
+    """The guide's state dict on the host: `--guide_key` of `--guide_ckpt`, or the post-hoc EMA of width
+    `--guide_sigma_rel` at `--guide_step` reconstructed from `--guide_snapshots` (posthoc_ema.reconstruct)."""
+    if args.guide_snapshots is not None:
+        import posthoc_ema
+        files = posthoc_ema.list_snapshots(args.guide_snapshots, args.guide_step)
+        sd, _ = posthoc_ema.reconstruct(files, args.guide_sigma_rel, args.guide_step)
+        return sd
+    ck = torch.load(args.guide_ckpt, map_location="cpu", weights_only=False)   # trusted checkpoint, as --ckpt_path
+    if args.guide_key not in ck:
+        raise SystemExit(f"{args.guide_ckpt} holds no '{args.guide_key}' weights (keys: {sorted(ck)})")
+    return {k.replace("_orig_mod.", ""): v for k, v in ck[args.guide_key].items()}
+
+
+def main(argv=None):
+    args = parse_args(argv)
     cfg = load_config(args.config)
     rank, size = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     local = int(os.environ.get("LOCAL_RANK", 0))
@@ -71,6 +134,14 @@ def main():
         # trusted checkpoint: reference checkpoints hold an argparse.Namespace under 'args' (train.py:259-265)
         ck = torch.load(args.ckpt_path, map_location=device, weights_only=False)
         net.load_state_dict({k.replace("_orig_mod.", ""): v for k, v in ck["ema"].items()})
+    gkw = {}
+    if args.guidance is not None:
+        guide = build_net(load_config(args.guide_config or args.config)).to(device).eval()
+        guide.load_state_dict(guide_state_dict(args))
+        net.check_guide(guide)
+        gkw = dict(guide_net=guide, guidance=args.guidance)
+    if args.guidance_interval is not None:
+        gkw["guidance_interval"] = tuple(args.guidance_interval)
     os.makedirs(args.results_dir, exist_ok=True)
     vae = None
     if args.pretrained_path:
@@ -86,13 +157,17 @@ def main():
             continue
         rnd = StackedRandomGenerator(device, bs)
         latents = rnd.randn([len(bs), net.img_channels, net.img_resolution, net.img_resolution], device=device)
-        labels = torch.eye(net.num_classes, device=device)[rnd.randint(net.num_classes, size=[len(bs)], device=device)]
+        labels = torch.zeros([len(bs), net.num_classes], device=device)      # sample.py:261-264
+        if net.num_classes:
+            labels = torch.eye(net.num_classes, device=device)[rnd.randint(net.num_classes, size=[len(bs)],
+                                                                           device=device)]
         if args.class_idx is not None:
             labels[:, :] = 0
             labels[:, args.class_idx] = 1
         with torch.no_grad():
             z = sampler_fn(net, latents.float(), labels.float(), cfg_scale=args.cfg_scale,
-                           randn_like=rnd.randn_like, num_steps=args.num_steps, S_churn=args.S_churn, **kw).float()
+                           randn_like=rnd.randn_like, num_steps=args.num_steps, S_churn=args.S_churn, **kw,
+                           **gkw).float()
         if vae is not None:       # images = vae.decode(z); add(1).mul(127.5).clamp(0,255).to(uint8) NHWC; PNG per seed
             px = ops.to_uint8_nhwc(vae.decode(z).contiguous()).cpu().numpy()
             for s, im in zip(bs, px):

@@ -218,6 +218,14 @@ int mdt_edm_precond_out_bwd(const float* gD, const float* sigma, float sigma_dat
 int mdt_cfg_precond_out(const float* F, const float* xin, const float* sigma, float sigma_data, float cfg_scale,
                         float* Dx, int B, int C, int R, int p, void* stream);
 
+/* Guidance by a second network (autoguidance, Karras et al. 2024), the same combine fused with the EDM output scaling:
+ *   F_main [B, L_main, p_main²·C], F_guide [B, L_guide, p_guide²·C], each as mdt_forward writes it for its own patch
+ *   size -> Dx [B,C,R,R] = c_skip*x + c_out*(Fg + w (Fm - Fg)), fp32, one thread per output pixel.
+ *   MDT_ERR_ARG for a NULL pointer, B/C/R <= 0, a patch size that does not divide R, or a non-finite w. */
+int mdt_guided_precond_out(const float* F_main, int p_main, const float* F_guide, int p_guide, const float* xin,
+                           const float* sigma, float sigma_data, float w, float* Dx, int B, int C, int R,
+                           void* stream);
+
 /* EDM Heun sampler state update in fp64 (sample.py:56-64):
  *   mode 0 (Euler):  d_cur = (x_hat - den)/t_hat ; x_next = x_hat + (t_next - t_hat) d_cur
  *   mode 1 (Heun):   d_prime = (x_next - den)/t_next ; x_next = x_hat + (t_next - t_hat)(0.5 d_cur + 0.5 d_prime) */

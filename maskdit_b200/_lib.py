@@ -88,6 +88,7 @@ _SIGS = {
     "mdt_edm_precond_out": [_P, _P, _P, _F, _P, _I, _I, _I, _I, _P],
     "mdt_edm_precond_out_bwd": [_P, _P, _F, _P, _I, _I, _I, _I, _P],
     "mdt_cfg_precond_out": [_P, _P, _P, _F, _F, _P, _I, _I, _I, _I, _P],
+    "mdt_guided_precond_out": [_P, _I, _P, _I, _P, _P, _F, _F, _P, _I, _I, _I, _P],
     "mdt_heun_update": [_I, _P, _P, _P, _P, _P, _D, _D, _LL, _P],
     "mdt_lincomb_f64": [_D, _P, _D, _P, _D, _P, _P, _P, _D, _LL, _P],
     "mdt_to_uint8_nhwc": [_P, _P, _I, _I, _I, _I, _P],

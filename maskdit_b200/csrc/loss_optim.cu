@@ -1,5 +1,5 @@
-// EDM preconditioning output, EDM + MAE loss (forward + gradient seed), CFG combine, Heun update, fused AdamW+EMA,
-// power-function EMA profiles (post-hoc EMA).
+// EDM preconditioning output, EDM + MAE loss (forward + gradient seed), CFG and guide-network combines, Heun update,
+// fused AdamW+EMA, power-function EMA profiles (post-hoc EMA).
 #include <math.h>
 
 #include "common.cuh"
@@ -142,6 +142,29 @@ __global__ void precond_out_kernel(const float* __restrict__ F, const float* __r
     Dx[px] = c_skip * xin[px] + c_out * f;
   }
 }
+// Guidance by a second network: D = c_skip*x + c_out*(Fg + w (Fm - Fg)), one thread per output pixel.  Fm and Fg are
+// each read in their own network's patch geometry (the patch sizes may differ); the combine is the CFG branch above.
+MDT_DEVINL float patch_at(const float* __restrict__ F, const PatchGeom& gm, int b, int c, int hh, int ww) {
+  const int l = (hh / gm.p) * gm.G + ww / gm.p, j = ((hh % gm.p) * gm.p + ww % gm.p) * gm.C + c;
+  return F[(static_cast<size_t>(b) * gm.L + l) * gm.pd + j];
+}
+__global__ void guided_precond_out_kernel(const float* __restrict__ Fm, PatchGeom gm, const float* __restrict__ Fg,
+                                          PatchGeom gg, const float* __restrict__ xin, const float* __restrict__ sigma,
+                                          float sd, float w, int B, float* __restrict__ Dx) {
+  const long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  const int R = gm.R, C = gm.C;
+  if (idx >= static_cast<long long>(B) * C * R * R) return;
+  const int ww = static_cast<int>(idx % R), hh = static_cast<int>(idx / R % R);
+  const int c = static_cast<int>(idx / (static_cast<long long>(R) * R) % C);
+  const int b = static_cast<int>(idx / (static_cast<long long>(C) * R * R));
+  const float sg = sigma[b];
+  const float den = sg * sg + sd * sd;
+  const float c_skip = sd * sd / den, c_out = sg * sd * rsqrtf(den);
+  const float fm = patch_at(Fm, gm, b, c, hh, ww), fg = patch_at(Fg, gg, b, c, hh, ww);
+  const float f = fg + w * (fm - fg);
+  Dx[idx] = c_skip * xin[idx] + c_out * f;
+}
+
 __global__ void precond_out_bwd_kernel(const float* __restrict__ gD, const float* __restrict__ sigma, float sd, int B,
                                        __nv_bfloat16* __restrict__ dF, PatchGeom gm) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -576,6 +599,19 @@ int mdt_cfg_precond_out(const float* F, const float* xin, const float* sigma, fl
   if (int rc = make_geom(&gm, C, R, p)) return rc;
   const int n = B * gm.L;
   precond_out_kernel<<<(n + 127) / 128, 128, 0, S(stream)>>>(F, xin, sigma, sigma_data, cfg_scale, 1, B, Dx, gm);
+  return launch_status();
+}
+
+int mdt_guided_precond_out(const float* F_main, int p_main, const float* F_guide, int p_guide, const float* xin,
+                           const float* sigma, float sigma_data, float w, float* Dx, int B, int C, int R,
+                           void* stream) {
+  if (!F_main || !F_guide || !xin || !sigma || !Dx || B <= 0 || !isfinite(w)) return MDT_ERR_ARG;
+  PatchGeom gm, gg;
+  if (int rc = make_geom(&gm, C, R, p_main)) return rc;
+  if (int rc = make_geom(&gg, C, R, p_guide)) return rc;
+  const long long n = static_cast<long long>(B) * C * R * R;
+  guided_precond_out_kernel<<<static_cast<int>((n + 255) / 256), 256, 0, S(stream)>>>(F_main, gm, F_guide, gg, xin,
+                                                                                       sigma, sigma_data, w, B, Dx);
   return launch_status();
 }
 

@@ -283,8 +283,13 @@ class EDMPrecond(nn.Module):
         return xf, sig, lab
 
     # -- eval-mode forward (no autograd): eager, or replayed from a CUDA graph ---------------------------------------
-    def _eval_eager(self, xf, sig, lab, cfg_scale):
+    def _eval_eager(self, xf, sig, lab, cfg_scale, guide=None):
         p = self.model.patch_size
+        if guide is not None:
+            # guidance by a second network: one eval pass of each at batch B, `cfg_scale` is the guide weight w
+            Fm, _ = self._engine.forward(xf, sig, lab, None, save=False)
+            Fg, _ = guide._engine.forward(xf, sig, lab, None, save=False)
+            return ops.guided_precond_out(Fm, p, Fg, guide.model.patch_size, xf, sig, self.sigma_data, cfg_scale)
         if cfg_scale is not None:
             # forward_with_cfg (models/maskdit.py:559-587): one eval pass at batch 2B, guidance fused in the output
             x2 = torch.cat([xf, xf], 0)
@@ -295,13 +300,16 @@ class EDMPrecond(nn.Module):
         Fo, _ = self._engine.forward(xf, sig, lab, None, save=False)
         return ops.edm_precond_out(Fo, xf, sig, self.sigma_data, p)
 
-    def _eval_graphed(self, xf, sig, lab, cfg_scale):
+    def _eval_graphed(self, xf, sig, lab, cfg_scale, guide=None):
         """The eval forward is ~280 launches with static shapes: the sampler calls it 35 times per batch and the host
         enqueue time (35 ms per evaluation at B=64) is as long as the device time (38 ms).  It is therefore captured
-        once per (shapes, cfg_scale) into a CUDA graph with static input buffers and replayed.  Weights are read from
-        the flat bf16 shadow, whose storage is stable (the cache is dropped when the store is re-attached).
-        MDT_CUDA_GRAPH=0 disables the graphs."""
+        once per (shapes, cfg_scale, guide) into a CUDA graph with static input buffers and replayed.  Weights are read
+        from the flat bf16 shadows, whose storage is stable: the cache is dropped when this store is re-attached, and a
+        guide's entry is keyed by its shadow's address too.  The entry holds the guide, so its id is not reused while
+        the entry exists.  MDT_CUDA_GRAPH=0 disables the graphs."""
         key = (tuple(xf.shape), None if lab is None else tuple(lab.shape), cfg_scale)
+        if guide is not None:
+            key += (id(guide), guide._store.w16.data_ptr())
         ent = self._graphs.get(key)
         if ent is None:
             sx, ss = torch.empty_like(xf), torch.empty_like(sig)
@@ -313,15 +321,15 @@ class EDMPrecond(nn.Module):
             side = torch.cuda.Stream()
             side.wait_stream(cur)
             with torch.cuda.stream(side):  # warm-up outside the capture (lazy kernel attributes, allocator pools)
-                self._eval_eager(sx, ss, sl, cfg_scale)
+                self._eval_eager(sx, ss, sl, cfg_scale, guide)
             cur.wait_stream(side)
             graph = torch.cuda.CUDAGraph()
             n0 = ops.L.LAUNCHES
             with torch.cuda.graph(graph):
-                out = self._eval_eager(sx, ss, sl, cfg_scale)
-            ent = (graph, sx, ss, sl, out, ops.L.LAUNCHES - n0)
+                out = self._eval_eager(sx, ss, sl, cfg_scale, guide)
+            ent = (graph, sx, ss, sl, out, ops.L.LAUNCHES - n0, guide)
             self._graphs[key] = ent
-        graph, sx, ss, sl, out, n_launch = ent
+        graph, sx, ss, sl, out, n_launch, _ = ent
         sx.copy_(xf), ss.copy_(sig)
         if sl is not None:
             sl.copy_(lab)
@@ -366,6 +374,33 @@ class EDMPrecond(nn.Module):
             Fo, _ = self._engine.forward(xf, sig, lab, md, save=False)
             out["x"] = ops.edm_precond_out(Fo, xf, sig, self.sigma_data, p).to(x.dtype)
         return out
+
+    def check_guide(self, guide):
+        """Raise ValueError unless `guide` can guide this network: an EDMPrecond with the same image geometry, classes
+        and sigma_data.  Depth, width, patch size and use_decoder may differ."""
+        if not isinstance(guide, EDMPrecond):
+            raise ValueError(f"the guide must be an EDMPrecond, not {type(guide).__name__}")
+        for k in ("img_resolution", "img_channels", "num_classes", "sigma_data"):
+            if getattr(guide, k) != getattr(self, k):
+                raise ValueError(f"the guide's {k} is {getattr(guide, k)}, the network's {getattr(self, k)}")
+
+    def forward_guided(self, x, sigma, class_labels, guide, guidance):
+        """D_x guided by a second network (autoguidance, Karras et al., NeurIPS 2024):
+        D = D_guide + guidance * (D_self - D_guide), from one eval pass of each network at batch B with the same
+        labels (None for unconditional networks), combined in fp32 with the EDM output scaling.  Returns D_x like
+        `forward(...)['x']`."""
+        self.check_guide(guide)
+        w = float(guidance)
+        if not math.isfinite(w):
+            raise ValueError(f"guidance must be finite, got {guidance}")
+        self._ready(x.device)
+        guide._ready(x.device)
+        xf, sig, lab = self._norm_inputs(x, sigma, class_labels)
+        use_graph = not self.training and os.environ.get("MDT_CUDA_GRAPH", "1") != "0" \
+            and not torch.cuda.is_current_stream_capturing()
+        with torch.no_grad():
+            fn = self._eval_graphed if use_graph else self._eval_eager
+            return fn(xf, sig, lab, w, guide).to(x.dtype)
 
 
 Precond_models = {"edm": EDMPrecond}

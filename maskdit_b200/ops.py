@@ -221,6 +221,15 @@ def cfg_precond_out(F, xin, sigma, sigma_data, cfg_scale, p):
     return Dx
 
 
+def guided_precond_out(F_main, p_main, F_guide, p_guide, xin, sigma, sigma_data, w):
+    """D = c_skip x + c_out (Fg + w (Fm - Fg)); each F token-major in its own network's patch size."""
+    B, C, R, _ = xin.shape
+    Dx = torch.empty_like(xin)
+    check(lib().mdt_guided_precond_out(ptr(F_main), p_main, ptr(F_guide), p_guide, ptr(xin), ptr(sigma), sigma_data,
+                                       w, ptr(Dx), B, C, R, stream_ptr()), "mdt_guided_precond_out")
+    return Dx
+
+
 def heun_update(mode, x_hat, denoised, d_cur, x_next, x_next_f32, t_hat, t_next):
     check(lib().mdt_heun_update(mode, ptr(x_hat), ptr(denoised), ptr(d_cur), ptr(x_next), ptr(x_next_f32),
                                 float(t_hat), float(t_next), x_hat.numel(), stream_ptr()), "mdt_heun_update")

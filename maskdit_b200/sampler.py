@@ -3,7 +3,9 @@
 Same signature and semantics as the reference `edm_sampler` (fp64 state, 2N-1 network evaluations, `randn_like`
 consumed once per step even when S_churn = 0).  With a `maskdit_b200.EDMPrecond` network each evaluation is one
 eval-mode engine pass at batch 2B with the classifier-free-guidance combine fused into the output kernel, and the
-fp64 Euler/Heun state updates are single fused kernels.
+fp64 Euler/Heun state updates are single fused kernels.  Both samplers can instead guide with a second network
+(`guide_net`, `guidance`: autoguidance) and apply either guidance only inside a noise-level interval
+(`guidance_interval`); see `_denoiser`.
 """
 from __future__ import annotations
 
@@ -13,9 +15,49 @@ import torch
 from . import ops
 
 
+def _denoiser(net, class_labels, cfg_scale, feat, guide_net, guidance, guidance_interval):
+    """The sampler's network evaluation D(x; sigma) as a function of (x, sigma as a Python float).
+
+    Without guide_net / guidance_interval it is the reference's call `net(x, sigma, labels, cfg_scale)`.  With a guide
+    network, D = D_guide + guidance (D_net - D_guide) (autoguidance, Karras et al., NeurIPS 2024); guidance == 1 is the
+    unguided network and evaluates no guide.  guidance_interval = (lo, hi) applies the active guidance (CFG or the
+    guide) only where lo < sigma <= hi (Kynkaanniemi et al., NeurIPS 2024), decided per evaluation; elsewhere the
+    evaluation is the unguided `net(x, sigma, labels, None)`."""
+    if guide_net is not None:
+        if cfg_scale is not None:
+            raise ValueError("cfg_scale and guide_net are mutually exclusive")
+        if guidance is None:
+            raise ValueError("guide_net needs a guidance weight")
+        net.check_guide(guide_net)
+        guidance = float(guidance)
+        if not np.isfinite(guidance):
+            raise ValueError(f"guidance must be finite, got {guidance}")
+    elif guidance is not None:
+        raise ValueError("guidance is the weight of guide_net; classifier-free guidance takes cfg_scale")
+    if guidance_interval is not None:
+        lo, hi = (float(v) for v in guidance_interval)
+        if not lo < hi:
+            raise ValueError(f"guidance_interval needs sigma_lo < sigma_hi, got ({lo}, {hi})")
+        if guide_net is None and cfg_scale is None:
+            raise ValueError("guidance_interval needs cfg_scale or guide_net")
+
+    def denoise(x, sigma):
+        s = torch.tensor(sigma, dtype=torch.float64, device=x.device)
+        if (guidance_interval is not None and not lo < sigma <= hi) or (guide_net is not None and guidance == 1):
+            return net(x, s, class_labels, None, feat=feat)["x"]
+        if guide_net is None:
+            return net(x, s, class_labels, cfg_scale, feat=feat)["x"]
+        return net.forward_guided(x, s, class_labels, guide_net, guidance)
+
+    return denoise
+
+
 def edm_sampler(net, latents, class_labels=None, cfg_scale=None, feat=None, randn_like=torch.randn_like,
                 num_steps=18, sigma_min=0.002, sigma_max=80, rho=7, S_churn=0, S_min=0, S_max=float("inf"),
-                S_noise=1):
+                S_noise=1, guide_net=None, guidance=None, guidance_interval=None):
+    """`guide_net`, `guidance` and `guidance_interval` (all opt-in) select guidance by a second network and limit the
+    guidance to a noise-level interval: see `_denoiser`.  Without them every evaluation is the reference's call."""
+    denoise = _denoiser(net, class_labels, cfg_scale, feat, guide_net, guidance, guidance_interval)
     sigma_min = max(sigma_min, net.sigma_min)
     sigma_max = min(sigma_max, net.sigma_max)
     dev = latents.device
@@ -36,12 +78,10 @@ def edm_sampler(net, latents, class_labels=None, cfg_scale=None, feat=None, rand
             x_hat = (x_next + float(np.sqrt(t_hat ** 2 - t_cur ** 2)) * S_noise * noise).contiguous()
         else:
             x_hat = x_next.clone()
-        den = net(x_hat.float(), torch.tensor(t_hat, dtype=torch.float64, device=dev), class_labels, cfg_scale,
-                  feat=feat)["x"].float().contiguous()
+        den = denoise(x_hat.float(), t_hat).float().contiguous()
         ops.heun_update(0, x_hat, den, d_cur, x_next, x32, t_hat, t_next)          # Euler step (sample.py:56-58)
         if k < num_steps - 1:
-            den = net(x32, torch.tensor(t_next, dtype=torch.float64, device=dev), class_labels, cfg_scale,
-                      feat=feat)["x"].float().contiguous()
+            den = denoise(x32, t_next).float().contiguous()
             ops.heun_update(1, x_hat, den, d_cur, x_next, x32, t_hat, t_next)      # 2nd-order correction (:61-64)
     return x_next
 
@@ -92,10 +132,13 @@ def _iddpm_sigmas(M, C_1, C_2, sigma_min, sigma_max, num_steps):
 def ablation_sampler(net, latents, class_labels=None, cfg_scale=None, feat=None, randn_like=torch.randn_like,
                      num_steps=18, sigma_min=None, sigma_max=None, rho=7, solver="heun", discretization="edm",
                      schedule="linear", scaling="none", epsilon_s=1e-3, C_1=0.001, C_2=0.008, M=1000, alpha=1,
-                     S_churn=0, S_min=0, S_max=float("inf"), S_noise=1):
+                     S_churn=0, S_min=0, S_max=float("inf"), S_noise=1, guide_net=None, guidance=None,
+                     guidance_interval=None):
     """Generalised sampler (reference: sample.py:73-188), same signature.  All schedule quantities are fp64 host
     scalars; the state lives on the device in fp64 and every update (churn, Euler, the alpha-weighted 2nd-order
-    correction) is one `mdt_lincomb_f64` launch that also emits the next fp32 network input x / s(t)."""
+    correction) is one `mdt_lincomb_f64` launch that also emits the next fp32 network input x / s(t).  The opt-in
+    `guide_net`, `guidance` and `guidance_interval` are those of `edm_sampler`; the interval is decided on sigma(t)."""
+    denoise = _denoiser(net, class_labels, cfg_scale, feat, guide_net, guidance, guidance_interval)
     assert solver in ("euler", "heun") and discretization in ("vp", "ve", "iddpm", "edm")
     assert schedule in ("vp", "ve", "linear") and scaling in ("vp", "none")
     vp_sig = lambda bd, bm, t: float((np.e ** (0.5 * bd * (t ** 2) + bm * t) - 1) ** 0.5)  # noqa: E731
@@ -133,7 +176,7 @@ def ablation_sampler(net, latents, class_labels=None, cfg_scale=None, feat=None,
         ops.lincomb_f64(sch.s(t_hat) / sch.s(t_cur), x_next, churn, noise, out=x_hat, out_f32=xin,
                         f32_scale=1.0 / sch.s(t_hat))
         h = t_next - t_hat
-        den = net(xin, f64(sch.sigma(t_hat)), class_labels, cfg_scale, feat=feat)["x"].float().contiguous()
+        den = denoise(xin, sch.sigma(t_hat)).float().contiguous()
         A, Bc = sch.ode_coeffs(t_hat)
         ops.lincomb_f64(A, x_hat, 0.0, None, -Bc, den, out=d_cur)                       # d_cur = A x_hat - B D
         if solver == "euler" or i == num_steps - 1:
@@ -141,7 +184,7 @@ def ablation_sampler(net, latents, class_labels=None, cfg_scale=None, feat=None,
             continue
         t_prime = t_hat + alpha * h
         ops.lincomb_f64(1.0, x_hat, alpha * h, d_cur, out=x_prime, out_f32=xin, f32_scale=1.0 / sch.s(t_prime))
-        den = net(xin, f64(sch.sigma(t_prime)), class_labels, cfg_scale, feat=feat)["x"].float().contiguous()
+        den = denoise(xin, sch.sigma(t_prime)).float().contiguous()
         A2, B2 = sch.ode_coeffs(t_prime)
         w1, w2 = h * (1 - 1 / (2 * alpha)), h / (2 * alpha)
         ops.lincomb_f64(w2 * A2, x_prime, w1, d_cur, -w2 * B2, den, out=x_prime)       # w1 d_cur + w2 d_prime
