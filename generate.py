@@ -24,6 +24,7 @@ import numpy as np
 import torch
 
 from maskdit_b200.config import build_net, load_config, parse_float_none, parse_int_list
+from maskdit_b200.maskdit import eval_state_dict
 from maskdit_b200 import ops
 from maskdit_b200.sampler import ablation_sampler, edm_sampler, rank_seed_batches, write_png
 
@@ -133,11 +134,11 @@ def main(argv=None):
     if args.ckpt_path:
         # trusted checkpoint: reference checkpoints hold an argparse.Namespace under 'args' (train.py:259-265)
         ck = torch.load(args.ckpt_path, map_location=device, weights_only=False)
-        net.load_state_dict({k.replace("_orig_mod.", ""): v for k, v in ck["ema"].items()})
+        net.load_state_dict(eval_state_dict(net, ck["ema"]))
     gkw = {}
     if args.guidance is not None:
         guide = build_net(load_config(args.guide_config or args.config)).to(device).eval()
-        guide.load_state_dict(guide_state_dict(args))
+        guide.load_state_dict(eval_state_dict(guide, guide_state_dict(args)))
         net.check_guide(guide)
         gkw = dict(guide_net=guide, guidance=args.guidance)
     if args.guidance_interval is not None:

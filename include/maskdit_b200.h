@@ -197,6 +197,24 @@ int mdt_gather_rows_bf16(const void* in_bf16, const int64_t* idx, void* out_bf16
 int mdt_edm_loss(const float* F, const float* xin, const float* y, const float* sigma, const float* mask,
                  const float* gl, float sigma_data, float mae_coef, float* loss, float* Dx, void* dF_bf16, int B,
                  int C, int R, int p, void* stream);
+/* Learned loss weighting (EDM2 uncertainty weighting, Karras et al. CVPR 2024): per sample
+ *   c = ln(sigma) / 4,  phi_j(c) = sqrt(2) cos(freqs_j c + phases_j),  u = sum_{j < channels} w_j phi_j(c)
+ * (phi in fp64 rounded to fp32, the sum in fp32; 1 <= channels <= 256).  mdt_edm_loss_logvar is mdt_edm_loss's pass
+ * with the EDM term E also summed apart from the MAE term M (mae_coef included): loss[b] = E + M bit for bit as
+ * mdt_edm_loss writes it, objective[b] = exp(-u) E + u + M, evaluated as loss + expm1(-u) E + u (so at u = 0 it is
+ * loss bit for bit), u[b].  With gl: dF_bf16 = d(sum_b gl[b]*objective[b]) / dF, i.e. the
+ * EDM term's seed scaled by gl[b] exp(-u) and the MAE term's by gl[b], and du[b] = gl[b] (1 - exp(-u) E) (both
+ * optional, both need gl).  No Dx output.
+ * mdt_logvar: u[b] alone, the same bits.  mdt_logvar_wgrad: dw[j] += sum_b du[b] phi_j(c_b), summed over b in index
+ * order in fp64 and added once (no atomics: the same bits on every run).                                       */
+int mdt_edm_loss_logvar(const float* F, const float* xin, const float* y, const float* sigma, const float* mask,
+                        const float* gl, float sigma_data, float mae_coef, const float* freqs, const float* phases,
+                        const float* w, int channels, float* objective, float* loss, float* u, float* du,
+                        void* dF_bf16, int B, int C, int R, int p, void* stream);
+int mdt_logvar(const float* sigma, const float* freqs, const float* phases, const float* w, int channels, int B,
+               float* u, void* stream);
+int mdt_logvar_wgrad(const float* sigma, const float* freqs, const float* phases, const float* du, int channels, int B,
+                     float* dw, void* stream);
 /* Step front (train.py:206,209 + train_utils/loss.py:35-39 + utils.py:59-65) in one pass, given pre-drawn randoms:
  *   y  = scale_factor * (mean + exp(0.5 * clamp(logvar, -30, 20)) * eps)   moments [B,2C,R,R] = (mean | logvar)
  *   sigma[b] = exp(P_std * rnd_normal[b] + P_mean) ;  yn = y + noise_unit * sigma[b]
@@ -372,7 +390,9 @@ int mdt_get_deterministic(void);
  * Packed blob (element offsets shared by the fp32 master w32, the bf16 shadow w16 and the fp32 gradient):
  *   [adaLN_modulation.1.weight of blocks 0..depth-1, decoder_layer, decoder_blocks 0.., final_layer]
  *   [the matching adaLN biases] [all other trainable tensors in registration order] [pos_embed, decoder_pos_embed]
- * every tensor on a 64-element boundary; names = the reference's state-dict keys (models/maskdit.py:242-332).
+ * every tensor on a 64-element boundary; names = the reference's state-dict keys (models/maskdit.py:242-332).  A
+ * handle with a learned loss weighting (mdt_model_set_logvar) adds logvar_linear.weight as the last trainable tensor
+ * and logvar_fourier.freqs / .phases after the position tables.
  *
  * Decoder-less DiT (use_decoder=False, the reference's default, models/maskdit.py:254): dec_hidden = dec_depth =
  * dec_heads = dec_mlp_hidden = 0 and has_mask_token = 0.  Any other combination with a zero dec_* field is rejected.
@@ -410,6 +430,13 @@ int mdt_model_mod_width(const mdt_model* m); /* columns of the concatenated adaL
  * mdt_forward(save = 1) at the same r, at r = 0 the workspace of a last saving forward that recomputed.              */
 int mdt_model_set_recompute(mdt_model* m, int r);
 int mdt_model_get_recompute(const mdt_model* m); /* -1 for a NULL handle */
+
+/* Learned loss weighting u(sigma) (mdt_edm_loss_logvar) with `channels` Fourier features: lays the handle out again with
+ * three more tensors, `logvar_linear.weight` [1, channels] at the end of the trainable region and
+ * `logvar_fourier.freqs`, `logvar_fourier.phases` [channels] in the frozen region after the position tables.  0 (the
+ * default) is the layout without them.  MDT_ERR_ARG for channels < 0 or > 256, and once the handle has sized or laid
+ * out a workspace (mdt_workspace_bytes, mdt_forward).                                                               */
+int mdt_model_set_logvar(mdt_model* m, int channels);
 
 /* Workspace bytes for batch B with T kept tokens per sample (T <= 0: no token dropping, T = L).
  * training != 0: every activation the backward needs stays resident (+ the backward's scratch; with recomputation only

@@ -84,6 +84,9 @@ _SIGS = {
     "mdt_unmask_tokens_bwd": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
     "mdt_gather_rows_bf16": [_P, _P, _P, _I, _I, _I, _I, _P],
     "mdt_edm_loss": [_P, _P, _P, _P, _P, _P, _F, _F, _P, _P, _P, _I, _I, _I, _I, _P],
+    "mdt_edm_loss_logvar": [_P, _P, _P, _P, _P, _P, _F, _F, _P, _P, _P, _I, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
+    "mdt_logvar": [_P, _P, _P, _P, _I, _I, _P, _P],
+    "mdt_logvar_wgrad": [_P, _P, _P, _P, _I, _I, _P, _P],
     "mdt_step_front": [_P, _P, _P, _P, _P, _F, _F, _F, _F, _P, _P, _P, _P, _I, _I, _I, _I, _P],
     "mdt_edm_precond_out": [_P, _P, _P, _F, _P, _I, _I, _I, _I, _P],
     "mdt_edm_precond_out_bwd": [_P, _P, _F, _P, _I, _I, _I, _I, _P],
@@ -99,6 +102,7 @@ _SIGS = {
     "mdt_model_mod_width": [_P],
     "mdt_model_set_recompute": [_P, _I],
     "mdt_model_get_recompute": [_P],
+    "mdt_model_set_logvar": [_P, _I],
     "mdt_forward": [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _LL, _P, _P],
     "mdt_backward": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _P, _LL, GRAD_READY_FN, _P, _P],
     "mdt_nccl_unique_id": [_P],

@@ -76,9 +76,11 @@ def parse_float_none(s):
 
 
 def build_net(cfg: Node, **extra):
-    """Precond_models[config.model.precond](...) exactly as train.py:123-131 / generate.py:31-40 call it."""
+    """Precond_models[config.model.precond](...) exactly as train.py:123-131 / generate.py:31-40 call it, plus
+    `model.logvar_channels` (the learned loss weighting, not in the reference's configs: default 0, off)."""
     from .maskdit import Precond_models
     m = cfg.model
     return Precond_models[m.precond](img_resolution=m.in_size, img_channels=m.in_channels, num_classes=m.num_classes,
                                      model_type=m.model_type, use_decoder=m.use_decoder,
-                                     mae_loss_coef=m.mae_loss_coef, pad_cls_token=m.pad_cls_token, **extra)
+                                     mae_loss_coef=m.mae_loss_coef, pad_cls_token=m.pad_cls_token,
+                                     logvar_channels=int(m.get("logvar_channels", 0) or 0), **extra)

@@ -12,6 +12,7 @@
 // Packed parameter blob (fp32 master `w32`, bf16 shadow `w16`, fp32 gradient `grad`: same element offsets):
 //   [adaLN_modulation.1.weight of blocks 0..depth-1, decoder_layer, decoder_blocks 0..dec_depth-1, final_layer]
 //   [the matching adaLN biases] [every other trainable tensor in registration order] [pos_embed, decoder_pos_embed]
+// (with mdt_model_set_logvar: logvar_linear.weight the last trainable tensor, logvar_fourier.* after the tables)
 // each tensor starting on a 64-element boundary.  The decoder-less DiT (use_decoder=False, models/maskdit.py:254,
 // 308-331: all four dec_* fields 0) has no decoder_layer, decoder blocks, decoder_pos_embed or mask token, and its
 // final layer reads the encoder width.  `build_layout` is the only place these offsets are decided:
@@ -67,6 +68,9 @@ struct mdt_model {
   std::vector<NamedTensor> named;  // registration order
   std::vector<int> order;          // blob order (indices into named)
   int recompute = 0;               // blocks whose activations the backward recomputes (mdt_model_set_recompute)
+  int logvar_channels = 0;         // learned loss weighting u(sigma) (mdt_model_set_logvar); 0: none
+  Tensor lv_freqs, lv_phases, lv_w;
+  mutable bool planned = false;    // a workspace was sized or laid out: the layout is final
   // the workspace of the last mdt_forward(save = 1) and the recompute count it was laid out for: mdt_backward refuses
   // to read a workspace with another count's plan
   mutable const void* fwd_ws = nullptr;
@@ -142,6 +146,13 @@ void build_layout(mdt_model* m) {
   add("model.final_layer.linear.bias", &m->flb, m->pd, 2);
   add("model.final_layer.adaLN_modulation.1.weight", &m->ada_w[head], 2ll * Df * D, 0, head);
   add("model.final_layer.adaLN_modulation.1.bias", &m->ada_b[head], 2ll * Df, 1, head);
+  // learned loss weighting (EDMPrecond registers it after model.*): the weight ends the trainable region, the Fourier
+  // features follow the position tables
+  if (m->logvar_channels > 0) {
+    add("logvar_fourier.freqs", &m->lv_freqs, m->logvar_channels, 3);
+    add("logvar_fourier.phases", &m->lv_phases, m->logvar_channels, 3);
+    add("logvar_linear.weight", &m->lv_w, m->logvar_channels, 2);
+  }
   m->NA = static_cast<int>(mod);
   // blob order: group 0 by rank, group 1 by rank, group 2 in registration order, group 3 last
   i64 off = 0;
@@ -521,9 +532,19 @@ int mdt_model_set_recompute(mdt_model* m, int r) {
 
 int mdt_model_get_recompute(const mdt_model* m) { return m ? m->recompute : -1; }
 
+int mdt_model_set_logvar(mdt_model* m, int channels) {
+  if (!m || channels < 0 || channels > 256 || m->planned) return MDT_ERR_ARG;
+  m->logvar_channels = channels;
+  m->named.clear();
+  m->order.clear();
+  build_layout(m);
+  return MDT_OK;
+}
+
 long long mdt_workspace_bytes(const mdt_model* m, int B, int T, int training) {
   if (!m || B <= 0) return -1;
   if (T <= 0) T = m->L;
+  m->planned = true;
   return make_plan(m, B, T, training != 0, training != 0).total;
 }
 
@@ -534,6 +555,7 @@ int mdt_forward(const mdt_model* m, const float* w32, const void* w16, const flo
   if (T <= 0) T = m->L;
   if ((ids_keep == nullptr) != (ids_restore == nullptr) || (!ids_keep && T != m->L)) return MDT_ERR_ARG;
   if (m->cfg.num_classes > 0 && !labels) return MDT_ERR_ARG;
+  m->planned = true;
   const Plan p = make_plan(m, B, T, save != 0, save != 0);
   if (p.total > workspace_bytes || (reinterpret_cast<uintptr_t>(workspace) & 255)) return MDT_ERR_ARG;
   if (save) m->fwd_ws = workspace, m->fwd_r = m->recompute;

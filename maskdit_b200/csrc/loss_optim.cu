@@ -36,14 +36,38 @@ MDT_DEVINL float block_sum(float v, float* s_buf) {
   return t;
 }
 
+// ---- Learned loss weighting (EDM2 uncertainty weighting, Karras et al. CVPR 2024) --------------------------------------
+// u(sigma) = sum_j w_j phi_j(c), c = ln(sigma) / 4, phi_j(c) = sqrt(2) cos(freqs_j c + phases_j), j < C <= 256.
+constexpr int kMaxLogvar = 256;
+struct LogvarArgs {
+  const float *freqs, *phases, *w;   // [C] each: the frozen Fourier features and the [1, C] linear's weight
+  int C;
+  float *objective, *u, *du;         // [B] each (du only with a gradient seed)
+};
+
+// The feature is evaluated in fp64 and rounded once: |freqs_j c| reaches ~30, where an fp32 argument alone is ~2e-6 off.
+MDT_DEVINL float logvar_phi(float freq, float phase, float sg) {
+  const double c = log(static_cast<double>(sg)) * 0.25;
+  return static_cast<float>(1.4142135623730951 * cos(static_cast<double>(freq) * c + static_cast<double>(phase)));
+}
+
+// u of one sample: thread j < C forms w_j phi_j, one block sum of 256 threads (every caller launches 256).
+MDT_DEVINL float logvar_u(const LogvarArgs& lv, float sg, float* s_buf) {
+  const int j = threadIdx.x;
+  return block_sum(j < lv.C ? lv.w[j] * logvar_phi(lv.freqs[j], lv.phases[j], sg) : 0.f, s_buf);
+}
+
 // One block per sample.  Thread per token.  kReg: the token's D and x live in registers (pd <= kMaxPD); otherwise
 // (patch 8: pd = 256) every later pass re-reads F and xin and recomputes D with the same expression.
-template <bool kReg>
+// kLogvar: also the learned weighting's objective exp(-u) E + u + mae_coef M, where E is the EDM term, summed apart,
+// and E + mae_coef M is `loss` (accumulated as without kLogvar): the EDM term's gradient seed is scaled by
+// gl[b] exp(-u), the MAE term's by gl[b], and du[b] = gl[b] (1 - exp(-u) E).
+template <bool kReg, bool kLogvar>
 __global__ void __launch_bounds__(256)
 edm_loss_kernel(const float* __restrict__ F, const float* __restrict__ xin, const float* __restrict__ y,
                 const float* __restrict__ sigma, const float* __restrict__ mask, const float* __restrict__ gl,
                 float sd, float mae_coef, float* __restrict__ loss, float* __restrict__ Dx,
-                __nv_bfloat16* __restrict__ dF, PatchGeom gm) {
+                __nv_bfloat16* __restrict__ dF, PatchGeom gm, LogvarArgs lv) {
   __shared__ float s_buf[32];
   const int b = blockIdx.x;
   const float sg = sigma[b];
@@ -51,6 +75,11 @@ edm_loss_kernel(const float* __restrict__ F, const float* __restrict__ xin, cons
   const float c_skip = sd * sd / den, c_out = sg * sd * rsqrtf(den);
   const float w = den / ((sg * sd) * (sg * sd));
   const float glb = gl ? gl[b] : 0.f;
+  float u = 0.f, glb_e = glb, acc_e = 0.f;   // glb_e: the EDM term's gradient scale
+  if constexpr (kLogvar) {
+    u = logvar_u(lv, sg, s_buf);
+    glb_e = glb * expf(-u);
+  }
   float n_mask = 0.f;
   if (mask) {
     float cnt = 0.f;
@@ -83,15 +112,17 @@ edm_loss_kernel(const float* __restrict__ F, const float* __restrict__ xin, cons
     const float inv_pd = 1.f / gm.pd;
     if (!mask) {
       acc += w * se;  // mean over all elements of the sample, applied below
+      if constexpr (kLogvar) acc_e += w * se;
       if (dF) {
-        const float k = glb * w * 2.f * c_out / (static_cast<float>(gm.L) * gm.pd);
+        const float k = glb_e * w * 2.f * c_out / (static_cast<float>(gm.L) * gm.pd);
         for (int j = 0; j < gm.pd; ++j)
           dF[(static_cast<size_t>(b) * gm.L + l) * gm.pd + j] = __float2bfloat16_rn(k * (dat(j) - y[gm.pix(b, l, j)]));
       }
     } else {
       const float mk = mask[static_cast<size_t>(b) * gm.L + l];
       float contrib = (1.f - mk) * w * se * inv_pd / n_keep;
-      float k_edm = glb * (1.f - mk) / n_keep * w * 2.f * inv_pd * c_out;
+      if constexpr (kLogvar) acc_e += contrib;
+      float k_edm = glb_e * (1.f - mk) / n_keep * w * 2.f * inv_pd * c_out;
       float k_mae = 0.f, mu = 0.f, rstd = 0.f;
       if (mae_coef > 0.f && mk != 0.f) {
         // mae_loss (train_utils/loss.py:87-101): target = per-patch normalised NOISY INPUT, unbiased variance
@@ -120,7 +151,37 @@ edm_loss_kernel(const float* __restrict__ F, const float* __restrict__ xin, cons
     }
   }
   const float tot = block_sum(acc, s_buf);
+  if constexpr (kLogvar) {
+    float e = block_sum(acc_e, s_buf);
+    if (threadIdx.x == 0) {
+      const float lb = mask ? tot : tot / (static_cast<float>(gm.L) * gm.pd);
+      if (!mask) e /= static_cast<float>(gm.L) * gm.pd;
+      // exp(-u) E + u + M written as (E + M) + expm1(-u) E + u: at u = 0 exactly the reference loss
+      lv.objective[b] = lb + expm1f(-u) * e + u;
+      lv.u[b] = u;
+      if (lv.du) lv.du[b] = glb * (1.f - expf(-u) * e);
+    }
+  }
   if (threadIdx.x == 0) loss[b] = mask ? tot : tot / (static_cast<float>(gm.L) * gm.pd);
+}
+
+// u(sigma_b) alone, one block of 256 threads per sample: the loss kernel's arithmetic, so the same bits.
+__global__ void __launch_bounds__(256) logvar_kernel(const float* __restrict__ sigma, LogvarArgs lv) {
+  __shared__ float s_buf[32];
+  const float u = logvar_u(lv, sigma[blockIdx.x], s_buf);
+  if (threadIdx.x == 0) lv.u[blockIdx.x] = u;
+}
+
+// dw_j += sum_i du_i phi_j(c_i): thread j sums the samples in index order in fp64 (no atomics, the same bits on every
+// run) and adds the rounded sum once, so gradient-accumulation rounds add up.
+__global__ void __launch_bounds__(256) logvar_wgrad_kernel(const float* __restrict__ sigma, const float* __restrict__ du,
+                                                           LogvarArgs lv, int B, float* __restrict__ dw) {
+  const int j = threadIdx.x;
+  if (j >= lv.C) return;
+  const float f = lv.freqs[j], ph = lv.phases[j];
+  double acc = 0.0;
+  for (int i = 0; i < B; ++i) acc += static_cast<double>(du[i]) * static_cast<double>(logvar_phi(f, ph, sigma[i]));
+  dw[j] += static_cast<float>(acc);
 }
 
 // D = c_skip*x + c_out*unpatchify(F) ; optional CFG combine of two halves of F
@@ -576,9 +637,44 @@ int mdt_edm_loss(const float* F, const float* xin, const float* y, const float* 
   if (dF_bf16 && !gl) return MDT_ERR_ARG;
   PatchGeom gm;
   if (int rc = make_geom(&gm, C, R, p)) return rc;
-  auto kern = gm.pd <= kMaxPD ? edm_loss_kernel<true> : edm_loss_kernel<false>;
+  auto kern = gm.pd <= kMaxPD ? edm_loss_kernel<true, false> : edm_loss_kernel<false, false>;
   kern<<<B, 256, 0, S(stream)>>>(F, xin, y, sigma, mask, gl, sigma_data, mae_coef, loss, Dx,
-                                 static_cast<__nv_bfloat16*>(dF_bf16), gm);
+                                 static_cast<__nv_bfloat16*>(dF_bf16), gm, LogvarArgs{});
+  return launch_status();
+}
+
+static bool logvar_args_ok(const float* freqs, const float* phases, int channels) {
+  return freqs && phases && channels >= 1 && channels <= kMaxLogvar;
+}
+
+int mdt_edm_loss_logvar(const float* F, const float* xin, const float* y, const float* sigma, const float* mask,
+                        const float* gl, float sigma_data, float mae_coef, const float* freqs, const float* phases,
+                        const float* w, int channels, float* objective, float* loss, float* u, float* du,
+                        void* dF_bf16, int B, int C, int R, int p, void* stream) {
+  if (!F || !xin || !y || !sigma || !loss || !objective || !u || !w || B <= 0) return MDT_ERR_ARG;
+  if (!logvar_args_ok(freqs, phases, channels) || ((dF_bf16 || du) && !gl)) return MDT_ERR_ARG;
+  PatchGeom gm;
+  if (int rc = make_geom(&gm, C, R, p)) return rc;
+  const LogvarArgs lv{freqs, phases, w, channels, objective, u, du};
+  auto kern = gm.pd <= kMaxPD ? edm_loss_kernel<true, true> : edm_loss_kernel<false, true>;
+  kern<<<B, 256, 0, S(stream)>>>(F, xin, y, sigma, mask, gl, sigma_data, mae_coef, loss, nullptr,
+                                 static_cast<__nv_bfloat16*>(dF_bf16), gm, lv);
+  return launch_status();
+}
+
+int mdt_logvar(const float* sigma, const float* freqs, const float* phases, const float* w, int channels, int B,
+               float* u, void* stream) {
+  if (!sigma || !w || !u || B <= 0 || !logvar_args_ok(freqs, phases, channels)) return MDT_ERR_ARG;
+  logvar_kernel<<<B, 256, 0, S(stream)>>>(sigma, LogvarArgs{freqs, phases, w, channels, nullptr, u, nullptr});
+  return launch_status();
+}
+
+int mdt_logvar_wgrad(const float* sigma, const float* freqs, const float* phases, const float* du, int channels, int B,
+                     float* dw, void* stream) {
+  if (!sigma || !du || !dw || B <= 0 || !logvar_args_ok(freqs, phases, channels)) return MDT_ERR_ARG;
+  logvar_wgrad_kernel<<<1, 256, 0, S(stream)>>>(sigma, du,
+                                                LogvarArgs{freqs, phases, nullptr, channels, nullptr, nullptr, nullptr},
+                                                B, dw);
   return launch_status();
 }
 

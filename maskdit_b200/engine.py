@@ -372,6 +372,8 @@ class CEngine:
         h = ctypes.c_void_p()
         ops.check(L.mdt_model_create(ctypes.byref(mc), ctypes.byref(h)), "mdt_model_create", 0)
         self._h, self._L = h, L
+        if getattr(cfg, "logvar_channels", 0):   # the learned loss weighting's tensors join the layout
+            ops.check(L.mdt_model_set_logvar(h, cfg.logvar_channels), "mdt_model_set_logvar", 0)
         self.NA = L.mdt_model_mod_width(h)   # width of the modulation vector = rows of the adaLN weight matrix
         # Activation recomputation (`mdt_model_set_recompute`) of the training pass.  `recompute` None: automatic, i.e.
         # nothing is recomputed unless the workspace allocation runs out of memory, then the smallest count that fits

@@ -3,7 +3,10 @@
 `Losses['edm']` has the reference's constructor and call signature.  When `net` is a `maskdit_b200.EDMPrecond`
 (bare, or wrapped in anything exposing `.module` like DDP / `DataParallelB200`), the loss runs fused:
 noise injection -> engine forward -> ONE kernel for unpatchify + EDM output scaling + weighted-SE / per-patch
-means / masked means / MAE term, whose backward seeds the hand-written network backward.  The random draws are
+means / masked means / MAE term, whose backward seeds the hand-written network backward.  A network with a learned loss
+weighting (`EDMPrecond(logvar_channels=C)`) returns the per-sample objective exp(-u) E + u + mae_coef M when gradients
+are enabled; `last_edm_loss` always holds the reference's per-sample loss E + mae_coef M of the last call (without a
+gradient, and without a weighting, the returned loss itself).  The random draws are
 made with torch's generator in the reference's order (loss.py:35 randn[B,1,1,1]; loss.py:39 randn_like; then
 maskdit.py:102 rand[B,L]) so a seeded run consumes the same RNG stream positions as the reference.
 """
@@ -48,6 +51,36 @@ class _FusedLossFn(torch.autograd.Function):
         _, _, dF = ops.edm_loss(Fo, yn, y, sigma, mask, gl.contiguous().float(), net.sigma_data, mae_coef, p,
                                 want_D=False, want_dF=True)
         net._run_backward(ctx.saved, dF.view(-1, dF.shape[-1]))
+        ctx.saved = ctx.args = None
+        return (torch.zeros(1, device=gl.device),) + (None,) * 7
+
+
+class _FusedLogvarLossFn(torch.autograd.Function):
+    """`_FusedLossFn` with the learned loss weighting: returns (objective, reference loss); the reference loss carries
+    no gradient.  The backward seeds the network with exp(-u)-scaled EDM gradients and adds w's gradient to the flat
+    buffer after the network backward."""
+
+    @staticmethod
+    def forward(ctx, anchor, net, yn, y, sigma, labels, mask_dict, mae_coef):
+        Fo, saved = net._engine.forward(yn, sigma, labels, mask_dict, save=True)
+        mask = mask_dict["mask"] if mask_dict is not None else None
+        p = net.model.patch_size
+        obj, loss, _, _, _ = ops.edm_loss_logvar(Fo, yn, y, sigma, mask, None, net.sigma_data, mae_coef, p,
+                                                 *net._logvar_tensors(), want_dF=False)
+        ctx.net, ctx.saved = net, saved
+        ctx.args = (Fo, yn, y, sigma, mask, mae_coef, p)
+        ctx.mark_non_differentiable(loss)
+        return obj, loss
+
+    @staticmethod
+    def backward(ctx, gl, _):
+        net = ctx.net
+        Fo, yn, y, sigma, mask, mae_coef, p = ctx.args
+        freqs, phases, w = net._logvar_tensors()
+        _, _, _, du, dF = ops.edm_loss_logvar(Fo, yn, y, sigma, mask, gl.contiguous().float(), net.sigma_data,
+                                              mae_coef, p, freqs, phases, w, want_dF=True)
+        net._run_backward(ctx.saved, dF.view(-1, dF.shape[-1]))   # also (re)attaches a zeroed gradient buffer
+        ops.logvar_wgrad(sigma, freqs, phases, du, net._store.gview("logvar_linear.weight").view(-1))
         ctx.saved = ctx.args = None
         return (torch.zeros(1, device=gl.device),) + (None,) * 7
 
@@ -121,6 +154,11 @@ class EDMLoss:
             L = raw.model.num_patches
             md = ops.mask_indices(self._rand((B, L), dev), int(L * (1 - mask_ratio)))  # maskdit.py:101-104
         coef = float(mae_loss_coef) if (mask_ratio > 0 and mae_loss_coef > 0) else 0.0
+        if torch.is_grad_enabled() and raw.logvar_channels:
+            # learned weighting: the objective is what the gradient follows, the reference loss is kept for logging
+            loss, self.last_edm_loss = _FusedLogvarLossFn.apply(raw._anchor, raw, yn, y, sigma, lab, md, coef)
+            self.last_mask_dict = md
+            return loss
         if torch.is_grad_enabled():
             loss = _FusedLossFn.apply(raw._anchor, raw, yn, y, sigma, lab, md, coef)
         else:
@@ -128,6 +166,7 @@ class EDMLoss:
             loss, _, _ = ops.edm_loss(Fo, yn, y, sigma, md["mask"] if md else None, None, raw.sigma_data, coef,
                                       raw.model.patch_size, want_dF=False)
         self.last_mask_dict = md
+        self.last_edm_loss = loss
         return loss
 
 

@@ -172,20 +172,47 @@ class _NetFn(torch.autograd.Function):
         return (torch.zeros(1, device=gD.device),) + (None,) * 5
 
 
+LOGVAR_MAX_CHANNELS = 256
+
+
 class EDMPrecond(nn.Module):
-    """EDM preconditioning wrapper (reference: models/maskdit.py:722-776) running on the sm_90a engine."""
+    """EDM preconditioning wrapper (reference: models/maskdit.py:722-776) running on the sm_90a engine.
+
+    `logvar_channels` C > 0 adds EDM2's learned loss weighting (Karras et al., CVPR 2024; Kendall et al.'s uncertainty
+    weighting), which the reference does not have: a tiny network u(sigma) = sum_j w_j phi_j(c), c = ln(sigma) / 4,
+    phi_j(c) = sqrt(2) cos(freqs_j c + phases_j), j < C <= 256.  `freqs = 2 pi randn(C)` and `phases = 2 pi rand(C)` are
+    drawn in that order at construction from `torch.Generator().manual_seed(0)` on the CPU, so two nets of one config
+    agree; they are frozen (`logvar_fourier.freqs`, `logvar_fourier.phases`).  `w` (`logvar_linear.weight` [1, C], no
+    bias) is trained and starts at zero.  Unlike EDM2 the linear has no forced weight normalisation: no other layer here
+    is magnitude-preserving, and AdamW treats w like every other weight.  The training loss (`Losses['edm']` with
+    gradients) then returns the per-sample objective exp(-u) E + u + mae_coef M, E and M being the EDM and MAE terms;
+    at the optimum exp(u(sigma)) is the expected E at sigma.  The three tensors are registered after `model.*`, so the
+    reference's parameters keep their positions.  0 (the default): none of this exists."""
 
     def __init__(self, img_resolution, img_channels, num_classes=0, sigma_min=0, sigma_max=float("inf"),
-                 sigma_data=0.5, model_type="DiT-B/2", **model_kwargs):
+                 sigma_data=0.5, model_type="DiT-B/2", logvar_channels=0, **model_kwargs):
         super().__init__()
         self.img_resolution, self.img_channels, self.num_classes = img_resolution, img_channels, num_classes
         self.sigma_min, self.sigma_max, self.sigma_data = sigma_min, sigma_max, sigma_data
         self.model_type = model_type
+        self.logvar_channels = int(logvar_channels)
+        if not 0 <= self.logvar_channels <= LOGVAR_MAX_CHANNELS:
+            raise ValueError(f"logvar_channels must be in [0, {LOGVAR_MAX_CHANNELS}], got {logvar_channels}")
         self._ctor = dict(img_resolution=img_resolution, img_channels=img_channels, num_classes=num_classes,
                           sigma_min=sigma_min, sigma_max=sigma_max, sigma_data=sigma_data, model_type=model_type,
-                          **model_kwargs)
+                          logvar_channels=self.logvar_channels, **model_kwargs)
         self.model = DiT_models[model_type](input_size=img_resolution, in_channels=img_channels,
                                             num_classes=num_classes, **model_kwargs)
+        if self.logvar_channels:
+            C, g = self.logvar_channels, torch.Generator().manual_seed(0)
+            self.logvar_fourier = _Node()
+            # on the CPU (the generator's device) also under a `with torch.device(...)` context
+            self.logvar_fourier.freqs = nn.Parameter(2 * np.pi * torch.randn(C, generator=g, device="cpu"),
+                                                     requires_grad=False)
+            self.logvar_fourier.phases = nn.Parameter(2 * np.pi * torch.rand(C, generator=g, device="cpu"),
+                                                      requires_grad=False)
+            self.logvar_linear = _Node()
+            self.logvar_linear.weight = nn.Parameter(torch.zeros(1, C))
         self._store, self._engine, self._anchor = None, None, None
         self._graphs = {}  # CUDA graphs of the eval-mode forward, keyed by input shapes (see _eval_graphed)
 
@@ -200,6 +227,7 @@ class EDMPrecond(nn.Module):
         c.num_patches, c.num_classes, c.sigma_data = m.num_patches, self.num_classes, self.sigma_data
         c.img_resolution, c.img_channels = self.img_resolution, self.img_channels
         c.patch_dim = m.patch_size * m.patch_size * m.out_channels
+        c.logvar_channels = self.logvar_channels
         return c
 
     def _params(self):
@@ -253,7 +281,7 @@ class EDMPrecond(nn.Module):
         new = EDMPrecond(**copy.deepcopy(self._ctor))
         dev = next(self.parameters()).device
         new.to(dev)
-        with torch.no_grad():
+        with torch.no_grad():   # every parameter, the frozen logvar features included
             for (k, p), (_, q) in zip(self.named_parameters(), new.named_parameters()):
                 q.copy_(p)
                 q.requires_grad_(p.requires_grad)
@@ -375,6 +403,24 @@ class EDMPrecond(nn.Module):
             out["x"] = ops.edm_precond_out(Fo, xf, sig, self.sigma_data, p).to(x.dtype)
         return out
 
+    # -- learned loss weighting ------------------------------------------------------------------------------------
+    def _logvar_tensors(self):
+        """(freqs, phases, w) as flat fp32 views of the store (w: [C])."""
+        st = self._store
+        return (st.view32("logvar_fourier.freqs"), st.view32("logvar_fourier.phases"),
+                st.view32("logvar_linear.weight").view(-1))
+
+    @torch.no_grad()
+    def logvar(self, sigma):
+        """u(sigma) [N] fp32 of the learned loss weighting (see the class docstring), one value per element of `sigma`
+        (a tensor or a sequence), on the network's CUDA device (`mdt_logvar`).  Inspection only: no gradient."""
+        if not self.logvar_channels:
+            raise ValueError("this network has no learned loss weighting (logvar_channels = 0)")
+        dev = next(self.parameters()).device
+        self._ready(dev)
+        sig = torch.as_tensor(sigma, dtype=torch.float32).to(dev).reshape(-1).contiguous()
+        return ops.logvar(sig, *self._logvar_tensors())
+
     def check_guide(self, guide):
         """Raise ValueError unless `guide` can guide this network: an EDMPrecond with the same image geometry, classes
         and sigma_data.  Depth, width, patch size and use_decoder may differ."""
@@ -404,3 +450,14 @@ class EDMPrecond(nn.Module):
 
 
 Precond_models = {"edm": EDMPrecond}
+
+
+def eval_state_dict(net, sd):
+    """`sd` ready for `net.load_state_dict` where a network is only evaluated (sampling, guides, the held-out loss):
+    `_orig_mod.` prefixes (torch.compile'd checkpoints) removed and, when `net` has no learned loss weighting, the
+    `logvar_*` tensors of a run trained with one dropped.  Sampling never reads u(sigma), so such a checkpoint samples
+    the same with or without them."""
+    sd = {k.replace("_orig_mod.", ""): v for k, v in sd.items()}
+    if not getattr(net, "logvar_channels", 0):
+        sd = {k: v for k, v in sd.items() if not k.startswith(("logvar_fourier.", "logvar_linear."))}
+    return sd

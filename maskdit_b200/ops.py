@@ -179,6 +179,36 @@ def edm_loss(F, xin, y, sigma, mask, gl, sigma_data, mae_coef, p, want_D=False, 
     return loss, Dx, dF
 
 
+def edm_loss_logvar(F, xin, y, sigma, mask, gl, sigma_data, mae_coef, p, freqs, phases, w, want_dF=True):
+    """`edm_loss` with the learned weighting u(sigma) (mdt_edm_loss_logvar).  Returns (objective, loss, u, du, dF):
+    objective = exp(-u) E + u + M, loss = E + M (`edm_loss`'s bits), u [B]; du [B] and dF only with `gl`."""
+    B, C, R, _ = xin.shape
+    dev = xin.device
+    obj, loss, u = (torch.empty(B, dtype=f32, device=dev) for _ in range(3))
+    du = torch.empty(B, dtype=f32, device=dev) if gl is not None else None
+    dF = torch.empty(F.shape, dtype=bf16, device=dev) if want_dF else None
+    check(lib().mdt_edm_loss_logvar(ptr(F), ptr(xin), ptr(y), ptr(sigma), ptr(mask), ptr(gl), sigma_data, mae_coef,
+                                    ptr(freqs), ptr(phases), ptr(w), freqs.numel(), ptr(obj), ptr(loss), ptr(u),
+                                    ptr(du), ptr(dF), B, C, R, p, stream_ptr()), "mdt_edm_loss_logvar")
+    return obj, loss, u, du, dF
+
+
+def logvar(sigma, freqs, phases, w):
+    """u(sigma) [B] of the learned loss weighting (mdt_logvar)."""
+    _c(sigma, f32), _c(freqs, f32), _c(phases, f32), _c(w, f32)
+    u = torch.empty(sigma.numel(), dtype=f32, device=sigma.device)
+    check(lib().mdt_logvar(ptr(sigma), ptr(freqs), ptr(phases), ptr(w), freqs.numel(), sigma.numel(), ptr(u),
+                           stream_ptr()), "mdt_logvar")
+    return u
+
+
+def logvar_wgrad(sigma, freqs, phases, du, dw):
+    """dw[j] += sum_b du[b] phi_j(c_b) in a fixed order (mdt_logvar_wgrad)."""
+    _c(sigma, f32), _c(freqs, f32), _c(phases, f32), _c(du, f32), _c(dw, f32)
+    check(lib().mdt_logvar_wgrad(ptr(sigma), ptr(freqs), ptr(phases), ptr(du), freqs.numel(), sigma.numel(), ptr(dw),
+                                 stream_ptr()), "mdt_logvar_wgrad")
+
+
 def step_front(moments, eps, rnd_normal, noise_unit, labels=None, drop_u=None, drop_prob=0.0, scale_factor=0.18215,
                P_mean=-1.2, P_std=1.2):
     """moments -> latent, label dropout (in place on `labels`), sigma draw, noise injection: one launch.

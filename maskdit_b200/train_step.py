@@ -110,6 +110,7 @@ class GradComm:
 
 class TrainStep:
     phema_emas = ()   # no post-hoc EMA profiles unless the constructor is given widths
+    edm_loss = None   # the last step's reference per-sample loss (see `step`)
 
     def __init__(self, net: EDMPrecond, ema: EDMPrecond | None = None, lr=1e-4, betas=(0.9, 0.999), eps=1e-8,
                  weight_decay=0.0, ema_decay=0.9999, loss_fn: EDMLoss | None = None, process_group=None,
@@ -465,7 +466,7 @@ class TrainStep:
                 self.st.grad.zero_()
                 loss = loss_call(self.net, gx, gy, mask_ratio, mae_loss_coef)
                 loss.mean().backward()
-                return loss.detach()
+                return loss.detach(), self._last_edm_loss()
 
             cur = torch.cuda.current_stream()
             side = torch.cuda.Stream()
@@ -479,15 +480,25 @@ class TrainStep:
                 out = body()
             ent = (graph, gx, gy, out, ops.L.LAUNCHES - n0)
             self._graphs[key] = ent
-        graph, gx, gy, out, n_launch = ent
+        graph, gx, gy, (out, out_edm), n_launch = ent
         gx.copy_(images), gy.copy_(labels)
         graph.replay()
         ops.L.LAUNCHES += n_launch
-        return out.clone()
+        loss = out.clone()
+        return loss, (out_edm.clone() if out_edm is not None else loss)
+
+    def _last_edm_loss(self):
+        """The reference loss of the last loss call when the network learns its loss weighting, else None."""
+        return self.loss_fn.last_edm_loss.detach() if self.net.logvar_channels else None
 
     def step(self, images, labels, mask_ratio=0.5, mae_loss_coef=0.1, grad_accum=1, moments=False,
              class_dropout_prob=0.0):
-        """One optimisation step on this rank's shard.  Returns the per-sample loss [B] (device tensor).
+        """One optimisation step on this rank's shard.  Returns the per-sample loss [B] (device tensor): the objective
+        the gradient follows, which for a network with a learned loss weighting (`EDMPrecond(logvar_channels=C)`) is
+        exp(-u) E + u + mae_coef M.  `edm_loss` then holds the reference's per-sample loss E + mae_coef M [B] of the
+        step (concatenated over the grad_accum rounds), comparable with runs without the weighting; without one it is
+        the returned tensor.  w, the weighting's one trainable tensor, lives in the flat buffers like every other
+        weight, so AdamW, the EMA, the post-hoc EMA profiles, clipping, the non-finite guard and the exchange cover it.
         `grad_accum` > 1: the shard is cut into that many equal micro-batches whose mean-loss gradients are averaged
         (train.py:211-227 under accelerate's `gradient_accumulation_steps`): the wgrad kernels accumulate into the
         flat buffer anyway, so the rounds simply run back to back and 1/rounds is folded into the optimizer kernel.
@@ -534,19 +545,24 @@ class TrainStep:
                 raise ValueError(f"batch {images.shape[0]} is not divisible by grad_accum {grad_accum}")
             mb = images.shape[0] // grad_accum
             st.grad.zero_()
-            losses = []
+            losses, edm = [], []
             for r in range(grad_accum):
                 lr_ = loss_call(self.net, images[r * mb:(r + 1) * mb], labels[r * mb:(r + 1) * mb], mask_ratio,
                                 mae_loss_coef)
                 lr_.mean().backward()
                 losses.append(lr_.detach())
+                edm.append(self._last_edm_loss())
             loss = torch.cat(losses)
+            edm_loss = torch.cat(edm) if self.net.logvar_channels else loss
         elif self.graph and ops.L.GEMM_PROFILE is None:
-            loss = self._fwd_bwd_graphed(images, labels, mask_ratio, mae_loss_coef, loss_call, moments)
+            loss, edm_loss = self._fwd_bwd_graphed(images, labels, mask_ratio, mae_loss_coef, loss_call, moments)
         else:
             st.grad.zero_()
             loss = loss_call(self.net, images, labels, mask_ratio, mae_loss_coef)
             loss.mean().backward()   # engine backward
+            edm_loss = self._last_edm_loss()
+        loss = loss.detach()
+        self.edm_loss = loss if edm_loss is None else edm_loss
         main = torch.cuda.current_stream()
         n = st.n_train
         # Under the guard the flag must be final before the first optimizer pass.  At world > 1 every rank checks its
@@ -600,4 +616,4 @@ class TrainStep:
         st.mark_shadow_fresh(self.net._params())   # the kernel refreshed the bf16 shadow itself
         if self.ema_st is not None:
             self.ema_st._versions = None           # EMA weights changed behind PyTorch's back: shadow is stale
-        return loss.detach()
+        return loss

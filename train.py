@@ -21,6 +21,9 @@ into the EMA of any width after the run.
 Held-out validation (not in the reference): `--val_every M` scores the EMA every M steps on the first `--val_count`
 items of the latent LMDB split `data.root`/val (`--synthetic`: moments drawn from a fixed seed) at `--val_levels` fixed
 noise levels (`maskdit_b200/validate.py`), a loss that compares across steps and runs; val_loss.py scores checkpoints.
+Learned loss weighting (not in the reference): `model.logvar_channels: 128` in the YAML trains EDM2's u(sigma) with the
+network (`EDMPrecond(logvar_channels=)`); `Train Loss` stays the reference's loss, `Weighted Loss` is the objective, and
+the validation line adds the EMA's u at the validation levels.
 Gradient-norm clipping (not in the reference): `--max_grad_norm 1.0` clips the global gradient norm as
 torch.nn.utils.clip_grad_norm_ does, `--max_grad_norm inf` only measures it; either way the log line reports the
 window's mean and maximum norm.
@@ -61,14 +64,17 @@ def skip_nonfinite(args):
     return not args.no_amp
 
 
-def log_line(step, loss, steps_per_sec, skipped=None, grad_norm=None):
-    """The training log line (the reference's format, train.py:247); `skipped` (a count) and `grad_norm` (the
-    window's mean and max) are appended only when given."""
+def log_line(step, loss, steps_per_sec, skipped=None, grad_norm=None, weighted=None):
+    """The training log line (the reference's format, train.py:247); `skipped` (a count), `grad_norm` (the
+    window's mean and max) and `weighted` (the mean objective of a learned loss weighting) are appended only when
+    given.  `loss` is always the reference's loss, so it compares across runs with and without the weighting."""
     line = f"(step={step:07d}) Train Loss: {loss:.4f}, Train Steps/Sec: {steps_per_sec:.2f}"
     if skipped is not None:
         line += f", Skipped Steps: {skipped}"
     if grad_norm is not None:
         line += f", Grad Norm: {grad_norm[0]:.4g} (max {grad_norm[1]:.4g})"
+    if weighted is not None:
+        line += f", Weighted Loss: {weighted:.4f}"
     return line
 
 
@@ -119,10 +125,14 @@ def build_parser():
     return ap
 
 
-def val_line(step, res):
-    """The validation log line (rank 0): the mean over levels, then each level's mean loss."""
+def val_line(step, res, logvar=None):
+    """The validation log line (rank 0): the mean over levels, then each level's mean loss; with a learned loss
+    weighting, `logvar` = the EMA's u(sigma_k) at the K validation levels."""
     from maskdit_b200.validate import format_levels
-    return f"(step={step:07d}) Val Loss: {format_levels(res)} ({res['count']} items, EMA)"
+    line = f"(step={step:07d}) Val Loss: {format_levels(res)} ({res['count']} items, EMA)"
+    if logvar is not None:
+        line += ", Logvar: [" + " ".join(f"{float(v):.4f}" for v in logvar) + "]"
+    return line
 
 
 def held_out_set(args, cfg):
@@ -209,7 +219,7 @@ def main():
             print(f"Validation: {len(held)} held-out items x {args.val_levels} noise levels every {args.val_every} "
                   f"steps", flush=True)
     log_every = cfg.log.log_every
-    running, log_steps, t0, step = 0.0, 0, time.time(), step0
+    running, weighted, log_steps, t0, step = 0.0, 0.0, 0, time.time(), step0
     gn_sum = gn_max = None   # the window's gradient norms, accumulated on the device like `running`
     recompute_shown = 0
     for moments, labels in loader:
@@ -219,7 +229,9 @@ def main():
         # moments -> latent (train.py:206), label dropout (:209), noise injection (loss.py:35-39): fused step front
         loss = ts.step(moments, labels, ratio, cfg.model.mae_loss_coef, grad_accum=rounds, moments=True,
                        class_dropout_prob=drop)
-        running = running + loss.mean()
+        running = running + ts.edm_loss.mean()   # the reference's loss; the objective differs with a weighting
+        if net.logvar_channels:
+            weighted = weighted + loss.mean()
         if ts.grad_norm is not None:
             gn = ts.grad_norm
             gn_sum = gn.clone() if gn_sum is None else gn_sum + gn
@@ -235,24 +247,30 @@ def main():
             break
         if step % log_every == 0:
             avg = running / log_steps
+            wavg = weighted / log_steps if net.logvar_channels else None
             if world > 1:
                 dist.all_reduce(avg)
                 avg = avg / world
+                if wavg is not None:
+                    dist.all_reduce(wavg)
+                    wavg = wavg / world
             torch.cuda.synchronize()
             if rank == 0:
                 # every rank takes the same skip decisions, so rank 0's tally is the run's
                 skipped = int(ts.skipped_steps) if ts.skipped_steps is not None else None
                 # every rank computes the same norm from the same summed gradient
                 gnorm = (float(gn_sum) / log_steps, float(gn_max)) if gn_sum is not None else None
-                print(log_line(step, float(avg), log_steps / (time.time() - t0), skipped, gnorm), flush=True)
-            running, log_steps, t0 = 0.0, 0, time.time()
+                print(log_line(step, float(avg), log_steps / (time.time() - t0), skipped, gnorm,
+                               float(wavg) if wavg is not None else None), flush=True)
+            running, weighted, log_steps, t0 = 0.0, 0.0, 0, time.time()
             gn_sum = gn_max = None
         if held is not None and step % args.val_every == 0:
             from maskdit_b200.validate import validate
             # eager, fixed draws from their own generators: the training step's RNG stream and memory plan are untouched
             res = validate(ema, held, levels=args.val_levels, batch=micro_batch)
             if rank == 0:
-                print(val_line(step, res), flush=True)
+                u = ema.logvar(res["sigma"]).tolist() if ema.logvar_channels else None
+                print(val_line(step, res, u), flush=True)
         if step % cfg.log.ckpt_every == 0 and step > step0:
             if rank == 0:
                 d = os.path.join(args.results_dir, "checkpoints")

@@ -18,6 +18,7 @@ import os
 import torch
 
 from maskdit_b200.config import build_net, load_config
+from maskdit_b200.maskdit import eval_state_dict
 from maskdit_b200.validate import HeldOut, format_levels, validate
 
 
@@ -81,7 +82,7 @@ def main(argv=None):
     net = build_net(cfg).to(device).eval()
     rows = []
     for name, sd in sources(args):
-        net.load_state_dict({k.replace("_orig_mod.", ""): v for k, v in sd.items()})
+        net.load_state_dict(eval_state_dict(net, sd))
         res = validate(net, held, levels=args.levels, seed=args.seed, batch=args.batch)
         rows.append({"name": name, "mean": res["mean"], "per_level": res["per_level"]})
         if rank == 0:
