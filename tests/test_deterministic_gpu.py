@@ -14,20 +14,9 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from test_model_gpu import GoldenLoss, load  # noqa: E402
+from support import GoldenLoss, assert_same, det_steps, lib, load, oracle_net, step_state  # noqa: E402,F401
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture
-def lib():
-    """The library; the torch flag, the library setting and the SM budget are restored afterwards."""
-    from maskdit_b200 import _lib
-    L = _lib.lib()
-    det, budget, flag = L.mdt_get_deterministic(), L.mdt_get_sm_budget(), torch.are_deterministic_algorithms_enabled()
-    yield L
-    torch.use_deterministic_algorithms(flag)
-    assert L.mdt_set_deterministic(det) == 0 and L.mdt_set_sm_budget(budget) == 0
 
 
 def _s():
@@ -204,56 +193,6 @@ def test_dgelu_column_sum(lib):
 
 
 # ---- steps -------------------------------------------------------------------------------------------------------------
-_SD = {}
-
-
-def _net(mt, R, ncls, dec):
-    """A fresh training network from a cached oracle state dict (seed 1)."""
-    from maskdit_b200.maskdit import Precond_models
-    from oracle import maskdit_oracle as O
-    key = (mt, R, ncls, dec)
-    if key not in _SD:
-        _SD[key] = O.make_state_dict(O.Cfg(model_type=mt, img_resolution=R, num_classes=ncls, use_decoder=dec), 1)
-    net = Precond_models["edm"](img_resolution=R, img_channels=4, num_classes=ncls, model_type=mt, use_decoder=dec,
-                                mae_loss_coef=0.1, pad_cls_token=False)
-    net.load_state_dict(_SD[key], strict=True)
-    return net.cuda().train()
-
-
-def _state(ts, losses):
-    st = ts.st
-    return [*losses, st.grad.clone(), st.w32.clone(), st.w16.clone(), ts.m.clone(), ts.v.clone(), ts.ema_st.w32.clone()]
-
-
-def _steps(mt, R, ncls, dec, B, mask, n=3, golden=None, seed=0, budget=0, grad_accum=1, **kw):
-    from maskdit_b200 import ops
-    from maskdit_b200.train_step import TrainStep
-    torch.use_deterministic_algorithms(True)
-    net = _net(mt, R, ncls, dec)
-    ts = TrainStep(net, copy.deepcopy(net).eval(), lr=1e-3, loss_fn=GoldenLoss(golden) if golden else None, **kw)
-    gen = torch.Generator().manual_seed(seed)
-    if golden:
-        x, lab = golden["images"].cuda(), (golden["labels"].cuda() if "labels" in golden else None)
-    else:
-        x = (torch.randn(B, 4, R, R, generator=gen) * 0.5).cuda()
-        lab = torch.eye(ncls)[torch.randint(0, ncls, (B,), generator=gen)].cuda() if ncls else None
-    torch.manual_seed(seed)
-    ops.check(ops.lib().mdt_set_sm_budget(budget), "mdt_set_sm_budget", 0)
-    losses = [ts.step(x, lab, mask, 0.1, grad_accum=grad_accum).clone() for _ in range(n)]
-    ops.check(ops.lib().mdt_set_sm_budget(0), "mdt_set_sm_budget", 0)
-    assert ops.lib().mdt_get_deterministic() == 1
-    out = _state(ts, losses)
-    del ts, net
-    torch.cuda.empty_cache()
-    return out
-
-
-def _same(a, b):
-    assert len(a) == len(b)
-    for i, (x, y) in enumerate(zip(a, b)):
-        assert torch.equal(x, y), (i, (x.double() - y.double()).abs().max().item())
-
-
 CASES = {
     "s2_mask50": dict(mt="DiT-S/2", R=8, ncls=10, dec=True, B=2, mask=0.5, golden="s2_train_mask"),
     "s2_nodecoder_uncond_mask30": dict(mt="DiT-S/2", R=32, ncls=0, dec=False, B=3, mask=0.3,
@@ -269,16 +208,16 @@ def test_train_steps_repeat_bit_for_bit(lib, case):
     kw = dict(CASES[case])
     if kw.get("golden"):
         kw["golden"] = load(kw["golden"])
-    _same(_steps(**kw), _steps(**kw))
+    assert_same(det_steps(**kw), det_steps(**kw))
 
 
 def test_graph_replay_and_sm_budget_give_the_same_bits(lib):
     g = load("s2_train_mask")
-    base = _steps("DiT-S/2", 8, 10, True, 2, 0.5, golden=g)
-    _same(base, _steps("DiT-S/2", 8, 10, True, 2, 0.5, golden=g, graph=True))
-    _same(base, _steps("DiT-S/2", 8, 10, True, 2, 0.5, golden=g, budget=66))
-    xl = _steps("DiT-XL/2", 32, 1000, True, 8, 0.5, n=1)
-    _same(xl, _steps("DiT-XL/2", 32, 1000, True, 8, 0.5, n=1, budget=66))
+    base = det_steps("DiT-S/2", 8, 10, True, 2, 0.5, golden=g)
+    assert_same(base, det_steps("DiT-S/2", 8, 10, True, 2, 0.5, golden=g, graph=True))
+    assert_same(base, det_steps("DiT-S/2", 8, 10, True, 2, 0.5, golden=g, budget=66))
+    xl = det_steps("DiT-XL/2", 32, 1000, True, 8, 0.5, n=1)
+    assert_same(xl, det_steps("DiT-XL/2", 32, 1000, True, 8, 0.5, n=1, budget=66))
 
 
 def test_resume_equals_uninterrupted(lib):
@@ -291,13 +230,13 @@ def test_resume_equals_uninterrupted(lib):
     lab = torch.eye(10)[torch.randint(0, 10, (4,), generator=gen)].cuda()
 
     def fresh():
-        net = _net("DiT-S/2", 8, 10, True)
+        net = oracle_net("DiT-S/2", 8, 10, True)
         return net, TrainStep(net, copy.deepcopy(net).eval(), lr=1e-3)
 
     torch.manual_seed(7)
     net, ts = fresh()
     la = [ts.step(x, lab, 0.5, 0.1).clone() for _ in range(4)]
-    a = _state(ts, la)[len(la) + 1:]   # w32, w16, m, v, ema (the gradient buffer is the last step's either way)
+    a = step_state(ts, la)[len(la) + 1:]   # w32, w16, m, v, ema (the gradient buffer is the last step's either way)
     torch.manual_seed(7)
     net, ts = fresh()
     lb = [ts.step(x, lab, 0.5, 0.1).clone() for _ in range(2)]
@@ -308,7 +247,7 @@ def test_resume_equals_uninterrupted(lib):
     torch.cuda.empty_cache()
     buf.seek(0)
     ck = torch.load(buf, weights_only=False)
-    net = _net("DiT-S/2", 8, 10, True)
+    net = oracle_net("DiT-S/2", 8, 10, True)
     net.load_state_dict(ck["model"])
     ema = copy.deepcopy(net).eval()
     ema.load_state_dict(ck["ema"])
@@ -316,15 +255,15 @@ def test_resume_equals_uninterrupted(lib):
     ts2.load_state_dict(ck["opt"])
     torch.cuda.set_rng_state(ck["rng"])
     lb += [ts2.step(x, lab, 0.5, 0.1).clone() for _ in range(2)]
-    _same(la, lb)
-    _same(a, _state(ts2, lb)[len(lb) + 1:])
+    assert_same(la, lb)
+    assert_same(a, step_state(ts2, lb)[len(lb) + 1:])
 
 
 def test_default_and_deterministic_gradients_differ_by_order_noise_only(lib):
     """One XL/2 backward (golden xl2_c1_grads inputs) in both modes: the gradients differ within the order noise the
     default mode's fp32 atomics produce between two of its own runs (DESIGN §5)."""
     g = load("xl2_c1_grads")
-    net = _net("DiT-XL/2", 32, 1000, True)
+    net = oracle_net("DiT-XL/2", 32, 1000, True)
     st = net.prepare()
     grads = []
     for det in (False, True, False):
@@ -352,7 +291,7 @@ def test_default_and_deterministic_gradients_differ_by_order_noise_only(lib):
 def test_sampler_repeats_bit_for_bit(lib):
     from maskdit_b200.sampler import edm_sampler
     torch.use_deterministic_algorithms(True)
-    net = _net("DiT-XL/2", 32, 1000, True).eval()
+    net = oracle_net("DiT-XL/2", 32, 1000, True).eval()
     gen = torch.Generator().manual_seed(9)
     lat = torch.randn(4, 4, 32, 32, generator=gen).cuda()
     lab = torch.eye(1000)[torch.randint(0, 1000, (4,), generator=gen)].cuda()

@@ -6,15 +6,11 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from support import ops  # noqa: F401
+
 pytestmark = pytest.mark.gpu
 
 EPIS = ("store16", "store32_resid", "gelu", "gate_resid", "dgelu", "atomic")
-
-
-@pytest.fixture(scope="module")
-def ops():
-    from maskdit_b200 import ops as o
-    return o
 
 
 def close(got, ref, tol, what=""):

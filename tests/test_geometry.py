@@ -12,7 +12,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 from oracle import maskdit_oracle as O  # noqa: E402
-from test_nodecoder import nd_dit_forward  # noqa: E402
+from support import nd_dit_forward  # noqa: E402
 
 GOLD = os.path.join(ROOT, "tests", "golden")
 
@@ -29,7 +29,7 @@ def cfg(model_type, R, ncls, use_decoder=True):
     return O.Cfg(model_type=model_type, img_resolution=R, num_classes=ncls, use_decoder=use_decoder)
 
 
-# name -> oracle config; the decoder-less ones run test_nodecoder.py's restatement of the forward
+# name -> oracle config; the decoder-less ones run support.nd_dit_forward, the restatement of the forward
 TRAIN = {
     "geo_s8_mask50": cfg("DiT-S/8", 32, 10),
     "geo_b8_nd_nomask": cfg("DiT-B/8", 32, 10, use_decoder=False),

@@ -3,7 +3,7 @@
 at T = 44, and DiT-H/2, whose head_dim 80 runs on the mma.sync attention kernels.  Also the C driver against the
 Python engine, the S/8 eval / CFG / sampler, and two training steps of DiT-S/8 on the C driver.
 
-Bounds: the constants of test_model_gpu.py; for DiT-H/2's 32-block forward, where the reference's own CPU bf16-autocast
+Bounds: the constants of support.py; for DiT-H/2's 32-block forward, where the reference's own CPU bf16-autocast
 output (geo_h2_bf16.npz) is further from its fp32 output, 1.5x that measured distance."""
 import copy
 import os
@@ -15,8 +15,8 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, ROOT)
-from test_model_gpu import (CFG_TOL, EVAL_TOL, FWD_TOL, LOSS_TOL, GoldenLoss, ImplRecorder,  # noqa: E402
-                            check_c_driver_matches_engine, check_grads, load, rel_l2)
+from support import (CFG_TOL, EVAL_TOL, FWD_TOL, LOSS_TOL, GoldenLoss, ImplRecorder,  # noqa: E402
+                     check_c_driver_matches_engine, check_grads, load, rel_l2)
 
 pytestmark = pytest.mark.gpu
 

@@ -14,15 +14,10 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from support import ops  # noqa: E402,F401
 
 pytestmark = pytest.mark.gpu
 f64 = torch.float64
-
-
-@pytest.fixture(scope="module")
-def ops():
-    from maskdit_b200 import ops as o
-    return o
 
 
 def dev():

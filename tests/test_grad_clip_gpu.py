@@ -11,7 +11,6 @@
 5. train.py end to end.
 """
 import copy
-import ctypes
 import gc
 import math
 import os
@@ -21,36 +20,16 @@ import sys
 import pytest
 import torch
 
-pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from support import (CFGS, LR, STEPS, YAML, adamw_inputs, assert_skipped, batches, clean_env, comm,  # noqa: E402,F401
+                     det, f32, live_net, ops, opt_state, poison, rank0_of_two, step_batch, ulp32)
+
+pytestmark = pytest.mark.gpu
 
 bf16 = torch.bfloat16
 NAN, INF = float("nan"), float("inf")
 XL2_TRAINABLE = 730_115_216   # DiT-XL/2 with the decoder: elements of the flat gradient
-
-
-@pytest.fixture(scope="module")
-def ops():
-    from maskdit_b200 import ops as o
-    return o
-
-
-@pytest.fixture
-def det():
-    """Deterministic mode on for the test; the torch flag and the SM budget are restored afterwards."""
-    from maskdit_b200 import _lib
-    flag = torch.are_deterministic_algorithms_enabled()
-    torch.use_deterministic_algorithms(True)
-    yield
-    torch.use_deterministic_algorithms(flag)
-    _lib.sync_deterministic()
-    assert _lib.lib().mdt_set_sm_budget(0) == 0
-
-
-def _ulp32(x64):
-    a = torch.as_tensor(x64, dtype=torch.float64).abs().float()
-    return (torch.nextafter(a, torch.full_like(a, INF)) - a).double()
 
 
 def _norm(ops, g, grad_scale=1.0, flag=None):
@@ -74,7 +53,7 @@ def _ref_norm(g, step=1 << 26):
 
 def _assert_norm(got, ref, what):
     err = abs(got.double().item() - ref)
-    assert err <= _ulp32(ref).item(), (what, got.item(), ref, err / _ulp32(ref).item())
+    assert err <= ulp32(ref).item(), (what, got.item(), ref, err / ulp32(ref).item())
 
 
 def _values(n, seed, lo=-2.0, hi=2.0):
@@ -191,32 +170,26 @@ def test_coefficient_formula_and_overflowing_norm(ops):
 
 
 # ---- 2. AdamW with the coefficient ---------------------------------------------------------------------------------------
-def _dp():
-    import test_dp_step_gpu as dp
-    return dp
-
-
 @pytest.mark.parametrize("guarded", [False, True], ids=["plain", "guarded"])
 @pytest.mark.parametrize("fp32_grad", [False, True], ids=["g16", "g32"])
 def test_coef_one_is_bit_identical(ops, guarded, fp32_grad):
-    dp = _dp()
     n = 1_000_004
-    wd, gs, _, _ = dp.CFGS["wd-half-ema"]
-    w0, ema0, grads = dp._state(n, seed=21)
+    wd, gs, _, _ = CFGS["wd-half-ema"]
+    w0, ema0, grads = adamw_inputs(n, seed=21)
     outs = []
     for use_coef in (False, True):
         s = {"w": w0.cuda(), "m": torch.zeros(n, device="cuda"), "v": torch.zeros(n, device="cuda"),
              "ema": ema0.cuda(), "w16": torch.zeros(n, dtype=bf16, device="cuda")}
         coef = torch.ones(1, device="cuda") if use_coef else None
         flag, counts = torch.zeros(1, device="cuda"), torch.zeros(2, dtype=torch.int64, device="cuda")
-        for step, g in zip(dp.STEPS, grads):
+        for step, g in zip(STEPS, grads):
             g = g.cuda().float() if fp32_grad else g.cuda()
             if guarded:
                 counts[0] = step - 1
-                ops.adamw_ema_guarded(s["w"], g, s["m"], s["v"], s["ema"], s["w16"], n, dp.LR, flag, counts,
+                ops.adamw_ema_guarded(s["w"], g, s["m"], s["v"], s["ema"], s["w16"], n, LR, flag, counts,
                                       weight_decay=wd, grad_scale=gs, max_blocks=3, coef=coef)
             else:
-                ops.adamw_ema(s["w"], g, s["m"], s["v"], s["ema"], s["w16"], n, dp.LR, step, weight_decay=wd,
+                ops.adamw_ema(s["w"], g, s["m"], s["v"], s["ema"], s["w16"], n, LR, step, weight_decay=wd,
                               grad_scale=gs, coef=coef)
         outs.append(s)
     for k in outs[0]:
@@ -228,69 +201,53 @@ def test_coef_one_is_bit_identical(ops, guarded, fp32_grad):
 def test_coef_below_one_vs_float64(ops, guarded, fp32_grad):
     """At the tolerance of the plain kernel's float64 test (test_dp_step_gpu.py::test_adamw_g16_vs_float64)."""
     from oracle import maskdit_oracle as O
-    dp = _dp()
     n = 2_500_004
-    wd, gs, _, _ = dp.CFGS["wd-half-ema"]
-    w0, ema0, grads = dp._state(n, seed=22)
+    wd, gs, _, _ = CFGS["wd-half-ema"]
+    w0, ema0, grads = adamw_inputs(n, seed=22)
     coefs = [0.37, 0.9, 1.0, 0.05, 0.61, 0.2]
     s = {"w": w0.cuda(), "m": torch.zeros(n, device="cuda"), "v": torch.zeros(n, device="cuda"), "ema": ema0.cuda()}
     flag, counts = torch.zeros(1, device="cuda"), torch.zeros(2, dtype=torch.int64, device="cuda")
-    for step, g, c in zip(dp.STEPS, grads, coefs):
+    for step, g, c in zip(STEPS, grads, coefs):
         g = g.cuda().float() if fp32_grad else g.cuda()
         coef = torch.tensor([c], device="cuda")
         if guarded:
             counts[0] = step - 1
-            ops.adamw_ema_guarded(s["w"], g, s["m"], s["v"], s["ema"], None, n, dp.LR, flag, counts,
+            ops.adamw_ema_guarded(s["w"], g, s["m"], s["v"], s["ema"], None, n, LR, flag, counts,
                                   weight_decay=wd, grad_scale=gs, coef=coef)
         else:
-            ops.adamw_ema(s["w"], g, s["m"], s["v"], s["ema"], None, n, dp.LR, step, weight_decay=wd, grad_scale=gs,
+            ops.adamw_ema(s["w"], g, s["m"], s["v"], s["ema"], None, n, LR, step, weight_decay=wd, grad_scale=gs,
                           coef=coef)
     got = {k: t.cpu() for k, t in s.items()}
-    f32 = dp.f32
-    sc = dict(lr=f32(dp.LR), b1=f32(0.9), b2=f32(0.999), eps=f32(1e-8), wd=f32(wd), ema_decay=f32(0.9999))
+    sc = dict(lr=f32(LR), b1=f32(0.9), b2=f32(0.999), eps=f32(1e-8), wd=f32(wd), ema_decay=f32(0.9999))
     w, m, v, e = w0.double(), torch.zeros(n, dtype=torch.float64), torch.zeros(n, dtype=torch.float64), ema0.double()
-    for step, g, c in zip(dp.STEPS, grads, coefs):
+    for step, g, c in zip(STEPS, grads, coefs):
         O.adamw_ema_step(w, g.double() * gs * f32(c), m, v, e, step, **sc)
-    slack = 1e-5 * dp.LR * len(dp.STEPS)
+    slack = 1e-5 * LR * len(STEPS)
     for name, ref in (("w", w), ("ema", e)):
         err = (got[name].double() - ref).abs()
-        assert (err <= 8 * dp._ulp32(ref) + slack).all(), (name, err.max().item())
+        assert (err <= 8 * ulp32(ref) + slack).all(), (name, err.max().item())
     for name, ref in (("m", m), ("v", v)):
         rel = (got[name].double() - ref).abs().max().item() / ref.abs().max().item()
         assert rel <= 1e-5, (name, rel)
 
 
 # ---- 3. the world-1 step -------------------------------------------------------------------------------------------------
-ENV = ("MDT_GRAD_AR", "MDT_COLLECTIVE", "MDT_AR_CHUNKS", "MDT_TRAIN_GRAPH")
-
-
-@pytest.fixture
-def clean_env(monkeypatch):
-    for k in ENV:
-        monkeypatch.delenv(k, raising=False)
-
-
-def _g():
-    import test_nonfinite_guard_gpu as g
-    return g
-
-
 def _trainstep(max_grad_norm, **kw):
     from maskdit_b200.train_step import TrainStep
-    net = _g()._net("S/2")
+    net = live_net("S/2")
     return TrainStep(net, copy.deepcopy(net).eval(), lr=1e-3, weight_decay=0.01, global_batch=4,
                      max_grad_norm=max_grad_norm, **kw)
 
 
 def _state(ts):
-    s = _g()._opt_state(ts)
+    s = opt_state(ts)
     for i, e in enumerate(ts.phema_emas):
         s[f"phema{i}"] = e.clone()
     return s
 
 
 def _run(ts, data, ga=1):
-    losses = [_g()._step(ts, b, ga) for b in data]
+    losses = [step_batch(ts, b, ga) for b in data]
     torch.cuda.synchronize()
     return losses
 
@@ -302,7 +259,7 @@ def _free():
 
 @pytest.mark.parametrize("guard", [False, True], ids=["plain", "guard"])
 def test_world1_inf_and_loose_bound_change_nothing(det, clean_env, guard):
-    data = _g()._batches("S/2", 3)
+    data = batches("S/2", 3)
     kw = dict(skip_nonfinite=guard, phema_sigma_rels=(0.05, 0.10))
     ts = _trainstep(None, **kw)
     loss_off = _run(ts, data)
@@ -330,9 +287,7 @@ def test_world1_inf_and_loose_bound_change_nothing(det, clean_env, guard):
 def test_world1_clipped_step_equals_torch(clean_env, ga):
     """A bound below the norm: `grad_norm` is clip_grad_norm_'s total norm of the p.grad views (x 1/grad_accum), and
     weights and moments equal torch.optim.AdamW after clip_grad_norm_ on a float64 copy."""
-    dp = _dp()
-    f32 = dp.f32
-    data = _g()._batches("S/2", 1)
+    data = batches("S/2", 1)
     ts = _trainstep(1e-3)
     n = ts.st.n_train
     params = [(k, p) for k, p in ts.net.named_parameters() if p.requires_grad]
@@ -355,7 +310,7 @@ def test_world1_clipped_step_equals_torch(clean_env, ga):
                            ("m", ts.m[lo:lo + cnt], st["exp_avg"].reshape(-1)),
                            ("v", ts.v[lo:lo + cnt], st["exp_avg_sq"].reshape(-1))):
             err = (a.double() - b).abs()
-            bound = 8 * dp._ulp32(b) + (1e-5 * ts.lr if name == "w" else 1e-5 * b.abs().max().item())
+            bound = 8 * ulp32(b) + (1e-5 * ts.lr if name == "w" else 1e-5 * b.abs().max().item())
             worst[name] = max(worst.get(name, 0.0), (err / bound).max().item())
             assert (err <= bound).all(), (ga, k, name, err.max().item())
     print(f"grad_accum {ga}: norm {got:.6g} clipped to {ts.max_grad_norm}; worst error / bound {worst}")
@@ -364,14 +319,14 @@ def test_world1_clipped_step_equals_torch(clean_env, ga):
 
 
 def test_world1_guard_skips_a_nonfinite_step(clean_env):
-    data = _g()._batches("S/2", 3)
+    data = batches("S/2", 3)
     ts = _trainstep(0.5, skip_nonfinite=True)
     _run(ts, data[:1])
     assert math.isfinite(ts.grad_norm.item()) and ts._counts.tolist() == [1, 0]
-    before = _g()._opt_state(ts)
-    _run(ts, [_g()._poison(data[1])])
+    before = opt_state(ts)
+    _run(ts, [poison(data[1])])
     assert not math.isfinite(ts.grad_norm.item()) and int(ts.skipped_steps) == 1
-    _g()._assert_skip(before, _g()._opt_state(ts), ts.ema_decay)
+    assert_skipped(before, opt_state(ts), ts.ema_decay)
     _run(ts, data[2:])
     assert math.isfinite(ts.grad_norm.item()) and ts._counts.tolist() == [2, 1]
     del ts
@@ -381,7 +336,7 @@ def test_world1_guard_skips_a_nonfinite_step(clean_env):
 def test_added_calls_do_not_synchronise(clean_env):
     """The norm pass, the coefficient and the coefficient-reading optimizer pass under sync debug mode 'error'."""
     from maskdit_b200 import ops
-    data = _g()._batches("S/2", 2)
+    data = batches("S/2", 2)
     for guard in (False, True):
         ts = _trainstep(0.5, skip_nonfinite=guard)
         _run(ts, data[:1])
@@ -399,60 +354,21 @@ def test_added_calls_do_not_synchronise(clean_env):
 
 
 # ---- 4. rank 0 of two emulated ranks ----------------------------------------------------------------------------------------
-class TwoIdenticalRanks:
-    """`GradComm` stand-in on rank 0 of two ranks holding the same gradient: the real one-rank `mdt_allreduce_grads`,
-    then the buffer doubled (the exact two-rank sum).  The guard's flag word is summed with a clear peer flag."""
-
-    def __init__(self, ts, comm, log):
-        self.ts, self.comm, self.log = ts, comm, log
-
-    def all_reduce(self, t):
-        from maskdit_b200 import ops
-        self.log.append(ops.lib().mdt_allreduce_grads(self.comm, t.data_ptr(), t.numel(), int(t.dtype == bf16),
-                                                      ops.stream_ptr()))
-        if self.ts._flag is None or t.data_ptr() != self.ts._flag.data_ptr():
-            t.mul_(2)
-
-    def close(self):
-        pass
-
-
-def make_rank0_of_two(ts, comm, log, ar_chunks):
-    ts.world = 2
-    ts.comm = TwoIdenticalRanks(ts, comm, log)
-    if ts.grad_dtype == "bf16":
-        ts.g16 = torch.empty(ts.st.n_train, dtype=bf16, device="cuda")
-    ts.ar_chunks = ar_chunks
-
-
-@pytest.fixture(scope="module")
-def comm(ops):
-    L = ops.lib()
-    uid = ctypes.create_string_buffer(128)
-    assert L.mdt_nccl_unique_id(uid) == 0
-    c = ctypes.c_void_p()
-    assert L.mdt_nccl_comm_create(bytes(uid.raw), 0, 1, 0, ctypes.byref(c)) == 0 and c.value
-    yield c
-    assert L.mdt_nccl_comm_destroy(c) == 0
-
-
-def _world2(max_grad_norm, grad_dtype, chunks, comm, log, **kw):
+def _world2(max_grad_norm, grad_dtype, chunks, rank0_of_two, **kw):
     ts = _trainstep(max_grad_norm, grad_dtype=grad_dtype, **kw)
     ts.global_batch = 8
-    make_rank0_of_two(ts, comm, log, chunks)
-    return ts
+    return rank0_of_two(ts, chunks)
 
 
 WORLD2 = [("bf16", 1), ("bf16", 4), ("fp32", 1), ("fp32", 4)]
 
 
 @pytest.mark.parametrize("grad_dtype,chunks", WORLD2, ids=[f"{d}-{c}" for d, c in WORLD2])
-def test_world2_inf_changes_nothing(det, clean_env, comm, grad_dtype, chunks):
-    data = _g()._batches("S/2", 2)
-    log = []
+def test_world2_inf_changes_nothing(det, clean_env, rank0_of_two, grad_dtype, chunks):
+    data = batches("S/2", 2)
     states = []
     for c in (None, INF):
-        ts = _world2(c, grad_dtype, chunks, comm, log, skip_nonfinite=True)
+        ts = _world2(c, grad_dtype, chunks, rank0_of_two, skip_nonfinite=True)
         _run(ts, data)
         states.append(_state(ts))
         if c is not None:
@@ -462,18 +378,16 @@ def test_world2_inf_changes_nothing(det, clean_env, comm, grad_dtype, chunks):
         _free()
     for k in states[0]:
         assert torch.equal(states[0][k], states[1][k]), (grad_dtype, chunks, k)
-    assert log and all(rc == 0 for rc in log), log
 
 
 @pytest.mark.parametrize("ga", [1, 2])
 @pytest.mark.parametrize("grad_dtype,chunks", WORLD2, ids=[f"{d}-{c}" for d, c in WORLD2])
-def test_world2_every_chunk_uses_the_final_coefficient(clean_env, comm, ops, grad_dtype, chunks, ga):
+def test_world2_every_chunk_uses_the_final_coefficient(clean_env, rank0_of_two, ops, grad_dtype, chunks, ga):
     """The norm is the float64 norm of the summed buffer x 1/(2 grad_accum), and one AdamW pass over the whole summed
     buffer with that step's coefficient reproduces every chunk's update bit for bit: a pass that ran before the last
     chunk's norm was known would have read the previous step's coefficient (0 before the first step)."""
-    data = _g()._batches("S/2", 3)
-    log = []
-    ts = _world2(1e-3, grad_dtype, chunks, comm, log)
+    data = batches("S/2", 3)
+    ts = _world2(1e-3, grad_dtype, chunks, rank0_of_two)
     n = ts.st.n_train
     coefs = []
     for step, b in enumerate(data, 1):
@@ -494,7 +408,6 @@ def test_world2_every_chunk_uses_the_final_coefficient(clean_env, comm, ops, gra
                                ("ema", ts.ema_st.w32[:n], pre["ema"]), ("w16", ts.st.w16[:n], w16)):
             assert torch.equal(got, exp), (grad_dtype, chunks, ga, step, name)
     assert len(set(coefs)) == len(coefs), coefs
-    assert log and all(rc == 0 for rc in log), log
     del ts
     _free()
 
@@ -505,12 +418,12 @@ LINE = re.compile(r"^\(step=\d{7}\) Train Loss: -?\d+\.\d{4}, Train Steps/Sec: \
 
 
 @pytest.mark.parametrize("bound", [None, "1.0", "inf"])
-def test_train_py_logs_the_norm(tmp_path, monkeypatch, capsys, bound):
+def test_train_py_logs_the_norm(tmp_path, monkeypatch, clean_env, capsys, bound):
     import train
-    for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK", *ENV):
+    for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
         monkeypatch.delenv(k, raising=False)
     cfg = tmp_path / "cfg.yaml"
-    cfg.write_text(_g().YAML.replace("max_num_steps: 4", "max_num_steps: 6").replace("ckpt_every: 4", "ckpt_every: 6"))
+    cfg.write_text(YAML.replace("max_num_steps: 4", "max_num_steps: 6").replace("ckpt_every: 4", "ckpt_every: 6"))
     argv = ["train.py", "--config", str(cfg), "--synthetic", "--max_steps", "6", "--results_dir", str(tmp_path / "r")]
     monkeypatch.setattr(sys, "argv", argv + (["--max_grad_norm", bound] if bound else []))
     train.main()

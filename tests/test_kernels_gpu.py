@@ -9,14 +9,10 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from support import ops  # noqa: F401
+
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
-
-
-@pytest.fixture(scope="module")
-def ops():
-    from maskdit_b200 import ops as o
-    return o
 
 
 def dev():

@@ -21,23 +21,12 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from support import det  # noqa: E402,F401
 
 pytestmark = pytest.mark.gpu
 
 C_LV, R, NCLS = 128, 8, 10
 _SD = {}
-
-
-@pytest.fixture
-def det():
-    """Deterministic mode for the test; the torch flag and the library setting are restored afterwards."""
-    from maskdit_b200 import _lib
-    L = _lib.lib()
-    was, flag = L.mdt_get_deterministic(), torch.are_deterministic_algorithms_enabled()
-    torch.use_deterministic_algorithms(True)
-    yield
-    torch.use_deterministic_algorithms(flag)
-    assert L.mdt_set_deterministic(was) == 0
 
 
 def _net(C=0, dec=True, w_scale=0.0, seed=3):
@@ -273,7 +262,7 @@ def test_weighted_gradient_is_a_combination_of_unweighted_runs(det, monkeypatch,
     for k, g in g_on.items():
         want = parts[0][k] + parts[1][k] - parts[2][k]
         # The MAE part is the difference of two runs, each with its own bf16 rounding of the seed: the bound is
-        # GRAD_TOL of tests/test_model_gpu.py (rel-L2 1.5e-2) relative to the parts' norms, not to their sum.
+        # GRAD_TOL of tests/support.py (rel-L2 1.5e-2) relative to the parts' norms, not to their sum.
         scale = sum(parts[i][k].norm() for i in range(3))
         if scale == 0:
             assert g.norm() == 0, k

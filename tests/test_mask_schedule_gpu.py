@@ -22,8 +22,8 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from test_deterministic_gpu import _net, _same, _state  # noqa: E402
-from test_model_gpu import FWD_TOL, GRAD_TOL, LOSS_TOL, GoldenLoss, ImplRecorder, rel_l2  # noqa: E402
+from support import (FWD_TOL, GRAD_TOL, LOSS_TOL, GoldenLoss, ImplRecorder, assert_same, lib,  # noqa: E402,F401
+                     oracle_net, ops, rel_l2, step_state)
 
 pytestmark = pytest.mark.gpu
 f64 = torch.float64
@@ -32,23 +32,6 @@ f64 = torch.float64
 MT, R, NCLS, B = "DiT-S/2", 32, 10, 2
 L = (R // 2) ** 2
 R_FULL = 1e-17   # a ratio the schedule reaches in its last steps: masking on, int(L * (1 - r)) == L
-
-
-@pytest.fixture
-def lib():
-    """The library; the torch flag, the library setting and the SM budget are restored afterwards."""
-    from maskdit_b200 import _lib
-    Lb = _lib.lib()
-    det, budget, flag = Lb.mdt_get_deterministic(), Lb.mdt_get_sm_budget(), torch.are_deterministic_algorithms_enabled()
-    yield Lb
-    torch.use_deterministic_algorithms(flag)
-    assert Lb.mdt_set_deterministic(det) == 0 and Lb.mdt_set_sm_budget(budget) == 0
-
-
-@pytest.fixture(scope="module")
-def ops():
-    from maskdit_b200 import ops as o
-    return o
 
 
 def dev():
@@ -244,7 +227,7 @@ def test_driver_step_at_schedule_T_vs_float64_oracle(lib, T):
     torch.use_deterministic_algorithms(False)
     g = draws(200 + T)
     r = ratio(T)
-    net = _net(MT, R, NCLS, True)
+    net = oracle_net(MT, R, NCLS, True)
     lf = GoldenLoss(g)
     x, lab = g["images"].cuda(), g["labels"].cuda()
     with ImplRecorder() as rec:
@@ -310,19 +293,19 @@ def test_T_changing_run_repeats_bit_for_bit(lib):
     runs = {}
     for name, kw in (("eager", {}), ("graph", dict(graph=True)), ("recompute 1", dict(recompute_blocks=1)),
                      ("recompute all", dict(recompute_blocks=20))):
-        net = _net(MT, R, NCLS, True)
+        net = oracle_net(MT, R, NCLS, True)
         runs[name] = TrainStep(net, copy.deepcopy(net).eval(), lr=1e-3, loss_fn=GoldenLoss(g), **kw)
     graphs = runs["graph"]._graphs
     for i, T in enumerate(T_SEQ):
         base = None
         for name, ts in runs.items():
-            st = _state(ts, [ts.step(x, lab, ratio(T), 0.1).clone()])
+            st = step_state(ts, [ts.step(x, lab, ratio(T), 0.1).clone()])
             if base is None:
                 base = st
                 assert torch.isfinite(st[0]).all()
                 continue
             try:
-                _same(base, st)
+                assert_same(base, st)
             except AssertionError as e:
                 raise AssertionError(f"step {i} (T = {T}): {name} differs from eager: {e}") from None
             del st

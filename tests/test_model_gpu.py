@@ -13,155 +13,10 @@ import numpy as np
 import pytest
 import torch
 
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from support import CFG_TOL, EVAL_TOL, FWD_TOL, LOSS_TOL, GoldenLoss, build, check_grads, load, rel_l2  # noqa: E402
+
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-GOLD = os.path.join(ROOT, "tests", "golden")
-
-
-def load(name):
-    return {k: (torch.from_numpy(np.asarray(v)) if v.dtype.kind in "fiub" else v)
-            for k, v in np.load(os.path.join(GOLD, name + ".npz")).items()}
-
-
-def rel_l2(a, b):
-    a, b = a.double().flatten().cpu(), b.double().flatten().cpu()
-    return ((a - b).norm() / (b.norm() + 1e-30)).item()
-
-
-def build(model_type="DiT-S/2", R=8, ncls=10, seed=1):
-    from maskdit_b200.maskdit import Precond_models
-    from oracle import maskdit_oracle as O
-    cfg = O.Cfg(model_type=model_type, img_resolution=R, num_classes=ncls)
-    net = Precond_models["edm"](img_resolution=R, img_channels=4, num_classes=ncls, model_type=model_type,
-                                use_decoder=True, mae_loss_coef=0.1, pad_cls_token=False)
-    sd = O.make_state_dict(cfg, seed)
-    net.load_state_dict(sd, strict=True)
-    return net.cuda(), cfg, sd
-
-
-FWD_TOL, GRAD_TOL, LOSS_TOL = 3e-3, 1.5e-2, 5e-3   # rel-L2 outputs / rel-L2 gradients / relative loss
-EVAL_TOL, CFG_TOL = 6e-3, 1e-2   # unmasked eval forward / CFG-combined output (see the yardstick in DESIGN.md §5)
-
-
-def check_grads(net, g, tol=GRAD_TOL, what=""):
-    """Every parameter-gradient norm, the stored full gradients and the stored 4x8 slices against the reference's."""
-    worst, n = (0.0, ""), 0
-    for k, p in net.named_parameters():
-        key = f"gnorm/{k}"
-        if key not in g:
-            continue
-        gn, ref = p.grad.double().norm().item(), float(g[key])
-        assert abs(gn - ref) <= tol * ref + 1e-7, (k, gn, ref)
-        n += 1
-        if f"grad/{k}" in g and ref > 0:
-            r = rel_l2(p.grad, g[f"grad/{k}"])
-            worst = max(worst, (r, k))
-            assert r <= tol, (k, r)
-        if f"gslice/{k}" in g and ref > 0:
-            sl = p.grad.reshape(p.grad.shape[0], -1)[:4, :8]
-            want = g[f"gslice/{k}"]
-            # a 32-element slice: compare against the scale of the whole tensor (rms), bf16 backward noise
-            rms = ref / max(p.grad.numel(), 1) ** 0.5
-            assert (sl.cpu().double() - want.double()).abs().max().item() <= 8 * tol * rms + 1e-9, k
-    assert n > 100
-    print(what, "worst grad rel-L2", worst, "over", n, "tensors")
-
-
-def check_c_driver_matches_engine(net, x, sigma, lab, md, what="", dF_same_grads=None):
-    """The C++ step driver (`mdt_forward` / `mdt_backward`: one ctypes call each, one workspace) of the training-mode
-    `net` against the kernel-by-kernel Python `Engine` on the same flat store.  The forward agrees BIT FOR BIT, with and
-    without saved activations: same kernels, same order, same operands.  The backward accumulates wgrads with fp32
-    atomics (run-to-run order noise), so the gradients of a random dF agree to 5e-5 of each tensor's scale (1e-2 on the
-    conditioning path, see below).  `dF_same_grads(dF)`, when given, is a second dF for which the driver must give the
-    same gradients.  Returns the driver, its context of the saving forward and its F."""
-    from maskdit_b200.engine import CEngine, Engine
-    st = net.prepare()
-    ce, pe = net._engine, Engine(net._cfg(), st)
-    assert isinstance(ce, CEngine)
-    for save in (False, True):
-        Fc, ctx_c = ce.forward(x, sigma, lab, md, save)
-        Fp, ctx_p = pe.forward(x, sigma, lab, md, save)
-        assert torch.equal(Fc, Fp), (save, (Fc - Fp).abs().max())
-    dF = (torch.randn_like(Fc) * 0.1).to(torch.bfloat16)
-
-    def grads(engine, ctx, dF_):
-        st.ensure_grad().zero_()
-        engine.backward(ctx, dF_)
-        return st.grad.clone()
-
-    got = [grads(ce, ctx_c, dF)]
-    gp = grads(pe, ctx_p, dF)
-    if dF_same_grads is not None:
-        got.append(grads(ce, ctx_c, dF_same_grads(dF)))
-    worst = 0.0
-    for k, (o, n, _) in st.offsets.items():
-        if o + n > st.n_train:
-            continue
-        b = gp[o:o + n]
-        scale = b.abs().max().item() + 1e-30
-        # Order noise of the fp32 atomics: 1e-7 .. 1e-5 on the block tensors.  On the conditioning path the noisy sums
-        # are re-rounded to bf16 several times before GEMMs that contract over only B = 2 rows (dmod -> bf16 -> adaLN
-        # wgrad; dsc -> dc (bf16) -> dth -> dpre (bf16) -> t_embedder wgrad): one flipped bf16 rounding moves an element
-        # by 2^-8, measured up to 2e-3 of a tensor's scale between two runs of the SAME engine - not a code difference.
-        cond = any(t in k for t in ("adaLN_modulation", "t_embedder", "y_embedder"))
-        for g in got:
-            err = (g[o:o + n] - b).abs().max().item() / scale
-            worst = max(worst, err)
-            assert err <= (1e-2 if cond else 5e-5), (k, err)
-    print(what, "C driver vs Python engine: forward bit-equal, worst gradient deviation", worst)
-    return ce, ctx_c, Fc
-
-
-class ImplRecorder:
-    """Which GEMM instances (BLOCK_N*10 + CTAs per tile) and which attention kernel families served the calls made
-    inside the `with` block — read from the library's own logs (mdt_gemm_configs_seen / mdt_attention_impl_log), so the
-    C++ step driver's internal launches are covered as well as per-kernel calls from Python."""
-
-    def __enter__(self):
-        from maskdit_b200 import ops
-        self.L = ops.lib()
-        self.L.mdt_gemm_configs_seen(1)
-        self.L.mdt_attention_impl_log(None, 0)
-        self.gemm_cfgs, self.attn_fwd, self.attn_bwd = set(), set(), set()
-        return self
-
-    def __exit__(self, *exc):
-        import ctypes
-        bits = self.L.mdt_gemm_configs_seen(1)
-        names = [1281, 1282, 1921, 1922, 2561, 2562]
-        self.gemm_cfgs = {names[i] for i in range(6) if bits >> i & 1}
-        buf = (ctypes.c_int * 4096)()
-        n = self.L.mdt_attention_impl_log(buf, 1024)
-        for i in range(n):
-            which, T, dh, impl = buf[4 * i:4 * i + 4]
-            (self.attn_bwd if which else self.attn_fwd).add((T, dh, impl))
-
-
-class GoldenLoss:
-    """EDMLoss with the golden random draws injected in the reference's draw order."""
-
-    def __new__(cls, g):
-        from maskdit_b200.loss import EDMLoss
-
-        class _L(EDMLoss):
-            def __init__(self):
-                super().__init__()
-                self.q_randn = [g["rnd_normal"].cuda(), g["noise_unit"].cuda()]
-                self.q_rand = [g["mask_noise"].cuda()] if "mask_noise" in g else []
-
-                self.n_randn = 0
-
-            def _randn(self, shape, device):   # draws cycle (sigma, noise, sigma, noise, ...): reusable across steps
-                t = self.q_randn[self.n_randn % 2]
-                self.n_randn += 1
-                assert tuple(t.shape) == tuple(shape)
-                return t
-
-            def _rand(self, shape, device):
-                return self.q_rand[0]
-
-        return _L()
 
 
 @pytest.mark.parametrize("name", ["s2_train_mask", "s2_train_nomask"])

@@ -8,8 +8,8 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from test_model_gpu import (CFG_TOL, EVAL_TOL, FWD_TOL, GRAD_TOL, LOSS_TOL, GoldenLoss, ImplRecorder, build,  # noqa: E402
-                            check_c_driver_matches_engine, check_grads, load, rel_l2)
+from support import (CFG_TOL, EVAL_TOL, FWD_TOL, GRAD_TOL, LOSS_TOL, GoldenLoss, ImplRecorder, build,  # noqa: E402
+                     check_c_driver_matches_engine, check_grads, load, rel_l2)
 
 pytestmark = pytest.mark.gpu
 

@@ -1,5 +1,5 @@
 """CPU tests of the decoder-less DiT (use_decoder=False, the reference's default, models/maskdit.py:254): a CPU fp32
-restatement of its forward against the unmodified reference (tests/golden/make_golden_nodecoder.py), the module's
+restatement of its forward (support.nd_dit_forward) against the unmodified reference (tests/golden/make_golden_nodecoder.py), the module's
 state-dict contract and the C driver's model-config validation."""
 import ctypes
 import os
@@ -8,11 +8,11 @@ import sys
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from oracle import maskdit_oracle as O  # noqa: E402
+from support import nd_dit_forward  # noqa: E402
 
 GOLD = os.path.join(ROOT, "tests", "golden")
 
@@ -27,35 +27,6 @@ def load(name):
 
 def t(a):
     return torch.from_numpy(np.asarray(a))
-
-
-def nd_dit_forward(sd, cfg, x, t, y, mask_dict=None, training=True):
-    """DiT.forward without the decoder (models/maskdit.py:511-557 with use_decoder=False), built from the oracle's
-    pieces: embedding + mask_out_token, the encoder blocks, FinalLayer on the encoder width, and for masked training
-    the kept rows scattered into zeros (:551-553).  The decoder model is left to `maskdit_oracle.dit_forward`."""
-    assert not cfg.use_decoder
-    D, P, B = cfg.hidden, cfg.patch, x.shape[0]
-    patches = x.reshape(B, cfg.img_channels, cfg.grid, P, cfg.grid, P).permute(0, 2, 4, 1, 3, 5).reshape(
-        B, cfg.num_patches, -1)
-    h = F.linear(patches, sd["model.x_embedder.proj.weight"].reshape(D, -1), sd["model.x_embedder.proj.bias"]) + \
-        sd["model.pos_embed"]
-    masked = mask_dict is not None and training
-    if masked:
-        h = torch.gather(h, 1, mask_dict["ids_keep"].unsqueeze(-1).expand(-1, -1, D))
-    te = F.linear(O.timestep_embedding(t, 256), sd["model.t_embedder.mlp.0.weight"], sd["model.t_embedder.mlp.0.bias"])
-    c = F.linear(F.silu(te), sd["model.t_embedder.mlp.2.weight"], sd["model.t_embedder.mlp.2.bias"])
-    if cfg.num_classes:
-        c = c + F.linear(y, sd["model.y_embedder.embedding_table.weight"])
-    for i in range(cfg.depth):
-        h = O._block(sd, f"model.blocks.{i}", h, c, cfg.heads)
-    sh, sc = F.linear(F.silu(c), sd["model.final_layer.adaLN_modulation.1.weight"],
-                      sd["model.final_layer.adaLN_modulation.1.bias"]).chunk(2, dim=1)
-    out = F.linear(O._modulate(O._ln(h), sh, sc), sd["model.final_layer.linear.weight"],
-                   sd["model.final_layer.linear.bias"])
-    if masked:
-        full = out.new_zeros(B, cfg.num_patches, out.shape[-1])
-        out = full.scatter(1, mask_dict["ids_keep"].unsqueeze(-1).expand(-1, -1, out.shape[-1]), out)
-    return O.unpatchify(out, P, cfg.img_channels)
 
 
 @pytest.fixture

@@ -2,7 +2,7 @@
 (tests/golden/make_golden_nodecoder.py), the C driver against the Python engine, the zero-filled output scatter, the
 eval CUDA graph, the optimizer-state layout and the train.py / generate.py entry points.
 
-Bounds: the existing constants of test_model_gpu.py; where the reference's own CPU bf16-autocast output of the same
+Bounds: the existing constants of support.py; where the reference's own CPU bf16-autocast output of the same
 XL/2 forward (nd_xl2_bf16.npz) is further from its fp32 output, 1.5x that measured distance."""
 import copy
 import io
@@ -17,8 +17,8 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 sys.path.insert(0, ROOT)
-from test_model_gpu import (CFG_TOL, EVAL_TOL, FWD_TOL, LOSS_TOL, GoldenLoss, ImplRecorder,  # noqa: E402
-                            check_c_driver_matches_engine, check_grads, load, rel_l2)
+from support import (CFG_TOL, EVAL_TOL, FWD_TOL, LOSS_TOL, GoldenLoss, ImplRecorder,  # noqa: E402
+                     check_c_driver_matches_engine, check_grads, load, rel_l2)
 
 pytestmark = pytest.mark.gpu
 

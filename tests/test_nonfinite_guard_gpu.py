@@ -9,7 +9,6 @@
 6. train.py end to end with a loader that yields one NaN batch, with and without --no_amp.
 """
 import copy
-import ctypes
 import gc
 import io
 import os
@@ -19,30 +18,16 @@ import sys
 import pytest
 import torch
 
-pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from support import (CFGS, LR, MODELS, STEPS, YAML, adamw_inputs, assert_skipped, batches,  # noqa: E402,F401
+                     clean_env, comm, det, f32, live_net, ops, opt_state, poison, rank0_of_two, run_adamw,
+                     step_batch, ulp32)
+
+pytestmark = pytest.mark.gpu
 
 bf16 = torch.bfloat16
 NAN, INF = float("nan"), float("inf")
-
-
-@pytest.fixture(scope="module")
-def ops():
-    from maskdit_b200 import ops as o
-    return o
-
-
-@pytest.fixture
-def det():
-    """Deterministic mode on for the test; the torch flag and the SM budget are restored afterwards."""
-    from maskdit_b200 import _lib
-    flag = torch.are_deterministic_algorithms_enabled()
-    torch.use_deterministic_algorithms(True)
-    yield
-    torch.use_deterministic_algorithms(flag)
-    _lib.sync_deterministic()
-    assert _lib.lib().mdt_set_sm_budget(0) == 0
 
 
 def _flag():
@@ -158,29 +143,22 @@ def test_check_at_xl2_size(ops):
 
 
 # ---- 2. guarded AdamW ------------------------------------------------------------------------------------------------------
-def _dp():
-    import test_dp_step_gpu as dp
-    return dp
-
-
 @pytest.mark.parametrize("fp32_grad", [False, True])
 @pytest.mark.parametrize("max_blocks", [0, 3])
 @pytest.mark.parametrize("cfg", ["wd0-half-ema-w16", "wd-16th-w16", "wd-half-ema", "wd0-16th-bare"])
 def test_guarded_adamw_flag_clear_is_bit_identical(ops, cfg, max_blocks, fp32_grad):
-    dp = _dp()
     n = 1_000_004
-    wd, gs, with_ema, with_w16 = dp.CFGS[cfg]
-    w0, ema0, grads = dp._state(n, seed=11)
-    ref = dp._run_kernel(ops, w0, ema0, grads, wd, gs, with_ema, with_w16, max_blocks=max_blocks,
-                         fp32_grad=fp32_grad)
+    wd, gs, with_ema, with_w16 = CFGS[cfg]
+    w0, ema0, grads = adamw_inputs(n, seed=11)
+    ref = run_adamw(ops, w0, ema0, grads, wd, gs, with_ema, with_w16, max_blocks=max_blocks, fp32_grad=fp32_grad)
     out = {"w": w0.cuda(), "m": torch.zeros(n, device="cuda"), "v": torch.zeros(n, device="cuda"),
            "ema": ema0.cuda() if with_ema else None,
            "w16": torch.zeros(n, dtype=bf16, device="cuda") if with_w16 else None}
     flag, counts = _flag(), torch.zeros(2, dtype=torch.int64, device="cuda")
-    for step, g in zip(dp.STEPS, grads):
+    for step, g in zip(STEPS, grads):
         g = g.cuda().float() if fp32_grad else g.cuda()
         counts[0] = step - 1
-        ops.adamw_ema_guarded(out["w"], g, out["m"], out["v"], out["ema"], out["w16"], n, dp.LR, flag, counts,
+        ops.adamw_ema_guarded(out["w"], g, out["m"], out["v"], out["ema"], out["w16"], n, LR, flag, counts,
                               weight_decay=wd, grad_scale=gs, max_blocks=max_blocks)
         ops.optim_guard_advance(flag, counts)
         assert counts.tolist() == [step, 0]
@@ -191,7 +169,6 @@ def test_guarded_adamw_flag_clear_is_bit_identical(ops, cfg, max_blocks, fp32_gr
 
 @pytest.mark.parametrize("fp32_grad", [False, True])
 def test_guarded_adamw_flag_set_moves_only_the_ema(ops, fp32_grad):
-    dp = _dp()
     n = 1_000_004
     gen = torch.Generator().manual_seed(3)
     w = torch.randn(n, generator=gen).cuda()
@@ -205,83 +182,20 @@ def test_guarded_adamw_flag_set_moves_only_the_ema(ops, fp32_grad):
     state = dict(w=w, m=m, v=v, w16=w16, counts=counts)
     before = {k: t.clone() for k, t in state.items()}
     before["ema"] = ema.clone()
-    ops.adamw_ema_guarded(w, g, m, v, ema, w16, n, dp.LR, flag, counts, weight_decay=0.03, grad_scale=0.5,
+    ops.adamw_ema_guarded(w, g, m, v, ema, w16, n, LR, flag, counts, weight_decay=0.03, grad_scale=0.5,
                           max_blocks=3)
     torch.cuda.synchronize()
     for k, t in state.items():
         assert torch.equal(t, before[k]), k
-    d = dp.f32(0.9999)
+    d = f32(0.9999)
     want = d * before["ema"].double() + (1 - d) * before["w"].double()
     err = (ema.double() - want).abs()
-    assert (err <= dp._ulp32(want)).all(), err.max().item()
+    assert (err <= ulp32(want)).all(), err.max().item()
     ops.optim_guard_advance(flag, counts)
     assert counts.tolist() == [7, 3]
 
 
-# ---- the emulated second rank ----------------------------------------------------------------------------------------------
-class Peer:
-    """What the other rank contributes to the summed flag word."""
-
-    def __init__(self, flag=0.0):
-        self.flag = flag
-
-
-class RankZeroOfTwo:
-    """`GradComm` stand-in on rank 0 of two ranks: runs the real one-rank `mdt_allreduce_grads`, then adds the other
-    rank's contribution (the same gradient, or the peer's flag word).  Records the statuses for the fixture to check."""
-
-    def __init__(self, ts, comm, peer, log):
-        self.ts, self.comm, self.peer, self.log = ts, comm, peer, log
-
-    def all_reduce(self, t):
-        from maskdit_b200 import ops
-        L = ops.lib()
-        self.log.append(L.mdt_allreduce_grads(self.comm, t.data_ptr(), t.numel(), int(t.dtype == bf16),
-                                              ops.stream_ptr()))
-        if t.data_ptr() == self.ts._flag.data_ptr():
-            t.add_(self.peer.flag)
-            return
-        t.mul_(2)
-
-    def close(self):
-        pass
-
-
-@pytest.fixture(scope="module")
-def comm(ops):
-    """A one-rank communicator."""
-    L = ops.lib()
-    uid = ctypes.create_string_buffer(128)
-    assert L.mdt_nccl_unique_id(uid) == 0
-    c = ctypes.c_void_p()
-    assert L.mdt_nccl_comm_create(bytes(uid.raw), 0, 1, 0, ctypes.byref(c)) == 0 and c.value
-    yield c
-    assert L.mdt_nccl_comm_destroy(c) == 0
-
-
-@pytest.fixture
-def rank0_of_two(comm):
-    """make(ts, peer, ar_chunks): turn a world-1 TrainStep into rank 0 of a two-rank job; the statuses are checked at
-    the end."""
-    logs = []
-
-    def make(ts, peer, ar_chunks):
-        log = []
-        logs.append(log)
-        ts.world = 2
-        ts.comm = RankZeroOfTwo(ts, comm, peer, log)
-        if ts.grad_dtype == "bf16":
-            ts.g16 = torch.empty(ts.st.n_train, dtype=bf16, device="cuda")
-        ts.ar_chunks = ar_chunks
-        return ts
-
-    yield make
-    for log in logs:
-        assert all(rc == 0 for rc in log), log
-
-
 # ---- 3. exact skip -----------------------------------------------------------------------------------------------------------
-MODELS = {"S/2": ("DiT-S/2", 32, 1000, 4), "XL/2": ("DiT-XL/2", 32, 1000, 8)}
 MODES = {
     "world1": dict(),
     "graph": dict(graph=True),
@@ -290,101 +204,36 @@ MODES = {
     "fp32-one-chunk": dict(world2=True, grad_dtype="fp32", ar_chunks=1),
     "fp32-chunked": dict(world2=True, grad_dtype="fp32", ar_chunks=4),
 }
-ENV = ("MDT_GRAD_AR", "MDT_COLLECTIVE", "MDT_AR_CHUNKS", "MDT_TRAIN_GRAPH")
 
 
-def _net(model):
-    from maskdit_b200.maskdit import Precond_models
-    mt, R, ncls, _ = MODELS[model]
-    torch.manual_seed(1)
-    with torch.device("cuda"):
-        net = Precond_models["edm"](img_resolution=R, img_channels=4, num_classes=ncls, model_type=mt,
-                                    use_decoder=True, mae_loss_coef=0.1, pad_cls_token=False)
-        gz = torch.Generator(device="cuda").manual_seed(2)
-        with torch.no_grad():   # the zero-initialised tensors (adaLN, final layer) get values: every gradient is live
-            for p in net.parameters():
-                if p.requires_grad and float(p.abs().sum()) == 0.0:
-                    p.copy_(torch.randn(p.shape, generator=gz, device="cuda") * 0.02)
-    return net.train()
-
-
-def _batches(model, k):
-    """k batches of VAE moments and one-hot labels; batch i is drawn with its own seed."""
-    _, R, ncls, B = MODELS[model]
-    out = []
-    for i in range(k):
-        g = torch.Generator().manual_seed(100 + i)
-        mom = torch.cat([torch.randn(B, 4, R, R, generator=g), torch.randn(B, 4, R, R, generator=g) - 2], 1)
-        lab = torch.nn.functional.one_hot(torch.randint(0, ncls, (B,), generator=g), ncls).float()
-        out.append((mom.cuda(), lab.cuda(), 1000 + i))
-    return out
-
-
-def _poison(batch):
-    mom, lab, seed = batch
-    mom = mom.clone()
-    mom[0, 0, 3, 5] = NAN   # one NaN in the moments' mean
-    return mom, lab, seed
-
-
-def _trainstep(model, mode, rank0_of_two=None, peer=None, lr_rampup_kimg=0.0):
+def _trainstep(model, mode, rank0_of_two=None, lr_rampup_kimg=0.0):
     from maskdit_b200.train_step import TrainStep
     kw = dict(MODES[mode])
     world2, ga = kw.pop("world2", False), kw.pop("grad_accum", 1)
     chunks = kw.pop("ar_chunks", 4)
-    net = _net(model)
+    net = live_net(model)
     B = MODELS[model][3]
     ts = TrainStep(net, copy.deepcopy(net).eval(), lr=1e-3, weight_decay=0.01, global_batch=B * (2 if world2 else 1),
                    lr_rampup_kimg=lr_rampup_kimg, reference_lr_schedule=True, skip_nonfinite=True, **kw)
     if world2:
-        rank0_of_two(ts, peer or Peer(), chunks)
+        rank0_of_two(ts, chunks)
     return ts, ga
 
 
-def _step(ts, batch, ga):
-    mom, lab, seed = batch
-    torch.manual_seed(seed)   # the step's draws (sigma, noise, latent eps, mask noise, label dropout) belong to the batch
-    return ts.step(mom, lab, 0.5, 0.1, grad_accum=ga, moments=True, class_dropout_prob=0.1)
-
-
-def _opt_state(ts):
-    n = ts.st.n_train
-    return {"w32": ts.st.w32[:n].clone(), "w16": ts.st.w16[:n].clone(), "m": ts.m.clone(), "v": ts.v.clone(),
-            "ema": ts.ema_st.w32[:n].clone()}
-
-
-def _assert_skip(before, after, ema_decay):
-    for k in ("w32", "w16", "m", "v"):
-        assert torch.equal(before[k], after[k]), k
-    from test_dp_step_gpu import _ulp32, f32
-    d = f32(ema_decay)
-    step = 1 << 26   # float64 temporaries in slices: XL/2 has 675 M trainable elements
-    for lo in range(0, before["ema"].numel(), step):
-        e0, w0, e1 = (before["ema"][lo:lo + step].double(), before["w32"][lo:lo + step].double(),
-                      after["ema"][lo:lo + step].double())
-        want = d * e0 + (1 - d) * w0
-        err = (e1 - want).abs()
-        # 1 ulp of the result, plus the rounding of either product (the fused multiply-add rounds one of them):
-        # trained weights include elements where d*ema and (1-d)*w nearly cancel, and there a product's rounding is
-        # many ulps of the result
-        bound = _ulp32(want) + _ulp32(d * e0) + _ulp32((1 - d) * w0)
-        assert (err <= bound).all(), (lo, (err / bound).max().item())
-
-
 def _exact_skip(model, mode, rank0_of_two):
-    data = _batches(model, 4)
-    bad = _poison(data[2])
+    data = batches(model, 4)
+    bad = poison(data[2])
     # run A: four steps, the third batch poisoned
     ts, ga = _trainstep(model, mode, rank0_of_two)
     for b in data[:2]:
-        _step(ts, b, ga)
-    before = _opt_state(ts)
-    loss = _step(ts, bad, ga)
+        step_batch(ts, b, ga)
+    before = opt_state(ts)
+    loss = step_batch(ts, bad, ga)
     torch.cuda.synchronize()
     assert not torch.isfinite(loss).all()
-    _assert_skip(before, _opt_state(ts), ts.ema_decay)
-    _step(ts, data[3], ga)
-    a = _opt_state(ts)
+    assert_skipped(before, opt_state(ts), ts.ema_decay)
+    step_batch(ts, data[3], ga)
+    a = opt_state(ts)
     a_counts, a_steps = ts._counts.tolist(), ts.step_count
     del ts
     gc.collect()
@@ -392,8 +241,8 @@ def _exact_skip(model, mode, rank0_of_two):
     # run B: the same batches without the poisoned one
     ts, ga = _trainstep(model, mode, rank0_of_two)
     for b in (data[0], data[1], data[3]):
-        _step(ts, b, ga)
-    b_ = _opt_state(ts)
+        step_batch(ts, b, ga)
+    b_ = opt_state(ts)
     b_counts = ts._counts.tolist()
     assert a_counts == [3, 1] and b_counts == [3, 0] and a_steps == 4 and ts.step_count == 3
     assert ts.applied_steps() == 3
@@ -407,39 +256,32 @@ def _exact_skip(model, mode, rank0_of_two):
 
 
 @pytest.mark.parametrize("mode", list(MODES))
-def test_exact_skip_s2(det, rank0_of_two, monkeypatch, mode):
-    for k in ENV:
-        monkeypatch.delenv(k, raising=False)
+def test_exact_skip_s2(det, rank0_of_two, clean_env, mode):
     _exact_skip("S/2", mode, rank0_of_two)
 
 
 @pytest.mark.parametrize("mode", ["world1", "bf16-chunked"])
-def test_exact_skip_xl2(det, rank0_of_two, monkeypatch, mode):
-    for k in ENV:
-        monkeypatch.delenv(k, raising=False)
+def test_exact_skip_xl2(det, rank0_of_two, clean_env, mode):
     _exact_skip("XL/2", mode, rank0_of_two)
 
 
 # ---- 4. consensus ------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("mode", ["bf16-chunked", "fp32-chunked", "fp32-one-chunk"])
-def test_other_rank_nonfinite_makes_this_rank_skip(det, rank0_of_two, monkeypatch, mode):
+def test_other_rank_nonfinite_makes_this_rank_skip(det, rank0_of_two, clean_env, mode):
     """This rank's gradients are finite, the other rank's are not: every rank checks its local values and one flag word
     is summed over the ranks, so the other rank's flag makes this rank skip too."""
-    for k in ENV:
-        monkeypatch.delenv(k, raising=False)
-    data = _batches("S/2", 2)
-    p = Peer()
-    ts, ga = _trainstep("S/2", mode, rank0_of_two, p)
-    _step(ts, data[0], ga)
-    before = _opt_state(ts)
-    p.flag = 1.0
-    loss = _step(ts, data[1], ga)
+    data = batches("S/2", 2)
+    ts, ga = _trainstep("S/2", mode, rank0_of_two)
+    step_batch(ts, data[0], ga)
+    before = opt_state(ts)
+    ts.comm.peer_flag = 1.0
+    loss = step_batch(ts, data[1], ga)
     torch.cuda.synchronize()
     assert torch.isfinite(loss).all()
-    _assert_skip(before, _opt_state(ts), ts.ema_decay)
+    assert_skipped(before, opt_state(ts), ts.ema_decay)
     assert ts._counts.tolist() == [1, 1] and int(ts.skipped_steps) == 1
-    p.flag = 0.0
-    _step(ts, data[0], ga)
+    ts.comm.peer_flag = 0.0
+    step_batch(ts, data[0], ga)
     assert ts._counts.tolist() == [2, 1]
     assert not torch.equal(before["w32"], ts.st.w32[:ts.st.n_train])
 
@@ -452,15 +294,15 @@ def _two_process_worker():
     torch.cuda.set_device(rank)
     dist.init_process_group("nccl", device_id=torch.device("cuda", rank))
     torch.use_deterministic_algorithms(True)
-    net = _net("S/2")
+    net = live_net("S/2")
     ts = TrainStep(net, copy.deepcopy(net).eval(), lr=1e-3, skip_nonfinite=True, global_batch=8)
-    data = _batches("S/2", 2)
-    _step(ts, data[0], 1)
-    before = _opt_state(ts)
-    _step(ts, _poison(data[1]) if rank == 1 else data[1], 1)
+    data = batches("S/2", 2)
+    step_batch(ts, data[0], 1)
+    before = opt_state(ts)
+    step_batch(ts, poison(data[1]) if rank == 1 else data[1], 1)
     torch.cuda.synchronize()
-    after = _opt_state(ts)
-    _assert_skip(before, after, ts.ema_decay)
+    after = opt_state(ts)
+    assert_skipped(before, after, ts.ema_decay)
     counts = ts._counts.clone()
     allc = [torch.zeros_like(counts) for _ in range(2)]
     dist.all_gather(allc, counts)
@@ -487,28 +329,28 @@ def test_resume_after_a_skip_equals_uninterrupted(det):
     The lr ramps over the four steps, so the resumed run's lr must follow the run's step counter (lr_step_offset, as
     train.py sets it) while Adam follows the applied count."""
     from maskdit_b200.train_step import TrainStep
-    data = _batches("S/2", 4)
-    data[1] = _poison(data[1])
+    data = batches("S/2", 4)
+    data[1] = poison(data[1])
     ramp = 4 * 4 / 1000   # 4 steps of batch 4
 
     def fresh():
-        net = _net("S/2")
+        net = live_net("S/2")
         return TrainStep(net, copy.deepcopy(net).eval(), lr=1e-3, global_batch=4, lr_rampup_kimg=ramp,
                          reference_lr_schedule=True, skip_nonfinite=True)
 
     ts = fresh()
     lrs_a = []
     for b in data:
-        _step(ts, b, 1)
+        step_batch(ts, b, 1)
         lrs_a.append(ts._lr_now)
-    a = _opt_state(ts)
+    a = opt_state(ts)
     assert ts.applied_steps() == 3
     del ts
     gc.collect()
     ts = fresh()
     lrs_b = []
     for b in data[:2]:
-        _step(ts, b, 1)
+        step_batch(ts, b, 1)
         lrs_b.append(ts._lr_now)
     sd = ts.state_dict()
     assert sd["param_groups"][0]["step"] == 1 and all(float(e["step"]) == 1.0 for e in sd["state"].values())
@@ -519,7 +361,7 @@ def test_resume_after_a_skip_equals_uninterrupted(det):
     torch.cuda.empty_cache()
     buf.seek(0)
     ck = torch.load(buf, weights_only=False)
-    net = _net("S/2")
+    net = live_net("S/2")
     net.load_state_dict(ck["model"])
     ema = copy.deepcopy(net).eval()
     ema.load_state_dict(ck["ema"])
@@ -529,42 +371,20 @@ def test_resume_after_a_skip_equals_uninterrupted(det):
     assert ts2.applied_steps() == 1 and int(ts2.skipped_steps) == 0
     ts2.lr_step_offset = 2 - ts2.step_count   # the run's step counter at the checkpoint minus Adam's count
     for b in data[2:]:
-        _step(ts2, b, 1)
+        step_batch(ts2, b, 1)
         lrs_b.append(ts2._lr_now)
     assert lrs_a == lrs_b and lrs_a[0] == 0.0 and len(set(lrs_a)) == 4, lrs_a
     assert ts2.applied_steps() == 3
-    b_ = _opt_state(ts2)
+    b_ = opt_state(ts2)
     for k in a:
         assert torch.equal(a[k], b_[k]), k
 
 
 # ---- 6. train.py end to end --------------------------------------------------------------------------------------------------
-YAML = """
-data: {dataset: imagenet256-latent, category: lmdb, resolution: 16, num_channels: 4, root: none, feat_path: None}
-model:
-  precond: edm
-  model_type: DiT-S/2
-  in_size: 16
-  in_channels: 4
-  num_classes: 1000
-  use_decoder: True
-  ext_feature_dim: 0
-  pad_cls_token: False
-  mask_ratio: 0.5
-  mask_ratio_fn: constant
-  mask_ratio_min: 0
-  mae_loss_coef: 0.1
-  class_dropout_prob: 0.1
-train: {tf32: False, amp: True, batchsize: 8, grad_accum: 1, epochs: 1, lr: 0.0001, lr_rampup_kimg: 0, xflip: False,
-        max_num_steps: 4}
-log: {log_every: 2, ckpt_every: 4, tag: t}
-"""
-
-
 @pytest.mark.parametrize("no_amp", [False, True])
-def test_train_py_skips_a_nan_batch(tmp_path, monkeypatch, capsys, no_amp):
+def test_train_py_skips_a_nan_batch(tmp_path, monkeypatch, clean_env, capsys, no_amp):
     import train
-    for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK", *ENV):
+    for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
         monkeypatch.delenv(k, raising=False)
     real = train.synthetic_loader
 

@@ -12,7 +12,6 @@
 6. train.py writes snapshots, posthoc_ema.py reconstructs sigma_rel 0.08 and generate.py samples from it.
 """
 import copy
-import ctypes
 import gc
 import io
 import os
@@ -28,36 +27,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from maskdit_b200 import phema  # noqa: E402
+from support import (MODELS, YAML, batches, clean_env, comm, det, f32, live_net, ops, poison,  # noqa: E402,F401
+                     rank0_of_two, step_batch, ulp32)
 
-bf16 = torch.bfloat16
 SIGMAS = (0.05, 0.10)
-
-
-@pytest.fixture(scope="module")
-def ops():
-    from maskdit_b200 import ops as o
-    return o
-
-
-@pytest.fixture
-def det():
-    """Deterministic mode on for the test; the torch flag and the SM budget are restored afterwards."""
-    from maskdit_b200 import _lib
-    flag = torch.are_deterministic_algorithms_enabled()
-    torch.use_deterministic_algorithms(True)
-    yield
-    torch.use_deterministic_algorithms(flag)
-    _lib.sync_deterministic()
-    assert _lib.lib().mdt_set_sm_budget(0) == 0
-
-
-def _f32(x):
-    return float(np.float32(x))
-
-
-def _ulp32(x64):
-    a = x64.abs().float()
-    return (torch.nextafter(a, torch.full_like(a, float("inf"))) - a).double()
 
 
 def _replay(ws, gammas, t0=1):
@@ -66,7 +39,7 @@ def _replay(ws, gammas, t0=1):
     for t, w in enumerate(ws, start=t0):
         w = w.double()
         for j, g in enumerate(gammas):
-            es[j] += _f32(phema.one_minus_beta(g, t)) * (w - es[j])
+            es[j] += f32(phema.one_minus_beta(g, t)) * (w - es[j])
     return es
 
 
@@ -74,10 +47,10 @@ def _assert_close(got, want, ws, what):
     """Each step rounds w - e, the product and the sum: at most ~2 ulp of max|w| per step (e is a convex combination
     of the w's, so it never exceeds them; an earlier error only shrinks by the factor 1 - c)."""
     mx = torch.stack([w.double().abs() for w in ws]).amax(0)
-    bound = 2 * len(ws) * _ulp32(mx) + 1e-30
+    bound = 2 * len(ws) * ulp32(mx) + 1e-30
     err = (got.double() - want).abs()
     assert (err <= bound).all(), (what, (err / bound).max().item())
-    return (err / _ulp32(mx).clamp_min(1e-30)).max().item()
+    return (err / ulp32(mx).clamp_min(1e-30)).max().item()
 
 
 # ---- 1. the kernel ------------------------------------------------------------------------------------------------------
@@ -129,49 +102,12 @@ def test_kernel_refuses_cpu_and_mismatched_buffers(ops):
 
 
 # ---- 2. TrainStep -----------------------------------------------------------------------------------------------------------
-R, NCLS, B = 32, 1000, 4
-
-
-def _net():
-    from maskdit_b200.maskdit import Precond_models
-    torch.manual_seed(1)
-    with torch.device("cuda"):
-        net = Precond_models["edm"](img_resolution=R, img_channels=4, num_classes=NCLS, model_type="DiT-S/2",
-                                    use_decoder=True, mae_loss_coef=0.1, pad_cls_token=False)
-        gz = torch.Generator(device="cuda").manual_seed(2)
-        with torch.no_grad():   # the zero-initialised tensors get values: every gradient is live
-            for p in net.parameters():
-                if p.requires_grad and float(p.abs().sum()) == 0.0:
-                    p.copy_(torch.randn(p.shape, generator=gz, device="cuda") * 0.02)
-    return net.train()
-
-
-def _batches(k):
-    out = []
-    for i in range(k):
-        g = torch.Generator().manual_seed(100 + i)
-        mom = torch.cat([torch.randn(B, 4, R, R, generator=g), torch.randn(B, 4, R, R, generator=g) - 2], 1)
-        lab = torch.nn.functional.one_hot(torch.randint(0, NCLS, (B,), generator=g), NCLS).float()
-        out.append((mom.cuda(), lab.cuda(), 1000 + i))
-    return out
-
-
-def _poison(batch):
-    mom, lab, seed = batch
-    mom = mom.clone()
-    mom[0, 0, 3, 5] = float("nan")
-    return mom, lab, seed
-
-
-def _step(ts, batch, ga=1):
-    mom, lab, seed = batch
-    torch.manual_seed(seed)
-    return ts.step(mom, lab, 0.5, 0.1, grad_accum=ga, moments=True, class_dropout_prob=0.1)
+B = MODELS["S/2"][3]
 
 
 def _trainstep(**kw):
     from maskdit_b200.train_step import TrainStep
-    net = _net()
+    net = live_net("S/2")
     return TrainStep(net, copy.deepcopy(net).eval(), lr=1e-3, weight_decay=0.01, global_batch=B, **kw)
 
 
@@ -187,22 +123,22 @@ MODES = {
 @pytest.mark.parametrize("mode", list(MODES))
 def test_trainstep_profiles_are_the_power_ema_of_the_weights(mode):
     kw = dict(MODES[mode])
-    ga, poison = kw.pop("grad_accum", 1), kw.pop("poison", None)
+    ga, bad = kw.pop("grad_accum", 1), kw.pop("poison", None)
     ts = _trainstep(phema_sigma_rels=SIGMAS, **kw)
     n = ts.st.n_train
     assert len(ts.phema_emas) == 2 and all(e.numel() == n for e in ts.phema_emas)
     ws = []
-    data = _batches(6)
+    data = batches("S/2", 6)
     for i, b in enumerate(data):
-        if i == poison:
-            b = _poison(b)
+        if i == bad:
+            b = poison(b)
             before = ts.st.w32[:n].clone()
-        _step(ts, b, ga)
+        step_batch(ts, b, ga)
         ws.append(ts.st.w32[:n].clone())
         if i == 0:
             for e in ts.phema_emas:
                 assert torch.equal(e, ws[0])       # t = 1: a copy of the weights after the first update
-        if i == poison:
+        if i == bad:
             assert torch.equal(ws[-1], before) and int(ts.skipped_steps) == 1
     torch.cuda.synchronize()
     assert ts.phema_origin == 0 and ts.phema_steps == 6
@@ -223,8 +159,8 @@ def test_off_by_default_and_invisible_to_training(det, ops):
         n = ts.st.n_train
         assert bool(ts.phema_emas) == (name == "on")
         n0 = ops.L.LAUNCHES
-        for b in _batches(3):
-            _step(ts, b)
+        for b in batches("S/2", 3):
+            step_batch(ts, b)
         torch.cuda.synchronize()
         runs[name] = (ops.L.LAUNCHES - n0, ts.st.w32[:n].clone(), ts.ema_st.w32[:n].clone(), ts.m.clone())
         del ts
@@ -238,10 +174,10 @@ def test_off_by_default_and_invisible_to_training(det, ops):
 
 # ---- 4. resume ---------------------------------------------------------------------------------------------------------------
 def test_resume_continues_the_profiles_bit_for_bit(det):
-    data = _batches(5)
+    data = batches("S/2", 5)
     ts = _trainstep(phema_sigma_rels=SIGMAS)
     for b in data:
-        _step(ts, b)
+        step_batch(ts, b)
     torch.cuda.synchronize()
     a = [e.clone() for e in ts.phema_emas]
     a_snap = ts.phema_snapshot()
@@ -249,7 +185,7 @@ def test_resume_continues_the_profiles_bit_for_bit(det):
     gc.collect()
     ts = _trainstep(phema_sigma_rels=SIGMAS)
     for b in data[:2]:
-        _step(ts, b)
+        step_batch(ts, b)
     buf = io.BytesIO()
     torch.save({"model": ts.net.state_dict(), "ema": ts.ema.state_dict(), "opt": ts.state_dict()}, buf)
     del ts
@@ -259,14 +195,14 @@ def test_resume_continues_the_profiles_bit_for_bit(det):
     ck = torch.load(buf, weights_only=False)
     assert ck["opt"]["phema"]["steps"] == 2 and ck["opt"]["phema"]["origin"] == 0
     from maskdit_b200.train_step import TrainStep
-    net = _net()
+    net = live_net("S/2")
     net.load_state_dict(ck["model"])
     ema = copy.deepcopy(net).eval()
     ema.load_state_dict(ck["ema"])
     ts2 = TrainStep(net, ema, lr=1e-3, weight_decay=0.01, global_batch=B, phema_sigma_rels=SIGMAS)
     ts2.load_state_dict(ck["opt"])
     for b in data[2:]:
-        _step(ts2, b)
+        step_batch(ts2, b)
     torch.cuda.synchronize()
     for x, y in zip(a, ts2.phema_emas):
         assert torch.equal(x, y)
@@ -281,45 +217,16 @@ def test_resume_continues_the_profiles_bit_for_bit(det):
     # a checkpoint without profiles (a reference one): new profiles counted from the resume step
     opt = dict(ck["opt"])
     del opt["phema"]
-    net3 = _net()
+    net3 = live_net("S/2")
     ts3 = TrainStep(net3, copy.deepcopy(net3).eval(), lr=1e-3, global_batch=B, phema_sigma_rels=SIGMAS)
     ts3.load_state_dict(opt)
     ts3.lr_step_offset = 7 - ts3.step_count       # as train.py sets it for a checkpoint of run step 7
-    _step(ts3, data[0])
+    step_batch(ts3, data[0])
     assert ts3.phema_origin == 7 and ts3.phema_steps == 1
     assert all(torch.equal(e, ts3.st.w32[:ts3.st.n_train]) for e in ts3.phema_emas)
 
 
 # ---- 5. world > 1 ------------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def comm(ops):
-    """A one-rank communicator."""
-    L = ops.lib()
-    uid = ctypes.create_string_buffer(128)
-    assert L.mdt_nccl_unique_id(uid) == 0
-    c = ctypes.c_void_p()
-    assert L.mdt_nccl_comm_create(bytes(uid.raw), 0, 1, 0, ctypes.byref(c)) == 0 and c.value
-    yield c
-    assert L.mdt_nccl_comm_destroy(c) == 0
-
-
-class TwoIdenticalRanks:
-    """Stand-in for `GradComm` on rank 0 of two ranks that hold the same gradient: the real one-rank
-    `mdt_allreduce_grads`, then the buffer doubled (the exact sum of the two ranks)."""
-
-    def __init__(self, comm):
-        self.comm = comm
-
-    def all_reduce(self, t):
-        from maskdit_b200 import ops
-        assert ops.lib().mdt_allreduce_grads(self.comm, t.data_ptr(), t.numel(), int(t.dtype == bf16),
-                                             ops.stream_ptr()) == 0
-        t.mul_(2)
-
-    def close(self):
-        pass
-
-
 WORLD2 = {
     "bf16-chunked": dict(grad_dtype="bf16", ar_chunks=4),
     "bf16-flat": dict(grad_dtype="bf16", ar_chunks=1),
@@ -329,18 +236,11 @@ WORLD2 = {
 
 
 @pytest.mark.parametrize("mode", list(WORLD2))
-def test_world2_every_element_once_after_its_pass(ops, comm, monkeypatch, mode):
+def test_world2_every_element_once_after_its_pass(ops, rank0_of_two, clean_env, monkeypatch, mode):
     from maskdit_b200.train_step import ar_chunk_bounds
-    for k in ("MDT_GRAD_AR", "MDT_COLLECTIVE", "MDT_AR_CHUNKS", "MDT_TRAIN_GRAPH"):
-        monkeypatch.delenv(k, raising=False)
     kw = dict(WORLD2[mode])
     chunks = kw.pop("ar_chunks")
-    ts = _trainstep(phema_sigma_rels=SIGMAS, **kw)
-    ts.world = 2
-    ts.comm = TwoIdenticalRanks(comm)
-    if ts.grad_dtype == "bf16":
-        ts.g16 = torch.empty(ts.st.n_train, dtype=bf16, device="cuda")
-    ts.ar_chunks = chunks
+    ts = rank0_of_two(_trainstep(phema_sigma_rels=SIGMAS, **kw), chunks)
     n = ts.st.n_train
     log = []
 
@@ -354,9 +254,9 @@ def test_world2_every_element_once_after_its_pass(ops, comm, monkeypatch, mode):
     for name in ("adamw_ema", "adamw_ema_guarded", "power_ema"):
         monkeypatch.setattr(ops, name, recorder(name, getattr(ops, name)))
     ws = []
-    for step, b in enumerate(_batches(3)):
+    for step, b in enumerate(batches("S/2", 3)):
         log.clear()
-        _step(ts, b)
+        step_batch(ts, b)
         ws.append(ts.st.w32[:n].clone())
         what = f"{mode} step {step}"
         pe = [(lo, hi, s) for name, lo, hi, s in log if name == "power_ema"]
@@ -375,28 +275,6 @@ def test_world2_every_element_once_after_its_pass(ops, comm, monkeypatch, mode):
 
 
 # ---- 6. train.py -> posthoc_ema.py -> generate.py --------------------------------------------------------------------------
-YAML = """
-data: {dataset: imagenet256-latent, category: lmdb, resolution: 16, num_channels: 4, root: none, feat_path: None}
-model:
-  precond: edm
-  model_type: DiT-S/2
-  in_size: 16
-  in_channels: 4
-  num_classes: 1000
-  use_decoder: True
-  ext_feature_dim: 0
-  pad_cls_token: False
-  mask_ratio: 0.5
-  mask_ratio_fn: constant
-  mask_ratio_min: 0
-  mae_loss_coef: 0.1
-  class_dropout_prob: 0.1
-train: {tf32: False, amp: True, batchsize: 8, grad_accum: 1, epochs: 1, lr: 0.0001, lr_rampup_kimg: 0, xflip: False,
-        max_num_steps: 6}
-log: {log_every: 2, ckpt_every: 4, tag: t}
-"""
-
-
 def _run(cmd, cwd):
     env = dict(os.environ, PYTHONPATH=ROOT)
     r = subprocess.run([sys.executable, *cmd], cwd=cwd, env=env, capture_output=True, text=True, timeout=600)
@@ -406,7 +284,7 @@ def _run(cmd, cwd):
 
 def test_train_posthoc_generate(tmp_path):
     cfg = tmp_path / "cfg.yaml"
-    cfg.write_text(YAML)
+    cfg.write_text(YAML.replace("max_num_steps: 4", "max_num_steps: 6"))
     res = tmp_path / "res"
     out = _run([os.path.join(ROOT, "train.py"), "--config", str(cfg), "--synthetic", "--max_steps", "6",
                 "--phema_sigma_rel", "0.05,0.10", "--phema_every", "2", "--results_dir", str(res)], str(tmp_path))

@@ -33,6 +33,7 @@ import torch.nn.functional as F
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from support import lib  # noqa: E402,F401
 
 pytestmark = pytest.mark.gpu
 f64, bf16 = torch.float64, torch.bfloat16
@@ -51,18 +52,6 @@ EPI_NAME = {EPI_STORE: "store", EPI_GELU: "gelu", EPI_GATE_RESID: "gate_resid", 
             EPI_ATOMIC: "atomic"}
 
 
-@pytest.fixture
-def lib():
-    """The library; the torch flag, the library setting and the SM budget are restored afterwards."""
-    from maskdit_b200 import _lib
-    Lb = _lib.lib()
-    det, budget, flag = Lb.mdt_get_deterministic(), Lb.mdt_get_sm_budget(), torch.are_deterministic_algorithms_enabled()
-    assert Lb.mdt_set_sm_budget(0) == 0
-    yield Lb
-    torch.use_deterministic_algorithms(flag)
-    assert Lb.mdt_set_deterministic(det) == 0 and Lb.mdt_set_sm_budget(budget) == 0
-
-
 @pytest.fixture(scope="module", autouse=True)
 def _report():
     """Wall time and peak allocated device memory of the whole file."""
@@ -76,7 +65,7 @@ def _report():
 
 
 def _net(dec, R):
-    """The training network with test_model_gpu.build()'s weights (the oracle's seeded state dict, every tensor the
+    """The training network with support.build()'s weights (the oracle's seeded state dict, every tensor the
     reference zero-inits randomised)."""
     from maskdit_b200.maskdit import Precond_models
     from oracle import maskdit_oracle as O

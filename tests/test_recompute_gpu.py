@@ -12,24 +12,13 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from test_deterministic_gpu import _net, _same, _steps  # noqa: E402
-from test_model_gpu import LOSS_TOL, GoldenLoss, check_grads, load, rel_l2  # noqa: E402
+from support import (LOSS_TOL, GoldenLoss, assert_same, check_grads, det_steps, lib, load,  # noqa: E402,F401
+                     oracle_net, rel_l2)
 
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture
-def lib():
-    """The library; the torch flag, the library setting and the SM budget are restored afterwards."""
-    from maskdit_b200 import _lib
-    L = _lib.lib()
-    det, budget, flag = L.mdt_get_deterministic(), L.mdt_get_sm_budget(), torch.are_deterministic_algorithms_enabled()
-    yield L
-    torch.use_deterministic_algorithms(flag)
-    assert L.mdt_set_deterministic(det) == 0 and L.mdt_set_sm_budget(budget) == 0
-
-
-# (case, depth, depth + dec_depth): the steps of _steps (test_deterministic_gpu) on existing goldens' shapes
+# (case, depth, depth + dec_depth): the steps of support.det_steps on existing goldens' shapes
 CASES = {
     "s2_mask50": (dict(mt="DiT-S/2", R=8, ncls=10, dec=True, B=2, mask=0.5, golden="s2_train_mask", n=2), 12, 20),
     "xl2_c1": (dict(mt="DiT-XL/2", R=32, ncls=1000, dec=True, B=2, mask=0.5, golden="xl2_c1_grads", n=1), 28, 36),
@@ -51,9 +40,9 @@ def test_recomputed_steps_are_bit_identical(lib, case):
     kw = dict(kw)
     if kw.get("golden"):
         kw["golden"] = load(kw["golden"])
-    base = _steps(**kw, recompute_blocks=0)
+    base = det_steps(**kw, recompute_blocks=0)
     for r in sorted({1, depth, nb}):
-        _same(base, _steps(**kw, recompute_blocks=r))
+        assert_same(base, det_steps(**kw, recompute_blocks=r))
 
 
 @pytest.mark.parametrize("name,mt,R,ncls,dec", [("s2_train_mask", "DiT-S/2", 8, 10, True),
@@ -63,7 +52,7 @@ def test_full_recompute_vs_reference_golden(lib, name, mt, R, ncls, dec):
     """Default mode, every block recomputed: loss and gradients within the bounds of the r = 0 golden tests."""
     torch.use_deterministic_algorithms(False)
     g = load(name)
-    net = _net(mt, R, ncls, dec)
+    net = oracle_net(mt, R, ncls, dec)
     net.prepare()
     ce = net._engine
     ce.recompute = ce.num_blocks
@@ -86,7 +75,7 @@ def _raw_backward(ce, ctx, dF):
 
 def test_backward_refuses_a_workspace_of_another_count(lib):
     torch.use_deterministic_algorithms(False)
-    net = _net("DiT-S/2", 8, 10, True)
+    net = oracle_net("DiT-S/2", 8, 10, True)
     st = net.prepare()
     st.ensure_grad().zero_()
     ce = net._engine
@@ -141,7 +130,7 @@ def test_nodecoder_xl2_batch256_unmasked_fits_one_card(lib):
     torch.use_deterministic_algorithms(False)
     torch.cuda.empty_cache()          # the workspace needs the blocks earlier tests left in the caching allocator
     total = torch.cuda.get_device_properties(0).total_memory
-    net = _net("DiT-XL/2", 32, 1000, False)
+    net = oracle_net("DiT-XL/2", 32, 1000, False)
     ts = TrainStep(net, None, lr=0.0)
     B = 256
     gen = torch.Generator().manual_seed(11)

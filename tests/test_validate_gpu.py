@@ -25,19 +25,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from maskdit_b200 import validate as V  # noqa: E402
 from oracle import maskdit_oracle as O  # noqa: E402
+from support import det  # noqa: E402,F401
 
 GOLD = os.path.join(ROOT, "tests", "golden", "val_s2.npz")
 LOSS_TOL = 5e-3
-
-
-@pytest.fixture
-def det():
-    from maskdit_b200 import _lib
-    flag = torch.are_deterministic_algorithms_enabled()
-    torch.use_deterministic_algorithms(True)
-    yield
-    torch.use_deterministic_algorithms(flag)
-    _lib.sync_deterministic()
 
 
 def _net(model_type, R, ncls, seed=1):
