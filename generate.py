@@ -14,7 +14,9 @@ per seed as well; without a VAE checkpoint `--png_preview` writes the raw latent
 Guidance beyond the reference's `--cfg_scale`: `--guide_ckpt` (or `--guide_snapshots` + `--guide_sigma_rel`, a post-hoc
 EMA built by `posthoc_ema.reconstruct`) with `--guidance W` guides with a second, weaker network of the same image
 geometry and classes (autoguidance; `--guide_config` when its architecture differs), and `--guidance_interval LO HI`
-applies CFG or the guide only at evaluations with LO < sigma <= HI.  Class-unconditional configs sample with all-zero
+applies CFG or the guide only at evaluations with LO < sigma <= HI.  A rectified-flow config (`model.precond: flow`)
+samples with `flow_sampler` (Heun on a uniform t grid, `--num_steps`, `--cfg_scale`, `--guidance_interval` on t) and
+refuses the ablation switches, `--S_churn` and autoguidance.  Class-unconditional configs sample with all-zero
 label rows as the reference does (sample.py:261-264).
 """
 import argparse
@@ -26,7 +28,7 @@ import torch
 from maskdit_b200.config import build_net, load_config, parse_float_none, parse_int_list
 from maskdit_b200.maskdit import eval_state_dict
 from maskdit_b200 import ops
-from maskdit_b200.sampler import ablation_sampler, edm_sampler, rank_seed_batches, write_png
+from maskdit_b200.sampler import ablation_sampler, edm_sampler, flow_sampler, rank_seed_batches, write_png
 
 
 class StackedRandomGenerator:
@@ -107,6 +109,19 @@ def parse_args(argv=None):
     return args
 
 
+def check_flow_args(args):
+    """A rectified-flow config (`model.precond: flow`) samples with `flow_sampler` (Heun on a uniform t grid,
+    `--num_steps`, `--cfg_scale`, `--guidance_interval` on t): refuse the EDM-only switches it has no meaning for."""
+    bad = [f"--{k}" for k in ("solver", "discretization", "schedule", "scaling") if getattr(args, k)]
+    if args.S_churn:
+        bad.append("--S_churn")
+    if args.guide_ckpt is not None or args.guide_snapshots is not None or args.guidance is not None:
+        bad.append("autoguidance (--guide_ckpt / --guide_snapshots / --guidance)")
+    if bad:
+        raise SystemExit(f"a flow config (model.precond: flow) samples with flow_sampler: {', '.join(bad)} "
+                         "apply to the EDM samplers only")
+
+
 def guide_state_dict(args):
     """The guide's state dict on the host: `--guide_key` of `--guide_ckpt`, or the post-hoc EMA of width
     `--guide_sigma_rel` at `--guide_step` reconstructed from `--guide_snapshots` (posthoc_ema.reconstruct)."""
@@ -130,6 +145,9 @@ def main(argv=None):
     device = torch.device("cuda", local)
     if size > 1:
         torch.distributed.init_process_group("nccl", device_id=device)
+    flow = cfg.model.precond == "flow"
+    if flow:
+        check_flow_args(args)
     net = build_net(cfg).to(device).eval()
     if args.ckpt_path:
         # trusted checkpoint: reference checkpoints hold an argparse.Namespace under 'args' (train.py:259-265)
@@ -166,9 +184,13 @@ def main(argv=None):
             labels[:, :] = 0
             labels[:, args.class_idx] = 1
         with torch.no_grad():
-            z = sampler_fn(net, latents.float(), labels.float(), cfg_scale=args.cfg_scale,
-                           randn_like=rnd.randn_like, num_steps=args.num_steps, S_churn=args.S_churn, **kw,
-                           **gkw).float()
+            if flow:
+                z = flow_sampler(net, latents.float(), labels.float(), cfg_scale=args.cfg_scale,
+                                 num_steps=args.num_steps, **gkw).float()
+            else:
+                z = sampler_fn(net, latents.float(), labels.float(), cfg_scale=args.cfg_scale,
+                               randn_like=rnd.randn_like, num_steps=args.num_steps, S_churn=args.S_churn, **kw,
+                               **gkw).float()
         if vae is not None:       # images = vae.decode(z); add(1).mul(127.5).clamp(0,255).to(uint8) NHWC; PNG per seed
             px = ops.to_uint8_nhwc(vae.decode(z).contiguous()).cpu().numpy()
             for s, im in zip(bs, px):

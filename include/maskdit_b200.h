@@ -25,6 +25,10 @@ extern "C" {
 #define MDT_ERR_TMAP (-4)   /* tensor-map encode rejected the operand */
 #define MDT_ERR_UNSUPPORTED (-5)
 
+/* Precondition kinds of a model handle (mdt_model_set_precond) and of the kernels that depend on it */
+#define MDT_PRECOND_EDM 0   /* sigma: EDM noise level; c_in = 1/sqrt(sigma^2 + sigma_data^2), c_noise = ln(sigma)/4 */
+#define MDT_PRECOND_FLOW 1  /* sigma holds the flow time t in [0, 1]; c_in = 1, c_noise = t                            */
+
 const char* mdt_status_string(int status);
 int mdt_abi_version(void);
 /* BLOCK_N * 10 + CTAs-per-tile (always 1) of the last mdt_gemm_bf16 launch (tests). */
@@ -113,6 +117,8 @@ int mdt_patch_embed_bwd(const float* x, const float* sigma, float sigma_data, co
 /* TimestepEmbedder.timestep_embedding (models/maskdit.py:41-58) on t = c_noise = ln(sigma)/4 (:767):
  *   out[b] = [cos(t f_k) | sin(t f_k)], f_k = exp(-ln(1e4) k / (dim/2)); out bf16 [B, dim]                  */
 int mdt_timestep_freq(const float* sigma, int B, int dim, void* out_bf16, void* stream);
+/* The same embedding on c_noise = t, the flow time (rectified flow, SiT).                                         */
+int mdt_flow_timestep_freq(const float* t, int B, int dim, void* out_bf16, void* stream);
 
 /* Pointwise helpers around the conditioning MLPs (nn.SiLU at models/maskdit.py:36,184,205,226).
  *   silu:      out_bf16 = silu(a [+ b])  (and out_f32 = a + b if non-NULL)
@@ -223,6 +229,29 @@ int mdt_logvar_wgrad(const float* sigma, const float* freqs, const float* phases
 int mdt_step_front(const float* moments, const float* eps, const float* rnd_normal, const float* noise_unit,
                    const float* drop_u, float drop_prob, float scale_factor, float P_mean, float P_std, float* y,
                    float* yn, float* sigma, float* labels, int B, int C, int R, int num_classes, void* stream);
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Rectified flow (linear interpolant, velocity prediction; SiT, Ma et al. 2024).  t in [0, 1], t = 0 data, t = 1 noise:
+ *   x_t = (1 - t) x + t eps ; network input x_t unscaled (c_in = 1), c_noise = t ; v^ = unpatchify(F) ; target
+ *   v = eps - x ; denoised estimate x^ = x_t - t v^.
+ * mdt_flow_loss: F [B,L,p*p*C] f32 ; xt [B,C,R,R] ; y = x [B,C,R,R] clean ; eps [B,C,R,R] the noise ; t [B]
+ *   mask != NULL: loss[b] = mean_{kept}(patch-mean((v^-v)^2)) + mae_coef * mean_{removed}(MSE(patchify(x^), norm-patchify(xt)))
+ *   mask == NULL: loss[b] = mean((v^-v)^2)
+ *   dF_bf16 (optional, needs gl) = d(sum_b gl[b]*loss[b]) / dF ; x_hat (optional) [B,C,R,R] f32.
+ *   The kept / removed-row rules and the pd handling are mdt_edm_loss's.
+ * mdt_flow_cfg_out: out [B,C,R,R] = unpatchify(Fu + s (Fc - Fu)) with use_cfg (F [2B,...], cond rows first), else
+ *   unpatchify(F) (F [B,...]).
+ * mdt_flow_step_front: mdt_step_front's latent and label dropout, then t[b] = 1 / (1 + exp(-(P_mean + P_std *
+ *   rnd_normal[b]))) and xt = (1 - t) y + t noise_unit, each product and sum rounded separately.
+ * ------------------------------------------------------------------------------------------------------------ */
+int mdt_flow_loss(const float* F, const float* xt, const float* y, const float* eps, const float* t, const float* mask,
+                  const float* gl, float mae_coef, float* loss, float* x_hat, void* dF_bf16, int B, int C, int R, int p,
+                  void* stream);
+int mdt_flow_cfg_out(const float* F, int use_cfg, float cfg_scale, float* out, int B, int C, int R, int p,
+                     void* stream);
+int mdt_flow_step_front(const float* moments, const float* eps, const float* rnd_normal, const float* noise_unit,
+                        const float* drop_u, float drop_prob, float scale_factor, float P_mean, float P_std, float* y,
+                        float* xt, float* t, float* labels, int B, int C, int R, int num_classes, void* stream);
 
 /* D only (sampler / generic autograd path): Dx = c_skip*xin + c_out*unpatchify(F); and its backward
  * dF_bf16 = c_out * patchify(gD).                                                                            */
@@ -437,6 +466,11 @@ int mdt_model_get_recompute(const mdt_model* m); /* -1 for a NULL handle */
  * default) is the layout without them.  MDT_ERR_ARG for channels < 0 or > 256, and once the handle has sized or laid
  * out a workspace (mdt_workspace_bytes, mdt_forward).                                                               */
 int mdt_model_set_logvar(mdt_model* m, int channels);
+
+/* Precondition kind of the handle: MDT_PRECOND_EDM (the default) or MDT_PRECOND_FLOW, where mdt_forward /
+ * mdt_backward read their `sigma` argument as the flow time t: the patch embedding (forward and backward) applies
+ * c_in = 1 and the timestep frequencies take c_noise = t.  The layout does not change.  MDT_ERR_ARG for another kind. */
+int mdt_model_set_precond(mdt_model* m, int kind);
 
 /* Workspace bytes for batch B with T kept tokens per sample (T <= 0: no token dropping, T = L).
  * training != 0: every activation the backward needs stays resident (+ the backward's scratch; with recomputation only

@@ -65,6 +65,7 @@ _SIGS = {
     "mdt_patch_embed": [_P, _P, _F, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     "mdt_patch_embed_bwd": [_P, _P, _F, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P],
     "mdt_timestep_freq": [_P, _I, _I, _P, _P],
+    "mdt_flow_timestep_freq": [_P, _I, _I, _P, _P],
     "mdt_silu": [_P, _P, _P, _P, _LL, _P],
     "mdt_silu_bwd": [_P, _P, _P, _P, _LL, _P],
     "mdt_cast_f32_bf16": [_P, _P, _LL, _P],
@@ -88,6 +89,9 @@ _SIGS = {
     "mdt_logvar": [_P, _P, _P, _P, _I, _I, _P, _P],
     "mdt_logvar_wgrad": [_P, _P, _P, _P, _I, _I, _P, _P],
     "mdt_step_front": [_P, _P, _P, _P, _P, _F, _F, _F, _F, _P, _P, _P, _P, _I, _I, _I, _I, _P],
+    "mdt_flow_step_front": [_P, _P, _P, _P, _P, _F, _F, _F, _F, _P, _P, _P, _P, _I, _I, _I, _I, _P],
+    "mdt_flow_loss": [_P, _P, _P, _P, _P, _P, _P, _F, _P, _P, _P, _I, _I, _I, _I, _P],
+    "mdt_flow_cfg_out": [_P, _I, _F, _P, _I, _I, _I, _I, _P],
     "mdt_edm_precond_out": [_P, _P, _P, _F, _P, _I, _I, _I, _I, _P],
     "mdt_edm_precond_out_bwd": [_P, _P, _F, _P, _I, _I, _I, _I, _P],
     "mdt_cfg_precond_out": [_P, _P, _P, _F, _F, _P, _I, _I, _I, _I, _P],
@@ -103,6 +107,7 @@ _SIGS = {
     "mdt_model_set_recompute": [_P, _I],
     "mdt_model_get_recompute": [_P],
     "mdt_model_set_logvar": [_P, _I],
+    "mdt_model_set_precond": [_P, _I],
     "mdt_forward": [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _LL, _P, _P],
     "mdt_backward": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _P, _LL, GRAD_READY_FN, _P, _P],
     "mdt_nccl_unique_id": [_P],

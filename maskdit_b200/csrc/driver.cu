@@ -70,6 +70,7 @@ struct mdt_model {
   int recompute = 0;               // blocks whose activations the backward recomputes (mdt_model_set_recompute)
   int logvar_channels = 0;         // learned loss weighting u(sigma) (mdt_model_set_logvar); 0: none
   Tensor lv_freqs, lv_phases, lv_w;
+  int precond = MDT_PRECOND_EDM;   // how mdt_forward / mdt_backward read `sigma` (mdt_model_set_precond)
   mutable bool planned = false;    // a workspace was sized or laid out: the layout is final
   // the workspace of the last mdt_forward(save = 1) and the recompute count it was laid out for: mdt_backward refuses
   // to read a workspace with another count's plan
@@ -541,6 +542,12 @@ int mdt_model_set_logvar(mdt_model* m, int channels) {
   return MDT_OK;
 }
 
+int mdt_model_set_precond(mdt_model* m, int kind) {
+  if (!m || (kind != MDT_PRECOND_EDM && kind != MDT_PRECOND_FLOW)) return MDT_ERR_ARG;
+  m->precond = kind;
+  return MDT_OK;
+}
+
 long long mdt_workspace_bytes(const mdt_model* m, int B, int T, int training) {
   if (!m || B <= 0) return -1;
   if (T <= 0) T = m->L;
@@ -566,10 +573,13 @@ int mdt_forward(const mdt_model* m, const float* w32, const void* w16, const flo
   cudaStream_t cs = static_cast<cudaStream_t>(stream);
 
   float* X = c.at<float>(p.X0);
-  c.ck(mdt_patch_embed(x_in, sigma, cf.sigma_data, c.W32(m->xw), c.W32(m->xb), c.W32(m->pos), ids_keep, X, B,
-                       cf.img_channels, cf.img_resolution, cf.patch_size, D, T, stream));
+  // flow: sigma holds t, the input is not scaled (a NULL sigma is c_in = 1) and c_noise = t
+  const bool flow = m->precond == MDT_PRECOND_FLOW;
+  c.ck(mdt_patch_embed(x_in, flow ? nullptr : sigma, cf.sigma_data, c.W32(m->xw), c.W32(m->xb), c.W32(m->pos),
+                       ids_keep, X, B, cf.img_channels, cf.img_resolution, cf.patch_size, D, T, stream));
   // conditioning: c = t_emb(c_noise) + y_emb(labels)   (models/maskdit.py:491-495, :767)
-  c.ck(mdt_timestep_freq(sigma, B, 256, c.at<void>(p.tf), stream));
+  c.ck(flow ? mdt_flow_timestep_freq(sigma, B, 256, c.at<void>(p.tf), stream)
+            : mdt_timestep_freq(sigma, B, 256, c.at<void>(p.tf), stream));
   float* th_pre = c.at<float>(p.th_pre);
   Gemm(c.at<void>(p.tf), c.W16(m->t0w), B, D, 256).out32(th_pre).bias(c.W32(m->t0b)).run(c);
   c.ck(mdt_silu(th_pre, nullptr, nullptr, c.at<void>(p.th), static_cast<i64>(B) * D, stream));
@@ -735,7 +745,7 @@ int mdt_backward(const mdt_model* m, const float* w32, const void* w16, float* g
     if (on_ready && c.rc == MDT_OK) on_ready(user, m->enc[i].lo, m->enc[i].hi);
   }
   // ---- patch embedding (no input gradient needed)
-  c.ck(mdt::patch_embed_bwd_s(x_in, sigma, cf.sigma_data, ids_keep, Ge, c.Gd(m->xw), c.Gd(m->xb), B, cf.img_channels,
+  c.ck(mdt::patch_embed_bwd_s(x_in, m->precond == MDT_PRECOND_FLOW ? nullptr : sigma, cf.sigma_data, ids_keep, Ge, c.Gd(m->xw), c.Gd(m->xb), B, cf.img_channels,
                               cf.img_resolution, cf.patch_size, D, T, c.scratch, cs));
   // ---- adaLN projections of all blocks at once, then the conditioning MLPs
   void* dmod16 = c.at<void>(p.dmod16);

@@ -168,13 +168,16 @@ __global__ void patch_embed_bwd_partial_kernel(const float* __restrict__ x, cons
 // =========================================================================================================
 // Conditioning pointwise ops
 // =========================================================================================================
+// kPrecond: MDT_PRECOND_EDM reads sigma and embeds c_noise = ln(sigma) / 4; MDT_PRECOND_FLOW reads the flow time t and
+// embeds c_noise = t (SiT).
+template <int kPrecond>
 __global__ void timestep_freq_kernel(const float* __restrict__ sigma, int B, int dim,
                                      __nv_bfloat16* __restrict__ out) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   const int half = dim / 2;
   if (idx >= B * half) return;
   const int b = idx / half, k = idx % half;
-  const float t = logf(sigma[b]) * 0.25f;  // c_noise, models/maskdit.py:767
+  const float t = kPrecond == MDT_PRECOND_FLOW ? sigma[b] : logf(sigma[b]) * 0.25f;  // c_noise, models/maskdit.py:767
   const float f = expf(-logf(10000.f) * static_cast<float>(k) / static_cast<float>(half));
   const float a = t * f;
   out[static_cast<size_t>(b) * dim + k] = __float2bfloat16_rn(cosf(a));
@@ -833,8 +836,16 @@ int mdt_patch_embed_bwd(const float* x, const float* sigma, float sigma_data, co
 int mdt_timestep_freq(const float* sigma, int B, int dim, void* out_bf16, void* stream) {
   if (!sigma || !out_bf16 || B <= 0 || dim <= 0 || dim % 2) return MDT_ERR_ARG;
   const int n = B * dim / 2;
-  timestep_freq_kernel<<<(n + 255) / 256, 256, 0, S(stream)>>>(sigma, B, dim,
-                                                                 static_cast<__nv_bfloat16*>(out_bf16));
+  timestep_freq_kernel<MDT_PRECOND_EDM><<<(n + 255) / 256, 256, 0, S(stream)>>>(sigma, B, dim,
+                                                                                 static_cast<__nv_bfloat16*>(out_bf16));
+  return launch_status();
+}
+
+int mdt_flow_timestep_freq(const float* t, int B, int dim, void* out_bf16, void* stream) {
+  if (!t || !out_bf16 || B <= 0 || dim <= 0 || dim % 2) return MDT_ERR_ARG;
+  const int n = B * dim / 2;
+  timestep_freq_kernel<MDT_PRECOND_FLOW><<<(n + 255) / 256, 256, 0, S(stream)>>>(t, B, dim,
+                                                                                  static_cast<__nv_bfloat16*>(out_bf16));
   return launch_status();
 }
 

@@ -1,5 +1,5 @@
 // EDM preconditioning output, EDM + MAE loss (forward + gradient seed), CFG and guide-network combines, Heun update,
-// fused AdamW+EMA, power-function EMA profiles (post-hoc EMA).
+// the rectified-flow loss, output and step front, fused AdamW+EMA, power-function EMA profiles (post-hoc EMA).
 #include <math.h>
 
 #include "common.cuh"
@@ -165,6 +165,94 @@ edm_loss_kernel(const float* __restrict__ F, const float* __restrict__ xin, cons
   if (threadIdx.x == 0) loss[b] = mask ? tot : tot / (static_cast<float>(gm.L) * gm.pd);
 }
 
+// Rectified flow (linear interpolant, velocity prediction; DESIGN §5): x_t = (1 - t) x + t eps, F unpatchified is the
+// velocity v^, the target is v = eps - x (formed from eps and x, not from x_t) and x^ = x_t - t v^ is the denoised
+// estimate that the MAE term reads.  edm_loss_kernel's structure: one block per sample, thread per token, kReg: the
+// token's velocity error and x_t live in registers (pd <= kMaxPD), otherwise later passes re-read F, x_t, eps and x.
+template <bool kReg>
+__global__ void __launch_bounds__(256)
+flow_loss_kernel(const float* __restrict__ F, const float* __restrict__ xt, const float* __restrict__ y,
+                 const float* __restrict__ eps, const float* __restrict__ tt, const float* __restrict__ mask,
+                 const float* __restrict__ gl, float mae_coef, float* __restrict__ loss, float* __restrict__ Dx,
+                 __nv_bfloat16* __restrict__ dF, PatchGeom gm) {
+  __shared__ float s_buf[32];
+  const int b = blockIdx.x;
+  const float tb = tt[b];
+  const float glb = gl ? gl[b] : 0.f;
+  float n_mask = 0.f;
+  if (mask) {
+    float cnt = 0.f;
+    for (int l = threadIdx.x; l < gm.L; l += blockDim.x) cnt += mask[static_cast<size_t>(b) * gm.L + l];
+    n_mask = block_sum(cnt, s_buf);
+  }
+  const float n_keep = static_cast<float>(gm.L) - n_mask;
+  float acc = 0.f;
+  for (int l = threadIdx.x; l < gm.L; l += blockDim.x) {
+    const float* f = F + (static_cast<size_t>(b) * gm.L + l) * gm.pd;
+    float ev[kReg ? kMaxPD : 1], xv[kReg ? kMaxPD : 1];
+    auto xat = [&](int j) -> float {
+      if constexpr (kReg) return xv[j];
+      else return xt[gm.pix(b, l, j)];
+    };
+    auto eat = [&](int j) -> float {   // v^ - v
+      if constexpr (kReg) return ev[j];
+      else {
+        const size_t px = gm.pix(b, l, j);
+        return f[j] - (eps[px] - y[px]);
+      }
+    };
+    auto dat = [&](int j) -> float { return __fmaf_rn(-tb, f[j], xat(j)); };   // x^ = x_t - t v^
+    float se = 0.f, sx = 0.f;
+    for (int j = 0; j < gm.pd; ++j) {
+      const size_t px = gm.pix(b, l, j);
+      const float xi = xt[px];
+      const float e = f[j] - (eps[px] - y[px]);
+      if (Dx) Dx[px] = __fmaf_rn(-tb, f[j], xi);
+      if constexpr (kReg) ev[j] = e, xv[j] = xi;
+      se += e * e, sx += xi;
+    }
+    const float inv_pd = 1.f / gm.pd;
+    if (!mask) {
+      acc += se;  // mean over all elements of the sample, applied below
+      if (dF) {
+        const float k = glb * 2.f / (static_cast<float>(gm.L) * gm.pd);
+        for (int j = 0; j < gm.pd; ++j)
+          dF[(static_cast<size_t>(b) * gm.L + l) * gm.pd + j] = __float2bfloat16_rn(k * eat(j));
+      }
+    } else {
+      const float mk = mask[static_cast<size_t>(b) * gm.L + l];
+      float contrib = (1.f - mk) * se * inv_pd / n_keep;
+      const float k_v = glb * (1.f - mk) / n_keep * 2.f * inv_pd;
+      float k_mae = 0.f, mu = 0.f, rstd = 0.f;
+      if (mae_coef > 0.f && mk != 0.f) {
+        // MaskDiT's MAE term with D replaced by x^: target = per-patch normalised x_t, unbiased variance
+        mu = sx * inv_pd;
+        float var = 0.f;
+        for (int j = 0; j < gm.pd; ++j) var += (xat(j) - mu) * (xat(j) - mu);
+        var /= static_cast<float>(gm.pd - 1);
+        rstd = rsqrtf(var + 1e-6f);
+        float sm = 0.f;
+        for (int j = 0; j < gm.pd; ++j) {
+          const float e = dat(j) - (xat(j) - mu) * rstd;
+          sm += e * e;
+        }
+        contrib += mae_coef * mk * sm * inv_pd / n_mask;
+        k_mae = -tb * glb * mae_coef * mk / n_mask * 2.f * inv_pd;   // d x^ / d v^ = -t
+      }
+      acc += contrib;
+      if (dF) {
+        for (int j = 0; j < gm.pd; ++j) {
+          float gval = k_v * eat(j);
+          if (k_mae != 0.f) gval += k_mae * (dat(j) - (xat(j) - mu) * rstd);
+          dF[(static_cast<size_t>(b) * gm.L + l) * gm.pd + j] = __float2bfloat16_rn(gval);
+        }
+      }
+    }
+  }
+  const float tot = block_sum(acc, s_buf);
+  if (threadIdx.x == 0) loss[b] = mask ? tot : tot / (static_cast<float>(gm.L) * gm.pd);
+}
+
 // u(sigma_b) alone, one block of 256 threads per sample: the loss kernel's arithmetic, so the same bits.
 __global__ void __launch_bounds__(256) logvar_kernel(const float* __restrict__ sigma, LogvarArgs lv) {
   __shared__ float s_buf[32];
@@ -224,6 +312,24 @@ __global__ void guided_precond_out_kernel(const float* __restrict__ Fm, PatchGeo
   const float fm = patch_at(Fm, gm, b, c, hh, ww), fg = patch_at(Fg, gg, b, c, hh, ww);
   const float f = fg + w * (fm - fg);
   Dx[idx] = c_skip * xin[idx] + c_out * f;
+}
+
+// Flow sampler output: out = unpatchify(Fu + s (Fc - Fu)) for CFG (cond rows first, uncond rows second), else
+// unpatchify(F).  One thread per output pixel.
+__global__ void flow_out_kernel(const float* __restrict__ F, float cfg_scale, int use_cfg, int B,
+                                float* __restrict__ out, PatchGeom gm) {
+  const long long idx = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  const int R = gm.R, C = gm.C;
+  if (idx >= static_cast<long long>(B) * C * R * R) return;
+  const int ww = static_cast<int>(idx % R), hh = static_cast<int>(idx / R % R);
+  const int c = static_cast<int>(idx / (static_cast<long long>(R) * R) % C);
+  const int b = static_cast<int>(idx / (static_cast<long long>(C) * R * R));
+  float f = patch_at(F, gm, b, c, hh, ww);
+  if (use_cfg) {
+    const float fu = patch_at(F, gm, b + B, c, hh, ww);
+    f = fu + cfg_scale * (f - fu);
+  }
+  out[idx] = f;
 }
 
 __global__ void precond_out_bwd_kernel(const float* __restrict__ gD, const float* __restrict__ sigma, float sd, int B,
@@ -618,6 +724,50 @@ step_front_kernel(const float* __restrict__ moments, const float* __restrict__ e
   }
 }
 
+
+// Flow step front: mdt_step_front with the flow time and interpolant in place of the sigma draw and noise injection.
+//   t = 1 / (1 + exp(-(P_mean + P_std * rnd)))                         x_t = (1 - t) y + t noise
+// Each product and sum is rounded separately (no contraction), so the fp32 formula evaluated op by op gives the same bits.
+__global__ void __launch_bounds__(256)
+flow_step_front_kernel(const float* __restrict__ moments, const float* __restrict__ eps, const float* __restrict__ rnd,
+                       const float* __restrict__ noise, const float* __restrict__ drop_u, float drop_prob, float sf,
+                       float P_mean, float P_std, float* __restrict__ y, float* __restrict__ xt, float* __restrict__ tt,
+                       float* __restrict__ labels, int B, int C, int plane4, int nc) {
+  const long long per = static_cast<long long>(C) * plane4;  // float4 groups per sample
+  const long long total = static_cast<long long>(B) * per;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int b = static_cast<int>(i / per);
+    const long long r = i - b * per;
+    const float a = __fadd_rn(__fmul_rn(rnd[b], P_std), P_mean);
+    const float t = __fdiv_rn(1.f, __fadd_rn(1.f, expf(-a)));
+    const float s = __fsub_rn(1.f, t);
+    const float4* mom = reinterpret_cast<const float4*>(moments) + static_cast<long long>(b) * 2 * per;
+    const float4 mu = mom[r], lv = mom[per + r];
+    const float4 e = reinterpret_cast<const float4*>(eps)[i], nz = reinterpret_cast<const float4*>(noise)[i];
+    float4 o, on;
+    o.x = sf * (mu.x + expf(0.5f * fminf(fmaxf(lv.x, -30.f), 20.f)) * e.x);
+    o.y = sf * (mu.y + expf(0.5f * fminf(fmaxf(lv.y, -30.f), 20.f)) * e.y);
+    o.z = sf * (mu.z + expf(0.5f * fminf(fmaxf(lv.z, -30.f), 20.f)) * e.z);
+    o.w = sf * (mu.w + expf(0.5f * fminf(fmaxf(lv.w, -30.f), 20.f)) * e.w);
+    on.x = __fadd_rn(__fmul_rn(s, o.x), __fmul_rn(t, nz.x));
+    on.y = __fadd_rn(__fmul_rn(s, o.y), __fmul_rn(t, nz.y));
+    on.z = __fadd_rn(__fmul_rn(s, o.z), __fmul_rn(t, nz.z));
+    on.w = __fadd_rn(__fmul_rn(s, o.w), __fmul_rn(t, nz.w));
+    reinterpret_cast<float4*>(y)[i] = o;
+    reinterpret_cast<float4*>(xt)[i] = on;
+    if (r == 0) tt[b] = t;
+  }
+  if (labels && drop_u) {
+    const long long nl = static_cast<long long>(B) * nc;
+    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < nl;
+         i += static_cast<long long>(gridDim.x) * blockDim.x) {
+      const int b = static_cast<int>(i / nc);
+      if (!(drop_u[b] >= drop_prob)) labels[i] = 0.f;
+    }
+  }
+}
+
 }  // namespace mdt
 
 using namespace mdt;
@@ -708,6 +858,29 @@ int mdt_guided_precond_out(const float* F_main, int p_main, const float* F_guide
   const long long n = static_cast<long long>(B) * C * R * R;
   guided_precond_out_kernel<<<static_cast<int>((n + 255) / 256), 256, 0, S(stream)>>>(F_main, gm, F_guide, gg, xin,
                                                                                        sigma, sigma_data, w, B, Dx);
+  return launch_status();
+}
+
+int mdt_flow_loss(const float* F, const float* xt, const float* y, const float* eps, const float* t, const float* mask,
+                  const float* gl, float mae_coef, float* loss, float* x_hat, void* dF_bf16, int B, int C, int R, int p,
+                  void* stream) {
+  if (!F || !xt || !y || !eps || !t || !loss || B <= 0) return MDT_ERR_ARG;
+  if (dF_bf16 && !gl) return MDT_ERR_ARG;
+  PatchGeom gm;
+  if (int rc = make_geom(&gm, C, R, p)) return rc;
+  auto kern = gm.pd <= kMaxPD ? flow_loss_kernel<true> : flow_loss_kernel<false>;
+  kern<<<B, 256, 0, S(stream)>>>(F, xt, y, eps, t, mask, gl, mae_coef, loss, x_hat,
+                                 static_cast<__nv_bfloat16*>(dF_bf16), gm);
+  return launch_status();
+}
+
+int mdt_flow_cfg_out(const float* F, int use_cfg, float cfg_scale, float* out, int B, int C, int R, int p,
+                     void* stream) {
+  if (!F || !out || B <= 0 || (use_cfg && !isfinite(cfg_scale))) return MDT_ERR_ARG;
+  PatchGeom gm;
+  if (int rc = make_geom(&gm, C, R, p)) return rc;
+  const long long n = static_cast<long long>(B) * C * R * R;
+  flow_out_kernel<<<static_cast<int>((n + 255) / 256), 256, 0, S(stream)>>>(F, cfg_scale, use_cfg != 0, B, out, gm);
   return launch_status();
 }
 
@@ -967,6 +1140,25 @@ int mdt_step_front(const float* moments, const float* eps, const float* rnd_norm
   step_front_kernel<<<static_cast<int>(blocks), 256, 0, S(stream)>>>(moments, eps, rnd_normal, noise_unit, drop_u,
                                                                      drop_prob, scale_factor, P_mean, P_std, y, yn,
                                                                      sigma, labels, B, C, R * R / 4, num_classes);
+  return launch_status();
+}
+
+
+int mdt_flow_step_front(const float* moments, const float* eps, const float* rnd_normal, const float* noise_unit,
+                        const float* drop_u, float drop_prob, float scale_factor, float P_mean, float P_std, float* y,
+                        float* xt, float* t, float* labels, int B, int C, int R, int num_classes, void* stream) {
+  if (!moments || !eps || !rnd_normal || !noise_unit || !y || !xt || !t || B <= 0 || C <= 0 || R <= 0)
+    return MDT_ERR_ARG;
+  if ((R * R) % 4) return MDT_ERR_ARG;
+  if ((reinterpret_cast<uintptr_t>(moments) | reinterpret_cast<uintptr_t>(eps) | reinterpret_cast<uintptr_t>(noise_unit) |
+       reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(xt)) & 15)
+    return MDT_ERR_ARG;
+  const long long total = static_cast<long long>(B) * C * (R * R / 4);
+  long long blocks = (total + 255) / 256;
+  if (blocks > kNumSMsDefault * 8) blocks = kNumSMsDefault * 8;
+  flow_step_front_kernel<<<static_cast<int>(blocks), 256, 0, S(stream)>>>(moments, eps, rnd_normal, noise_unit, drop_u,
+                                                                          drop_prob, scale_factor, P_mean, P_std, y,
+                                                                          xt, t, labels, B, C, R * R / 4, num_classes);
   return launch_status();
 }
 

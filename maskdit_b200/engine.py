@@ -374,6 +374,8 @@ class CEngine:
         self._h, self._L = h, L
         if getattr(cfg, "logvar_channels", 0):   # the learned loss weighting's tensors join the layout
             ops.check(L.mdt_model_set_logvar(h, cfg.logvar_channels), "mdt_model_set_logvar", 0)
+        if getattr(cfg, "precond", 0):   # flow: sigma carries t, c_in = 1, c_noise = t
+            ops.check(L.mdt_model_set_precond(h, cfg.precond), "mdt_model_set_precond", 0)
         self.NA = L.mdt_model_mod_width(h)   # width of the modulation vector = rows of the adaLN weight matrix
         # Activation recomputation (`mdt_model_set_recompute`) of the training pass.  `recompute` None: automatic, i.e.
         # nothing is recomputed unless the workspace allocation runs out of memory, then the smallest count that fits

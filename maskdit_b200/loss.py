@@ -1,4 +1,4 @@
-"""EDM training loss (reference: train_utils/loss.py) on the H100 engine.
+"""EDM training loss (reference: train_utils/loss.py) on the H100 engine, and the rectified-flow loss (`FlowLoss`).
 
 `Losses['edm']` has the reference's constructor and call signature.  When `net` is a `maskdit_b200.EDMPrecond`
 (bare, or wrapped in anything exposing `.module` like DDP / `DataParallelB200`), the loss runs fused:
@@ -15,7 +15,7 @@ from __future__ import annotations
 import torch
 
 from . import ops
-from .maskdit import EDMPrecond
+from .maskdit import EDMPrecond, FlowPrecond
 
 
 def _unwrap(net):
@@ -140,8 +140,10 @@ class EDMLoss:
 
     def _net(self, net, dev):
         raw = _unwrap(net)
-        if not isinstance(raw, EDMPrecond):
-            raise TypeError("maskdit_b200.Losses['edm'] drives a maskdit_b200.EDMPrecond network")
+        if not isinstance(raw, EDMPrecond) or isinstance(raw, FlowPrecond):
+            raise TypeError("maskdit_b200.Losses['edm'] drives a maskdit_b200.EDMPrecond network"
+                            + (" (this one is a FlowPrecond: use Losses['flow'])" if isinstance(raw, FlowPrecond)
+                               else ""))
         raw._ready(dev)
         return raw
 
@@ -170,4 +172,107 @@ class EDMLoss:
         return loss
 
 
-Losses = {"edm": EDMLoss}
+class _FusedFlowLossFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, anchor, net, xt, y, eps, t, labels, mask_dict, mae_coef):
+        Fo, saved = net._engine.forward(xt, t, labels, mask_dict, save=True)
+        mask = mask_dict["mask"] if mask_dict is not None else None
+        p = net.model.patch_size
+        loss, _, _ = ops.flow_loss(Fo, xt, y, eps, t, mask, None, mae_coef, p, want_dF=False)
+        ctx.net, ctx.saved = net, saved
+        ctx.args = (Fo, xt, y, eps, t, mask, mae_coef, p)
+        return loss
+
+    @staticmethod
+    def backward(ctx, gl):
+        net = ctx.net
+        Fo, xt, y, eps, t, mask, mae_coef, p = ctx.args
+        _, _, dF = ops.flow_loss(Fo, xt, y, eps, t, mask, gl.contiguous().float(), mae_coef, p, want_dF=True)
+        net._run_backward(ctx.saved, dF.view(-1, dF.shape[-1]))
+        ctx.saved = ctx.args = None
+        return (torch.zeros(1, device=gl.device),) + (None,) * 8
+
+
+class FlowLoss:
+    """Rectified-flow training loss of a `FlowPrecond` (DESIGN §5), with `EDMLoss`'s constructor style and call
+    signature.  t = sigmoid(P_mean + P_std n) (logit-normal) with n drawn where EDMLoss draws its `rnd_normal`,
+    x_t = (1 - t) x + t eps, and per sample: the mean over kept patches of the per-patch mean of (v^ - v)^2, v = eps - x,
+    plus mae_coef times MaskDiT's MAE term on the removed patches with D replaced by x^ = x_t - t v^; without a mask
+    mean((v^ - v)^2).  Forward, loss and gradient seed run fused as in `EDMLoss`; the draws are made in EDMLoss's order.
+    `last_edm_loss` holds the per-sample loss of the last call (for the training log)."""
+
+    def __init__(self, P_mean=0.0, P_std=1.0):
+        self.P_mean, self.P_std = P_mean, P_std
+
+    def _randn(self, shape, device):
+        return torch.randn(shape, device=device)
+
+    def _rand(self, shape, device):
+        return torch.rand(shape, device=device)
+
+    def __call__(self, net, images, labels=None, mask_ratio=0, mae_loss_coef=0, feat=None, augment_pipe=None):
+        if feat is not None or augment_pipe is not None:
+            raise NotImplementedError("feat / augment_pipe are not part of the MaskDiT latent training path")
+        raw = self._net(net, images.device)
+        B = images.shape[0]
+        x = images.contiguous().float()
+        rnd = self._randn([B, 1, 1, 1], images.device)
+        t4 = 1.0 / (1.0 + torch.exp(-(rnd * self.P_std + self.P_mean)))
+        eps = self._randn(tuple(x.shape), images.device).contiguous()
+        xt = ((1.0 - t4) * x + t4 * eps).contiguous()
+        return self._finish(raw, x, xt, eps, t4.reshape(B).contiguous(), labels, mask_ratio, mae_loss_coef)
+
+    def from_moments(self, net, moments, labels=None, mask_ratio=0, mae_loss_coef=0, class_dropout_prob=0.0,
+                     scale_factor=0.18215, eps=None, drop_u=None):
+        """`EDMLoss.from_moments` with the flow step front (`ops.flow_step_front`): latent, label dropout, t draw and
+        x_t in one launch, the same draws in the same order, `eps` / `drop_u` as there."""
+        dev = moments.device
+        raw = self._net(net, dev)
+        B, C2, R, _ = moments.shape
+        moments = moments.contiguous().float()
+        if eps is None:
+            eps = self._randn((B, C2 // 2, R, R), dev)
+        if class_dropout_prob > 0 and labels is not None:
+            if drop_u is None:
+                drop_u = self._rand((B, 1), dev).reshape(B)
+            drop_u = drop_u.contiguous()
+            if labels.dtype != torch.float32 or not labels.is_contiguous():
+                labels = labels.contiguous().float()
+        else:
+            drop_u = None
+        rnd_normal = self._randn([B, 1, 1, 1], dev).reshape(B).contiguous()
+        noise = self._randn((B, C2 // 2, R, R), dev).contiguous()
+        x, xt, t = ops.flow_step_front(moments, eps, rnd_normal, noise, labels, drop_u, float(class_dropout_prob),
+                                       scale_factor, self.P_mean, self.P_std)
+        return self._finish(raw, x, xt, noise, t, labels, mask_ratio, mae_loss_coef)
+
+    def _net(self, net, dev):
+        raw = _unwrap(net)
+        if not isinstance(raw, FlowPrecond):
+            raise TypeError("maskdit_b200.Losses['flow'] drives a maskdit_b200.FlowPrecond network"
+                            + (" (this one is an EDMPrecond: use Losses['edm'])" if isinstance(raw, EDMPrecond)
+                               else ""))
+        raw._ready(dev)
+        return raw
+
+    def _finish(self, raw, x, xt, eps, t, labels, mask_ratio, mae_loss_coef):
+        dev, B = x.device, x.shape[0]
+        _, _, lab = raw._norm_inputs(x, t, labels)
+        md = None
+        if mask_ratio > 0:
+            assert raw.training, "masked loss needs net.train()"
+            L = raw.model.num_patches
+            md = ops.mask_indices(self._rand((B, L), dev), int(L * (1 - mask_ratio)))
+        coef = float(mae_loss_coef) if (mask_ratio > 0 and mae_loss_coef > 0) else 0.0
+        if torch.is_grad_enabled():
+            loss = _FusedFlowLossFn.apply(raw._anchor, raw, xt, x, eps, t, lab, md, coef)
+        else:
+            Fo, _ = raw._engine.forward(xt, t, lab, md, save=False)
+            loss, _, _ = ops.flow_loss(Fo, xt, x, eps, t, md["mask"] if md else None, None, coef,
+                                       raw.model.patch_size, want_dF=False)
+        self.last_mask_dict = md
+        self.last_edm_loss = loss
+        return loss
+
+
+Losses = {"edm": EDMLoss, "flow": FlowLoss}

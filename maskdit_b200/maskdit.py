@@ -2,7 +2,7 @@
 
 Exports the same registries the reference's entry points consume (SURVEY.md §8b):
     DiT_models      name -> constructor            (models/maskdit.py:709-715)
-    Precond_models  {'edm': EDMPrecond}            (models/maskdit.py:779-781)
+    Precond_models  {'edm': EDMPrecond}            (models/maskdit.py:779-781), plus 'flow': FlowPrecond
 `EDMPrecond` is an `nn.Module` with the reference's constructor signature, attributes and state-dict key set
 (378 entries for XL/2), so `train.py`/`generate.py`-style drivers, `deepcopy` (EMA), `load_state_dict` of reference
 checkpoints and the reference's own `EDMLoss`/`edm_sampler` work against it unchanged.  Its arithmetic is the
@@ -189,6 +189,8 @@ class EDMPrecond(nn.Module):
     at the optimum exp(u(sigma)) is the expected E at sigma.  The three tensors are registered after `model.*`, so the
     reference's parameters keep their positions.  0 (the default): none of this exists."""
 
+    PRECOND = 0   # the C handle's precondition kind (mdt_model_set_precond): MDT_PRECOND_EDM
+
     def __init__(self, img_resolution, img_channels, num_classes=0, sigma_min=0, sigma_max=float("inf"),
                  sigma_data=0.5, model_type="DiT-B/2", logvar_channels=0, **model_kwargs):
         super().__init__()
@@ -228,6 +230,7 @@ class EDMPrecond(nn.Module):
         c.img_resolution, c.img_channels = self.img_resolution, self.img_channels
         c.patch_dim = m.patch_size * m.patch_size * m.out_channels
         c.logvar_channels = self.logvar_channels
+        c.precond = self.PRECOND
         return c
 
     def _params(self):
@@ -278,7 +281,7 @@ class EDMPrecond(nn.Module):
         self._engine.backward(saved, dF16)
 
     def __deepcopy__(self, memo):
-        new = EDMPrecond(**copy.deepcopy(self._ctor))
+        new = type(self)(**copy.deepcopy(self._ctor))
         dev = next(self.parameters()).device
         new.to(dev)
         with torch.no_grad():   # every parameter, the frozen logvar features included
@@ -449,7 +452,88 @@ class EDMPrecond(nn.Module):
             return fn(xf, sig, lab, w, guide).to(x.dtype)
 
 
-Precond_models = {"edm": EDMPrecond}
+class FlowPrecond(EDMPrecond):
+    """The DiT trained with the rectified-flow objective (linear interpolant, velocity prediction; SiT, Ma et al. 2024)
+    on the same engine, flat store, state-dict keys and CUDA-graph eval path as `EDMPrecond`.
+
+    t in [0, 1], t = 0 is data and t = 1 is noise: x_t = (1 - t) x + t eps.  The network reads x_t unscaled (c_in = 1)
+    with c_noise = t in the unchanged timestep embedder, and `forward(x_t, t, class_labels, cfg_scale)` returns
+    {'x': v^ [, 'mask': mask]}: the unpatchified network output is the velocity, whose target is v = eps - x; the
+    denoised estimate is x_t - t v^.  `Losses['flow']` trains it and `flow_sampler` integrates dx/dt = v^ from t = 1 to 0.
+    There is no autograd path through `forward` (train through `Losses['flow']`), no autoguidance and no learned loss
+    weighting (defined over sigma).  `sigma_data`, `sigma_min` and `sigma_max` are kept for the shared constructor and
+    are not read."""
+
+    PRECOND = 1   # MDT_PRECOND_FLOW
+
+    def __init__(self, img_resolution, img_channels, num_classes=0, sigma_min=0, sigma_max=float("inf"),
+                 sigma_data=0.5, model_type="DiT-B/2", logvar_channels=0, **model_kwargs):
+        if logvar_channels:
+            raise ValueError("the learned loss weighting (logvar_channels) is defined over the EDM noise level sigma: "
+                             "flow networks do not have it")
+        super().__init__(img_resolution, img_channels, num_classes, sigma_min, sigma_max, sigma_data, model_type, 0,
+                         **model_kwargs)
+
+    def _eval_eager(self, xf, t, lab, cfg_scale, guide=None):
+        if guide is not None:
+            raise ValueError("autoguidance is not available for flow networks")
+        B, p = xf.shape[0], self.model.patch_size
+        C, R = self.img_channels, self.img_resolution
+        if cfg_scale is not None:
+            # forward_with_cfg (models/maskdit.py:559-587): one eval pass at batch 2B, guidance fused in the output
+            Fo, _ = self._engine.forward(torch.cat([xf, xf], 0), torch.cat([t, t], 0),
+                                         torch.cat([lab, torch.zeros_like(lab)], 0), None, save=False)
+            return ops.flow_cfg_out(Fo, B, C, R, p, float(cfg_scale))
+        Fo, _ = self._engine.forward(xf, t, lab, None, save=False)
+        return ops.flow_cfg_out(Fo, B, C, R, p)
+
+    def forward(self, x, t, class_labels=None, cfg_scale=None, **model_kwargs):
+        """{'x': v^ [, 'mask': mask]} of x = x_t at flow time t (a scalar or [B]); the call contract of
+        `EDMPrecond.forward` with t in place of sigma."""
+        mask_ratio = model_kwargs.pop("mask_ratio", 0)
+        mask_dict = model_kwargs.pop("mask_dict", None)
+        feat = model_kwargs.pop("feat", None)
+        if feat is not None or model_kwargs:
+            raise NotImplementedError(f"unsupported arguments: feat / {list(model_kwargs)}")
+        self._ready(x.device)
+        xf, tt, lab = self._norm_inputs(x, t, class_labels)
+        B, p = xf.shape[0], self.model.patch_size
+        out = {}
+        use_graph = not self.training and os.environ.get("MDT_CUDA_GRAPH", "1") != "0" \
+            and not torch.cuda.is_current_stream_capturing()
+        if cfg_scale is not None:
+            assert self.num_classes and lab is not None
+            with torch.no_grad():
+                fn = self._eval_graphed if use_graph else self._eval_eager
+                out["x"] = fn(xf, tt, lab, cfg_scale).to(x.dtype)
+            return out
+        if torch.is_grad_enabled() and any(q.requires_grad for q in self.parameters()):
+            raise RuntimeError("FlowPrecond.forward has no autograd path: train through Losses['flow'] and evaluate "
+                               "under torch.no_grad()")
+        md = None
+        if mask_ratio > 0:
+            L = self.model.num_patches
+            if mask_dict is None:
+                noise = torch.rand(B, L, device=x.device)  # get_mask, models/maskdit.py:102
+                mask_dict = ops.mask_indices(noise, int(L * (1 - mask_ratio)))
+            out["mask"] = mask_dict["mask"]
+            if self.training:
+                md = mask_dict
+        if md is None and use_graph:
+            out["x"] = self._eval_graphed(xf, tt, lab, None).to(x.dtype)
+        else:
+            Fo, _ = self._engine.forward(xf, tt, lab, md, save=False)
+            out["x"] = ops.flow_cfg_out(Fo, B, self.img_channels, self.img_resolution, p).to(x.dtype)
+        return out
+
+    def check_guide(self, guide):
+        raise ValueError("autoguidance is not available for flow networks")
+
+    def forward_guided(self, x, sigma, class_labels, guide, guidance):
+        raise ValueError("autoguidance is not available for flow networks")
+
+
+Precond_models = {"edm": EDMPrecond, "flow": FlowPrecond}
 
 
 def eval_state_dict(net, sd):

@@ -59,6 +59,14 @@ def timestep_freq(sigma, dim=256):
     return out
 
 
+def flow_timestep_freq(t, dim=256):
+    """The timestep embedding's frequencies on c_noise = t (mdt_flow_timestep_freq)."""
+    _c(t, f32)
+    out = torch.empty(t.numel(), dim, dtype=bf16, device=t.device)
+    check(lib().mdt_flow_timestep_freq(ptr(t), t.numel(), dim, ptr(out), stream_ptr()), "mdt_flow_timestep_freq")
+    return out
+
+
 def silu(a, b=None, want_sum=False):
     _c(a, f32), _c(b, f32)
     out = torch.empty(a.shape, dtype=bf16, device=a.device)
@@ -224,6 +232,45 @@ def step_front(moments, eps, rnd_normal, noise_unit, labels=None, drop_u=None, d
                                scale_factor, P_mean, P_std, ptr(y), ptr(yn), ptr(sigma),
                                ptr(labels) if drop_u is not None else 0, B, C, R, nc, stream_ptr()), "mdt_step_front")
     return y, yn, sigma
+
+
+def flow_step_front(moments, eps, rnd_normal, noise_unit, labels=None, drop_u=None, drop_prob=0.0,
+                    scale_factor=0.18215, P_mean=0.0, P_std=1.0):
+    """`step_front` for rectified flow: moments -> latent x, label dropout, t = sigmoid(P_mean + P_std rnd_normal),
+    x_t = (1 - t) x + t noise_unit: one launch.  Returns (x, x_t, t)."""
+    _c(moments, f32), _c(eps, f32), _c(rnd_normal, f32), _c(noise_unit, f32), _c(labels, f32), _c(drop_u, f32)
+    B, C2, R, _ = moments.shape
+    C = C2 // 2
+    y = torch.empty(B, C, R, R, dtype=f32, device=moments.device)
+    xt = torch.empty_like(y)
+    t = torch.empty(B, dtype=f32, device=moments.device)
+    nc = labels.shape[1] if labels is not None else 0
+    check(lib().mdt_flow_step_front(ptr(moments), ptr(eps), ptr(rnd_normal), ptr(noise_unit), ptr(drop_u), drop_prob,
+                                    scale_factor, P_mean, P_std, ptr(y), ptr(xt), ptr(t),
+                                    ptr(labels) if drop_u is not None else 0, B, C, R, nc, stream_ptr()),
+          "mdt_flow_step_front")
+    return y, xt, t
+
+
+def flow_loss(F, xt, y, eps, t, mask, gl, mae_coef, p, want_xhat=False, want_dF=True):
+    """Rectified-flow loss of the velocity F (mdt_flow_loss).  Returns (loss [B], x_hat or None, dF bf16 or None)."""
+    B, C, R, _ = xt.shape
+    loss = torch.empty(B, dtype=f32, device=xt.device)
+    xh = torch.empty_like(xt) if want_xhat else None
+    dF = torch.empty(F.shape, dtype=bf16, device=xt.device) if want_dF else None
+    check(lib().mdt_flow_loss(ptr(F), ptr(xt), ptr(y), ptr(eps), ptr(t), ptr(mask), ptr(gl), mae_coef, ptr(loss),
+                              ptr(xh), ptr(dF), B, C, R, p, stream_ptr()), "mdt_flow_loss")
+    return loss, xh, dF
+
+
+def flow_cfg_out(F, B, C, R, p, cfg_scale=None):
+    """The velocity [B, C, R, R]: unpatchify(F), or with `cfg_scale` the CFG combine Fu + s (Fc - Fu) of F's two
+    halves (cond rows first)."""
+    out = torch.empty(B, C, R, R, dtype=f32, device=F.device)
+    use = cfg_scale is not None
+    check(lib().mdt_flow_cfg_out(ptr(F), int(use), float(cfg_scale) if use else 0.0, ptr(out), B, C, R, p,
+                                 stream_ptr()), "mdt_flow_cfg_out")
+    return out
 
 
 def edm_precond_out(F, xin, sigma, sigma_data, p):

@@ -5,7 +5,7 @@ consumed once per step even when S_churn = 0).  With a `maskdit_b200.EDMPrecond`
 eval-mode engine pass at batch 2B with the classifier-free-guidance combine fused into the output kernel, and the
 fp64 Euler/Heun state updates are single fused kernels.  Both samplers can instead guide with a second network
 (`guide_net`, `guidance`: autoguidance) and apply either guidance only inside a noise-level interval
-(`guidance_interval`); see `_denoiser`.
+(`guidance_interval`); see `_denoiser`.  `flow_sampler` integrates a rectified-flow network's velocity instead.
 """
 from __future__ import annotations
 
@@ -84,6 +84,42 @@ def edm_sampler(net, latents, class_labels=None, cfg_scale=None, feat=None, rand
             den = denoise(x32, t_next).float().contiguous()
             ops.heun_update(1, x_hat, den, d_cur, x_next, x32, t_hat, t_next)      # 2nd-order correction (:61-64)
     return x_next
+
+
+def flow_grid(num_steps):
+    """The flow sampler's time grid: num_steps + 1 uniform points from t = 1 (noise) to t = 0 (data), fp64."""
+    if num_steps < 1:
+        raise ValueError(f"num_steps must be at least 1, got {num_steps}")
+    return 1.0 - np.arange(num_steps + 1, dtype=np.float64) / num_steps
+
+
+@torch.no_grad()
+def flow_sampler(net, latents, class_labels=None, cfg_scale=None, num_steps=50, solver="heun",
+                 guidance_interval=None):
+    """ODE sampler of a rectified-flow network (`FlowPrecond`): integrates dx/dt = v^(x, t) from x(1) = `latents` to
+    t = 0 on `flow_grid(num_steps)`.  The state is fp64 and every update is one `mdt_lincomb_f64` launch that also
+    writes the next fp32 network input.  solver 'euler': num_steps evaluations; 'heun': Heun's second-order step with
+    an Euler last step (the corrector would evaluate at t = 0), 2 num_steps - 1 evaluations.  `cfg_scale` and
+    `guidance_interval` = (lo, hi), which applies CFG only where lo < t <= hi, are those of `edm_sampler` with t in
+    place of sigma."""
+    if solver not in ("euler", "heun"):
+        raise ValueError(f"solver must be 'euler' or 'heun', got {solver!r}")
+    denoise = _denoiser(net, class_labels, cfg_scale, None, None, None, guidance_interval)
+    t = flow_grid(num_steps)
+    x = latents.to(torch.float64).contiguous().clone()
+    xin = x.float().contiguous()
+    for k in range(num_steps):
+        t_cur, t_next = float(t[k]), float(t[k + 1])
+        h = t_next - t_cur
+        v = denoise(xin, t_cur).float().contiguous()
+        if solver == "euler" or k == num_steps - 1:
+            ops.lincomb_f64(1.0, x, 0.0, None, h, v, out=x, out_f32=xin)                 # x + h v
+            continue
+        ops.lincomb_f64(1.0, x, 0.0, None, h, v, out_f32=xin)                           # predictor input x + h v
+        ops.lincomb_f64(1.0, x, 0.0, None, 0.5 * h, v, out=x)                           # x + h/2 v
+        v2 = denoise(xin, t_next).float().contiguous()
+        ops.lincomb_f64(1.0, x, 0.0, None, 0.5 * h, v2, out=x, out_f32=xin)             # ... + h/2 v'
+    return x
 
 
 class _Schedules:

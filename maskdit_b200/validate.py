@@ -1,5 +1,9 @@
 """Held-out denoising loss: a fixed estimate of the EDM training objective of the network the sampler runs.
 
+A rectified-flow network (`FlowPrecond`) is scored with its own objective at the levels
+`t_k = sigmoid(P_mean + P_std * z_k)` (P_mean 0, P_std 1), with the same per-item draws; its numbers are not comparable
+with an EDM network's, and the result says which objective was scored (`objective`: 'flow', levels under `t`).
+
 The training loss cannot be compared across a run: it is a one-batch estimate over random sigma draws, and it depends
 on the mask ratio, which a schedule such as the fine-tune's `cos4` changes every step.  This module scores a network on
 a fixed held-out set instead, with every draw fixed, so two checkpoints, two EMA widths or two runs scored with the same
@@ -30,6 +34,7 @@ import numpy as np
 import torch
 
 P_MEAN, P_STD = -1.2, 1.2
+FLOW_P_MEAN, FLOW_P_STD = 0.0, 1.0   # FlowLoss's logit-normal t
 SCALE_FACTOR = 0.18215
 
 
@@ -44,6 +49,11 @@ def level_normals(levels, dtype=np.float64):
 def sigma_levels(levels, P_mean=P_MEAN, P_std=P_STD):
     """sigma_k = exp(P_mean + P_std * z_k) in float64: quantiles of the training lognormal (K = 1: its median)."""
     return np.exp(P_mean + P_std * level_normals(levels))
+
+
+def t_levels(levels, P_mean=FLOW_P_MEAN, P_std=FLOW_P_STD):
+    """t_k = sigmoid(P_mean + P_std * z_k) in float64: quantiles of a flow network's logit-normal training t."""
+    return 1.0 / (1.0 + np.exp(-(P_mean + P_std * level_normals(levels))))
 
 
 def item_draws(seed, index, channels, resolution, levels):
@@ -105,12 +115,19 @@ class HeldOut:
 
 # ---- scoring ---------------------------------------------------------------------------------------------------------
 class CudaScorer:
-    """Per-row losses of a `maskdit_b200.EDMPrecond` in eval mode on its device: step front, eval forward, EDM loss."""
+    """Per-row losses of a `maskdit_b200.EDMPrecond` in eval mode on its device: step front, eval forward, EDM loss.
+    A `FlowPrecond` is scored with its own objective: the flow step front (t_k enters as `rnd_normal = z_k`, P_mean and
+    P_std default to FlowLoss's 0 and 1), the eval forward and the unmasked flow loss mean((v^ - v)^2)."""
 
-    def __init__(self, net, P_mean=P_MEAN, P_std=P_STD, scale_factor=SCALE_FACTOR):
+    def __init__(self, net, P_mean=None, P_std=None, scale_factor=SCALE_FACTOR):
         from .loss import _unwrap
-        from .maskdit import EDMPrecond
+        from .maskdit import EDMPrecond, FlowPrecond
         raw = _unwrap(net)
+        self.objective = "flow" if isinstance(raw, FlowPrecond) else "edm"
+        if P_mean is None:
+            P_mean = FLOW_P_MEAN if self.objective == "flow" else P_MEAN
+        if P_std is None:
+            P_std = FLOW_P_STD if self.objective == "flow" else P_STD
         if not isinstance(raw, EDMPrecond):
             raise TypeError("CudaScorer scores a maskdit_b200.EDMPrecond network")
         if raw.training:
@@ -126,6 +143,15 @@ class CudaScorer:
         net, dev = self.net, self.device
         net._ready(dev)                                   # the bf16 weight shadow follows the fp32 weights
         to = lambda t: None if t is None else t.to(dev, non_blocking=True).contiguous()  # noqa: E731
+        if self.objective == "flow":
+            with torch.no_grad():
+                x, xt, t = ops.flow_step_front(to(moments), to(eps), to(rnd_normal), to(noise), None, None, 0.0,
+                                               self.scale_factor, self.P_mean, self.P_std)
+                _, _, lab = net._norm_inputs(x, t, to(labels))
+                Fo, _ = net._engine.forward(xt, t, lab, None, save=False)
+                loss, _, _ = ops.flow_loss(Fo, xt, x, to(noise), t, None, None, 0.0, net.model.patch_size,
+                                           want_dF=False)
+            return loss
         with torch.no_grad():
             y, yn, sigma = ops.step_front(to(moments), to(eps), to(rnd_normal), to(noise), None, None, 0.0,
                                           self.scale_factor, self.P_mean, self.P_std)
@@ -191,16 +217,19 @@ def gather_items(local, count, group=None):
                       for r, p in enumerate(parts)])
 
 
-def summarize(per_item, P_mean=P_MEAN, P_std=P_STD):
+def summarize(per_item, P_mean=P_MEAN, P_std=P_STD, objective="edm"):
     """{sigma, per_level, mean, count, levels} of per-item losses [N, K]: per-level means of float64 sums taken
-    item by item in index order, and their mean over the levels."""
+    item by item in index order, and their mean over the levels.  objective 'flow': {t, ..., objective} instead, the
+    levels being `t_levels(K, P_mean, P_std)`."""
     a = per_item.double().numpy()
     N, K = a.shape
     if N == 0:
         raise ValueError("no items to summarize")
     per_level = np.cumsum(a, axis=0)[-1] / N             # sequential, in index order
-    return {"sigma": sigma_levels(K, P_mean, P_std).tolist(), "per_level": per_level.tolist(),
-            "mean": float(per_level.mean()), "count": N, "levels": K}
+    rest = {"per_level": per_level.tolist(), "mean": float(per_level.mean()), "count": N, "levels": K}
+    if objective == "flow":
+        return {"t": t_levels(K, P_mean, P_std).tolist(), **rest, "objective": "flow"}
+    return {"sigma": sigma_levels(K, P_mean, P_std).tolist(), **rest}
 
 
 def validate(net_or_scorer, held, levels=8, seed=0, batch=64, group=None):
@@ -219,7 +248,10 @@ def validate(net_or_scorer, held, levels=8, seed=0, batch=64, group=None):
         per_item = gather_items(score_items(scorer, held, lo, hi, levels, seed, batch), count, group)
     else:
         per_item = score_items(scorer, held, 0, count, levels, seed, batch)
-    res = summarize(per_item)
+    if getattr(scorer, "objective", "edm") == "flow":
+        res = summarize(per_item, scorer.P_mean, scorer.P_std, "flow")
+    else:
+        res = summarize(per_item)
     res["per_item"] = per_item
     return res
 

@@ -129,7 +129,8 @@ def val_line(step, res, logvar=None):
     """The validation log line (rank 0): the mean over levels, then each level's mean loss; with a learned loss
     weighting, `logvar` = the EMA's u(sigma_k) at the K validation levels."""
     from maskdit_b200.validate import format_levels
-    line = f"(step={step:07d}) Val Loss: {format_levels(res)} ({res['count']} items, EMA)"
+    what = "Val Loss (flow)" if res.get("objective") == "flow" else "Val Loss"   # the flow loss is on its own scale
+    line = f"(step={step:07d}) {what}: {format_levels(res)} ({res['count']} items, EMA)"
     if logvar is not None:
         line += ", Logvar: [" + " ".join(f"{float(v):.4f}" for v in logvar) + "]"
     return line

@@ -87,15 +87,19 @@ def main(argv=None):
         rows.append({"name": name, "mean": res["mean"], "per_level": res["per_level"]})
         if rank == 0:
             print(f"{name}: {format_levels(res)}", flush=True)
-        sigma = res["sigma"]
+        # a flow network is scored with the flow loss at flow times t: not comparable with EDM numbers
+        level_key = "t" if res.get("objective") == "flow" else "sigma"
+        sigma = res[level_key]
     best = min(rows, key=lambda r: r["mean"])
     if rank == 0:
-        print(f"best: {best['name']} {best['mean']:.5f} ({len(held)} items x {args.levels} levels, sigma "
+        what = "flow loss, " if level_key == "t" else ""
+        print(f"best: {best['name']} {best['mean']:.5f} ({what}{len(held)} items x {args.levels} levels, {level_key} "
               + " ".join(f"{s:.3g}" for s in sigma) + ")", flush=True)
         if args.json:
+            extra = {"objective": "flow"} if level_key == "t" else {}
             with open(args.json, "w") as f:
-                json.dump({"count": len(held), "levels": args.levels, "seed": args.seed, "sigma": sigma,
-                           "rows": rows, "best": best["name"]}, f, indent=1)
+                json.dump({"count": len(held), "levels": args.levels, "seed": args.seed, level_key: sigma,
+                           "rows": rows, "best": best["name"], **extra}, f, indent=1)
     if size > 1:
         torch.distributed.destroy_process_group()
     return rows
