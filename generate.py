@@ -16,7 +16,9 @@ EMA built by `posthoc_ema.reconstruct`) with `--guidance W` guides with a second
 geometry and classes (autoguidance; `--guide_config` when its architecture differs), and `--guidance_interval LO HI`
 applies CFG or the guide only at evaluations with LO < sigma <= HI.  A rectified-flow config (`model.precond: flow`)
 samples with `flow_sampler` (Heun on a uniform t grid, `--num_steps`, `--cfg_scale`, `--guidance_interval` on t) and
-refuses the ablation switches, `--S_churn` and autoguidance.  Class-unconditional configs sample with all-zero
+refuses the ablation switches, `--S_churn` and autoguidance.  `--consistency_sigmas S0 [S1 ...]` samples a
+consistency-tuned EDM network (train.py with `train.objective: ect`) with `consistency_sampler`, one evaluation per
+noise level, and refuses the ablation switches, `--S_churn` and flow configs.  Class-unconditional configs sample with all-zero
 label rows as the reference does (sample.py:261-264).
 """
 import argparse
@@ -28,7 +30,8 @@ import torch
 from maskdit_b200.config import build_net, load_config, parse_float_none, parse_int_list
 from maskdit_b200.maskdit import eval_state_dict
 from maskdit_b200 import ops
-from maskdit_b200.sampler import ablation_sampler, edm_sampler, flow_sampler, rank_seed_batches, write_png
+from maskdit_b200.sampler import (ablation_sampler, consistency_sampler, consistency_sigmas, edm_sampler, flow_sampler,
+                                  rank_seed_batches, write_png)
 
 
 class StackedRandomGenerator:
@@ -81,6 +84,9 @@ def build_parser():
                     help="guide weight w: D = D_guide + w (D_net - D_guide); 1 is the unguided network")
     ap.add_argument("--guidance_interval", type=float, nargs=2, default=None, metavar=("LO", "HI"),
                     help="apply the guidance (--cfg_scale or the guide) only at evaluations with LO < sigma <= HI")
+    ap.add_argument("--consistency_sigmas", type=float, nargs="+", default=None, metavar="SIGMA",
+                    help="sample a consistency-tuned network (train.objective: ect) at these strictly decreasing noise "
+                         "levels, one network evaluation each (e.g. 80, or 80 0.8)")
     return ap
 
 
@@ -106,6 +112,17 @@ def parse_args(argv=None):
             ap.error(f"--guidance_interval needs LO < HI, got {lo:g} {hi:g}")
         if not guide and args.cfg_scale is None:
             ap.error("--guidance_interval needs --cfg_scale or a guide network")
+    if args.consistency_sigmas is not None:
+        bad = [f"--{k}" for k in ("solver", "discretization", "schedule", "scaling") if getattr(args, k)]
+        if args.S_churn:
+            bad.append("--S_churn")
+        if bad:
+            ap.error(f"--consistency_sigmas samples with consistency_sampler: {', '.join(bad)} apply to the EDM "
+                     "samplers only")
+        try:
+            consistency_sigmas(args.consistency_sigmas)
+        except ValueError as e:
+            ap.error(f"--consistency_sigmas: {e}")
     return args
 
 
@@ -139,13 +156,16 @@ def guide_state_dict(args):
 def main(argv=None):
     args = parse_args(argv)
     cfg = load_config(args.config)
+    flow = cfg.model.precond == "flow"
+    if flow and args.consistency_sigmas is not None:
+        raise SystemExit("--consistency_sigmas samples a consistency-tuned EDM network, not a flow config "
+                         "(model.precond: flow)")
     rank, size = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     local = int(os.environ.get("LOCAL_RANK", 0))
     torch.cuda.set_device(local)
     device = torch.device("cuda", local)
     if size > 1:
         torch.distributed.init_process_group("nccl", device_id=device)
-    flow = cfg.model.precond == "flow"
     if flow:
         check_flow_args(args)
     net = build_net(cfg).to(device).eval()
@@ -184,7 +204,10 @@ def main(argv=None):
             labels[:, :] = 0
             labels[:, args.class_idx] = 1
         with torch.no_grad():
-            if flow:
+            if args.consistency_sigmas is not None:
+                z = consistency_sampler(net, latents.float(), labels.float(), cfg_scale=args.cfg_scale,
+                                        randn_like=rnd.randn_like, sigmas=args.consistency_sigmas, **gkw).float()
+            elif flow:
                 z = flow_sampler(net, latents.float(), labels.float(), cfg_scale=args.cfg_scale,
                                  num_steps=args.num_steps, **gkw).float()
             else:

@@ -253,6 +253,27 @@ int mdt_flow_step_front(const float* moments, const float* eps, const float* rnd
                         const float* drop_u, float drop_prob, float scale_factor, float P_mean, float P_std, float* y,
                         float* xt, float* t, float* labels, int B, int C, int R, int num_classes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Easy Consistency Tuning (ECT; Geng et al., ICLR 2025) of an EDM network f(x, s) = D(x; s) = c_skip(s) x + c_out(s) F.
+ * mdt_ect_step_front: mdt_step_front's latent and label dropout, then, each product and sum rounded separately,
+ *   t[b] = exp(P_std * rnd_normal[b] + P_mean) ; r[b] = t * max(0, 1 - qs[0] * (1 + k / (1 + exp(b_coef * t))))
+ *   xt = y + t noise_unit ; xr = y + r noise_unit ; sr[b] = r > 0 ? r : t  (the target forward's sigma)
+ *   qs: ONE fp32 word on the device, q^-(s+1) of the tuning stage s (a graph replay reads the current stage).
+ * mdt_ect_loss: Ft, Fr [B,L,p*p*C] f32 the student's (at xt, t) and the target's (at xr, sr) outputs with the same
+ *   kept tokens ; xt, xr, y [B,C,R,R] ; t, r [B].  D_t = c_skip(t) xt + c_out(t) F_t ; D_r = r > 0 ? c_skip(r) xr +
+ *   c_out(r) F_r : y (a select: F_r of an r = 0 row is never read into the result) ; delta = D_t - D_r.
+ *   S = (L / T) sum_{kept} delta^2 (T = L unmasked) ; loss[b] = (sqrt(S + c^2) - c) / (t - r) + mae_coef * M, M the
+ *   mdt_edm_loss MAE term on the removed patches with D = D_t (mask == NULL: M = 0).
+ *   dF_bf16 (optional, needs gl) = d(sum_b gl[b] loss[b]) / dF_t ; D_t (optional) [B,C,R,R] f32.
+ * ------------------------------------------------------------------------------------------------------------ */
+int mdt_ect_step_front(const float* moments, const float* eps, const float* rnd_normal, const float* noise_unit,
+                       const float* drop_u, float drop_prob, float scale_factor, float P_mean, float P_std,
+                       const float* qs, float k, float b_coef, float* y, float* xt, float* xr, float* sr, float* t,
+                       float* r, float* labels, int B, int C, int R, int num_classes, void* stream);
+int mdt_ect_loss(const float* Ft, const float* Fr, const float* xt, const float* xr, const float* y, const float* t,
+                 const float* r, const float* mask, const float* gl, float sigma_data, float c, float mae_coef,
+                 float* loss, float* D_t, void* dF_bf16, int B, int C, int R, int p, void* stream);
+
 /* D only (sampler / generic autograd path): Dx = c_skip*xin + c_out*unpatchify(F); and its backward
  * dF_bf16 = c_out * patchify(gD).                                                                            */
 int mdt_edm_precond_out(const float* F, const float* xin, const float* sigma, float sigma_data, float* Dx, int B,

@@ -84,3 +84,34 @@ def build_net(cfg: Node, **extra):
                                      model_type=m.model_type, use_decoder=m.use_decoder,
                                      mae_loss_coef=m.mae_loss_coef, pad_cls_token=m.pad_cls_token,
                                      logvar_channels=int(m.get("logvar_channels", 0) or 0), **extra)
+
+
+ECT_KEYS = ("stage_steps", "q", "k", "b", "P_mean", "P_std")
+
+
+def build_loss(cfg: Node):
+    """The training loss of a config: `Losses[model.precond]()` as train.py:137 builds it, or, with
+    `train.objective: ect`, Easy Consistency Tuning (`Losses['ect']`) of an EDM network with the `train.ect` block's
+    `stage_steps` (required), `q`, `k`, `b`, `P_mean` and `P_std`.  An absent `train.objective` is the precond's own
+    objective.  Raises ValueError for a combination that cannot train."""
+    from .loss import Losses
+    m, tr = cfg.model, cfg.get("train") or Node()
+    obj = tr.get("objective", None)
+    block = tr.get("ect", None)
+    if obj in (None, m.precond):
+        if block is not None:
+            raise ValueError("train.ect configures consistency tuning: set train.objective: ect")
+        return Losses[m.precond]()
+    if obj != "ect":
+        raise ValueError(f"unknown train.objective {obj!r} (the precond's own, or 'ect')")
+    if m.precond != "edm":
+        raise ValueError(f"train.objective: ect tunes an EDM network, not model.precond: {m.precond}")
+    if int(m.get("logvar_channels", 0) or 0):
+        raise ValueError("train.objective: ect does not train a learned loss weighting: drop model.logvar_channels")
+    block = dict(block or {})
+    unknown = sorted(set(block) - set(ECT_KEYS))
+    if unknown:
+        raise ValueError(f"unknown train.ect keys {unknown} (known: {list(ECT_KEYS)})")
+    if block.get("stage_steps") is None:
+        raise ValueError("train.objective: ect needs train.ect.stage_steps (steps per tuning stage)")
+    return Losses["ect"](**block)

@@ -253,6 +253,106 @@ flow_loss_kernel(const float* __restrict__ F, const float* __restrict__ xt, cons
   if (threadIdx.x == 0) loss[b] = mask ? tot : tot / (static_cast<float>(gm.L) * gm.pd);
 }
 
+// Easy Consistency Tuning (DESIGN §5): the student D_t = c_skip(t) x_t + c_out(t) F_t against the no-gradient target
+// D_r = c_skip(r) x_r + c_out(r) F_r (r > 0) or the clean latent y (r = 0, selected, so F_r of such a row never enters).
+// Per sample: S = (L / T) sum_kept delta^2, loss = (sqrt(S + c^2) - c) / (t - r) + mae_coef M; the pseudo-Huber term is
+// formed as S / (sqrt(S + c^2) + c), which has no cancellation when S << c^2 (a small stage gap).  edm_loss_kernel's
+// structure: one block per sample, thread per token, fixed block sums.  S must be complete before any gradient seed,
+// so the seed is a second pass over the tokens that re-reads its operands (every patch size, pd 16 / 64 / 256).
+__global__ void __launch_bounds__(256)
+ect_loss_kernel(const float* __restrict__ Ft, const float* __restrict__ Fr, const float* __restrict__ xt,
+                const float* __restrict__ xr, const float* __restrict__ y, const float* __restrict__ tt,
+                const float* __restrict__ rr, const float* __restrict__ mask, const float* __restrict__ gl, float sd,
+                float c_h, float mae_coef, float* __restrict__ loss, float* __restrict__ Dx,
+                __nv_bfloat16* __restrict__ dF, PatchGeom gm) {
+  __shared__ float s_buf[32];
+  const int b = blockIdx.x;
+  const float t = tt[b], r = rr[b];
+  const bool has_r = r > 0.f;
+  const float den_t = t * t + sd * sd, den_r = r * r + sd * sd;
+  const float cs_t = sd * sd / den_t, co_t = t * sd * rsqrtf(den_t);
+  // r > 0: delta = c_skip(t) (x_t - x_r) + dcs x_r + c_out(t) (F_t - F_r) + dco F_r, where dcs = c_skip(t) - c_skip(r)
+  // and dco = c_out(t) - c_out(r) are formed from t - r (exact in fp32 for r >= t / 2) instead of as differences of
+  // nearly equal values: at a small gap and small t, fp32 rounding of c_skip alone is as large as c_skip(t) - c_skip(r).
+  const float gap = t - r, tpr = t + r, rt_t = sqrtf(den_t), rt_r = sqrtf(den_r);
+  const float dcs = -sd * sd * gap * tpr / (den_t * den_r);
+  const float dco = sd * sd * sd * gap * tpr / ((t * rt_r + r * rt_t) * rt_t * rt_r);
+  auto d_t = [&](size_t px, float f) -> float { return cs_t * xt[px] + co_t * f; };
+  auto delta = [&](size_t px, float ft, float fr) -> float {
+    if (!has_r) return d_t(px, ft) - y[px];       // a select: F_r of an r = 0 row is never read
+    const float xrv = xr[px];
+    return cs_t * (xt[px] - xrv) + dcs * xrv + co_t * (ft - fr) + dco * fr;
+  };
+  // MaskDiT's MAE statistics of one removed token: the per-patch mean and 1 / std (unbiased) of x_t
+  auto mae_stats = [&](int l, float* mu, float* rstd) {
+    float sx = 0.f;
+    for (int j = 0; j < gm.pd; ++j) sx += xt[gm.pix(b, l, j)];
+    *mu = sx / gm.pd;
+    float var = 0.f;
+    for (int j = 0; j < gm.pd; ++j) {
+      const float v = xt[gm.pix(b, l, j)] - *mu;
+      var += v * v;
+    }
+    *rstd = rsqrtf(var / static_cast<float>(gm.pd - 1) + 1e-6f);
+  };
+  float n_mask = 0.f;
+  if (mask) {
+    float cnt = 0.f;
+    for (int l = threadIdx.x; l < gm.L; l += blockDim.x) cnt += mask[static_cast<size_t>(b) * gm.L + l];
+    n_mask = block_sum(cnt, s_buf);
+  }
+  const float n_keep = static_cast<float>(gm.L) - n_mask;
+  const bool mae = mask && mae_coef > 0.f;
+  float acc_s = 0.f, acc_m = 0.f;
+  for (int l = threadIdx.x; l < gm.L; l += blockDim.x) {
+    const size_t row = (static_cast<size_t>(b) * gm.L + l) * gm.pd;
+    const float mk = mask ? mask[static_cast<size_t>(b) * gm.L + l] : 0.f;
+    float se = 0.f;
+    for (int j = 0; j < gm.pd; ++j) {
+      const size_t px = gm.pix(b, l, j);
+      if (Dx) Dx[px] = d_t(px, Ft[row + j]);
+      const float e = delta(px, Ft[row + j], Fr[row + j]);
+      se += e * e;
+    }
+    acc_s += (1.f - mk) * se;
+    if (mae && mk != 0.f) {
+      float mu, rstd, sm = 0.f;
+      mae_stats(l, &mu, &rstd);
+      for (int j = 0; j < gm.pd; ++j) {
+        const size_t px = gm.pix(b, l, j);
+        const float e = d_t(px, Ft[row + j]) - (xt[px] - mu) * rstd;
+        sm += e * e;
+      }
+      acc_m += mk * sm / gm.pd / n_mask;
+    }
+  }
+  const float scale = static_cast<float>(gm.L) / n_keep;          // L / T
+  const float S = block_sum(acc_s, s_buf) * scale;
+  const float M = mae ? block_sum(acc_m, s_buf) : 0.f;
+  const float root = sqrtf(S + c_h * c_h);
+  if (threadIdx.x == 0) loss[b] = S / (root + c_h) / gap + mae_coef * M;
+  if (!dF) return;
+  const float glb = gl[b];
+  const float k_s = glb * co_t / (gap * root) * scale;
+  for (int l = threadIdx.x; l < gm.L; l += blockDim.x) {
+    const size_t row = (static_cast<size_t>(b) * gm.L + l) * gm.pd;
+    const float mk = mask ? mask[static_cast<size_t>(b) * gm.L + l] : 0.f;
+    const float k_d = k_s * (1.f - mk);
+    float k_mae = 0.f, mu = 0.f, rstd = 0.f;
+    if (mae && mk != 0.f) {
+      mae_stats(l, &mu, &rstd);
+      k_mae = glb * mae_coef * mk / n_mask * 2.f / gm.pd * co_t;
+    }
+    for (int j = 0; j < gm.pd; ++j) {
+      const size_t px = gm.pix(b, l, j);
+      float gval = 0.f;
+      if (k_d != 0.f) gval = k_d * delta(px, Ft[row + j], Fr[row + j]);
+      if (k_mae != 0.f) gval += k_mae * (d_t(px, Ft[row + j]) - (xt[px] - mu) * rstd);
+      dF[row + j] = __float2bfloat16_rn(gval);
+    }
+  }
+}
+
 // u(sigma_b) alone, one block of 256 threads per sample: the loss kernel's arithmetic, so the same bits.
 __global__ void __launch_bounds__(256) logvar_kernel(const float* __restrict__ sigma, LogvarArgs lv) {
   __shared__ float s_buf[32];
@@ -768,6 +868,60 @@ flow_step_front_kernel(const float* __restrict__ moments, const float* __restric
   }
 }
 
+// ECT step front: mdt_step_front's latent and label dropout, then the pair of noise levels and both noisy inputs.
+//   t = exp(P_std rnd + P_mean)      r = t max(0, 1 - qs (1 + k / (1 + exp(b t))))      (k / (1 + exp(b t)) = k sigmoid(-b t))
+//   x_t = y + t noise                x_r = y + r noise                                   sr = r > 0 ? r : t
+// qs = q^-(s+1) is read from the device, so a replayed graph follows the stage.  Each product and sum is rounded
+// separately (no contraction), so the fp32 formula evaluated op by op gives the same bits.
+__global__ void __launch_bounds__(256)
+ect_step_front_kernel(const float* __restrict__ moments, const float* __restrict__ eps, const float* __restrict__ rnd,
+                      const float* __restrict__ noise, const float* __restrict__ drop_u, float drop_prob, float sf,
+                      float P_mean, float P_std, const float* __restrict__ qs, float k, float bc,
+                      float* __restrict__ y, float* __restrict__ xt, float* __restrict__ xr, float* __restrict__ sr,
+                      float* __restrict__ tt, float* __restrict__ rr, float* __restrict__ labels, int B, int C,
+                      int plane4, int nc) {
+  const long long per = static_cast<long long>(C) * plane4;  // float4 groups per sample
+  const long long total = static_cast<long long>(B) * per;
+  const float q = qs[0];
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int b = static_cast<int>(i / per);
+    const long long rem = i - b * per;
+    const float t = expf(__fadd_rn(__fmul_rn(rnd[b], P_std), P_mean));
+    const float sig = __fdiv_rn(1.f, __fadd_rn(1.f, expf(__fmul_rn(bc, t))));
+    const float w = __fsub_rn(1.f, __fmul_rn(q, __fadd_rn(1.f, __fmul_rn(k, sig))));
+    const float r = __fmul_rn(t, fmaxf(w, 0.f));
+    const float4* mom = reinterpret_cast<const float4*>(moments) + static_cast<long long>(b) * 2 * per;
+    const float4 mu = mom[rem], lv = mom[per + rem];
+    const float4 e = reinterpret_cast<const float4*>(eps)[i], nz = reinterpret_cast<const float4*>(noise)[i];
+    float4 o, ot, orr;
+    o.x = sf * (mu.x + expf(0.5f * fminf(fmaxf(lv.x, -30.f), 20.f)) * e.x);
+    o.y = sf * (mu.y + expf(0.5f * fminf(fmaxf(lv.y, -30.f), 20.f)) * e.y);
+    o.z = sf * (mu.z + expf(0.5f * fminf(fmaxf(lv.z, -30.f), 20.f)) * e.z);
+    o.w = sf * (mu.w + expf(0.5f * fminf(fmaxf(lv.w, -30.f), 20.f)) * e.w);
+    ot.x = __fadd_rn(o.x, __fmul_rn(t, nz.x));
+    ot.y = __fadd_rn(o.y, __fmul_rn(t, nz.y));
+    ot.z = __fadd_rn(o.z, __fmul_rn(t, nz.z));
+    ot.w = __fadd_rn(o.w, __fmul_rn(t, nz.w));
+    orr.x = __fadd_rn(o.x, __fmul_rn(r, nz.x));
+    orr.y = __fadd_rn(o.y, __fmul_rn(r, nz.y));
+    orr.z = __fadd_rn(o.z, __fmul_rn(r, nz.z));
+    orr.w = __fadd_rn(o.w, __fmul_rn(r, nz.w));
+    reinterpret_cast<float4*>(y)[i] = o;
+    reinterpret_cast<float4*>(xt)[i] = ot;
+    reinterpret_cast<float4*>(xr)[i] = orr;
+    if (rem == 0) tt[b] = t, rr[b] = r, sr[b] = r > 0.f ? r : t;
+  }
+  if (labels && drop_u) {
+    const long long nl = static_cast<long long>(B) * nc;
+    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < nl;
+         i += static_cast<long long>(gridDim.x) * blockDim.x) {
+      const int b = static_cast<int>(i / nc);
+      if (!(drop_u[b] >= drop_prob)) labels[i] = 0.f;
+    }
+  }
+}
+
 }  // namespace mdt
 
 using namespace mdt;
@@ -1159,6 +1313,38 @@ int mdt_flow_step_front(const float* moments, const float* eps, const float* rnd
   flow_step_front_kernel<<<static_cast<int>(blocks), 256, 0, S(stream)>>>(moments, eps, rnd_normal, noise_unit, drop_u,
                                                                           drop_prob, scale_factor, P_mean, P_std, y,
                                                                           xt, t, labels, B, C, R * R / 4, num_classes);
+  return launch_status();
+}
+
+int mdt_ect_step_front(const float* moments, const float* eps, const float* rnd_normal, const float* noise_unit,
+                       const float* drop_u, float drop_prob, float scale_factor, float P_mean, float P_std,
+                       const float* qs, float k, float b_coef, float* y, float* xt, float* xr, float* sr, float* t,
+                       float* r, float* labels, int B, int C, int R, int num_classes, void* stream) {
+  if (!moments || !eps || !rnd_normal || !noise_unit || !qs || !y || !xt || !xr || !sr || !t || !r || B <= 0 ||
+      C <= 0 || R <= 0)
+    return MDT_ERR_ARG;
+  if ((R * R) % 4) return MDT_ERR_ARG;
+  if ((reinterpret_cast<uintptr_t>(moments) | reinterpret_cast<uintptr_t>(eps) | reinterpret_cast<uintptr_t>(noise_unit) |
+       reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(xt) | reinterpret_cast<uintptr_t>(xr)) & 15)
+    return MDT_ERR_ARG;
+  const long long total = static_cast<long long>(B) * C * (R * R / 4);
+  long long blocks = (total + 255) / 256;
+  if (blocks > kNumSMsDefault * 8) blocks = kNumSMsDefault * 8;
+  ect_step_front_kernel<<<static_cast<int>(blocks), 256, 0, S(stream)>>>(
+      moments, eps, rnd_normal, noise_unit, drop_u, drop_prob, scale_factor, P_mean, P_std, qs, k, b_coef, y, xt, xr,
+      sr, t, r, labels, B, C, R * R / 4, num_classes);
+  return launch_status();
+}
+
+int mdt_ect_loss(const float* Ft, const float* Fr, const float* xt, const float* xr, const float* y, const float* t,
+                 const float* r, const float* mask, const float* gl, float sigma_data, float c, float mae_coef,
+                 float* loss, float* D_t, void* dF_bf16, int B, int C, int R, int p, void* stream) {
+  if (!Ft || !Fr || !xt || !xr || !y || !t || !r || !loss || B <= 0 || !(c > 0.f)) return MDT_ERR_ARG;
+  if (dF_bf16 && !gl) return MDT_ERR_ARG;
+  PatchGeom gm;
+  if (int rc = make_geom(&gm, C, R, p)) return rc;
+  ect_loss_kernel<<<B, 256, 0, S(stream)>>>(Ft, Fr, xt, xr, y, t, r, mask, gl, sigma_data, c, mae_coef, loss, D_t,
+                                            static_cast<__nv_bfloat16*>(dF_bf16), gm);
   return launch_status();
 }
 

@@ -1,4 +1,5 @@
-"""EDM training loss (reference: train_utils/loss.py) on the H100 engine, and the rectified-flow loss (`FlowLoss`).
+"""EDM training loss (reference: train_utils/loss.py) on the H100 engine, the rectified-flow loss (`FlowLoss`) and
+Easy Consistency Tuning of an EDM network (`ECTLoss`).
 
 `Losses['edm']` has the reference's constructor and call signature.  When `net` is a `maskdit_b200.EDMPrecond`
 (bare, or wrapped in anything exposing `.module` like DDP / `DataParallelB200`), the loss runs fused:
@@ -11,6 +12,8 @@ made with torch's generator in the reference's order (loss.py:35 randn[B,1,1,1];
 maskdit.py:102 rand[B,L]) so a seeded run consumes the same RNG stream positions as the reference.
 """
 from __future__ import annotations
+
+import math
 
 import torch
 
@@ -275,4 +278,153 @@ class FlowLoss:
         return loss
 
 
-Losses = {"edm": EDMLoss, "flow": FlowLoss}
+def ect_r(t, qs, k=8.0, b=1.0):
+    """ECT's target noise level r = t max(0, 1 - qs (1 + k sigmoid(-b t))), qs = q^-(s+1) of the tuning stage s (a
+    float or a device tensor), evaluated op by op as `mdt_ect_step_front` does."""
+    sig = 1.0 / (1.0 + torch.exp(b * t))
+    return t * (1.0 - qs * (1.0 + k * sig)).clamp_min(0.0)
+
+
+class _FusedECTLossFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, anchor, net, xt, xr, sr, y, t, r, labels, mask_dict, mae_coef, c):
+        # the target first: the student's saving forward must be the handle's last, its backward reads that workspace
+        Fr, _ = net._engine.forward(xr, sr, labels, mask_dict, save=False)
+        Ft, saved = net._engine.forward(xt, t, labels, mask_dict, save=True)
+        mask = mask_dict["mask"] if mask_dict is not None else None
+        p = net.model.patch_size
+        loss, _, _ = ops.ect_loss(Ft, Fr, xt, xr, y, t, r, mask, None, net.sigma_data, c, mae_coef, p,
+                                  want_dF=False)
+        ctx.net, ctx.saved = net, saved
+        ctx.args = (Ft, Fr, xt, xr, y, t, r, mask, mae_coef, c, p)
+        return loss
+
+    @staticmethod
+    def backward(ctx, gl):
+        net = ctx.net
+        Ft, Fr, xt, xr, y, t, r, mask, mae_coef, c, p = ctx.args
+        _, _, dF = ops.ect_loss(Ft, Fr, xt, xr, y, t, r, mask, gl.contiguous().float(), net.sigma_data, c, mae_coef, p,
+                                want_dF=True)
+        net._run_backward(ctx.saved, dF.view(-1, dF.shape[-1]))
+        ctx.saved = ctx.args = None
+        return (torch.zeros(1, device=gl.device),) + (None,) * 11
+
+
+class ECTLoss:
+    """Easy Consistency Tuning (ECT; Geng et al., ICLR 2025) of a trained `EDMPrecond`, whose output D(x; sigma) is
+    the consistency function f (DESIGN §5), with `EDMLoss`'s call signature.  Per sample: t = exp(P_mean + P_std n)
+    with n drawn where EDMLoss draws `rnd_normal`, r = `ect_r(t, q^-(s+1), k, b)` at the tuning stage s, one eps for
+    x_t = x + t eps and x_r = x + r eps.  The student D_t = D(x_t; t) carries the gradient; the target D_r = D(x_r; r)
+    is a no-gradient forward of the same weights with the same kept tokens and labels (x itself where r = 0).  The
+    loss is (sqrt(S + c^2) - c) / (t - r) + mae_coef M, S = (L / T) sum over kept patches of (D_t - D_r)^2,
+    c = 0.00054 sqrt(C R R), M MaskDiT's MAE term on the removed patches with D = D_t.  `last_edm_loss` holds the
+    per-sample loss of the last call (for the training log).
+
+    The stage enters as one fp32 device word, q^-(s+1): `stage_scale` when set (`TrainStep` owns it and moves it
+    with the run's step), otherwise built from `stage`."""
+
+    def __init__(self, stage_steps, q=2.0, k=8.0, b=1.0, P_mean=-1.1, P_std=2.0, sigma_data=0.5):
+        if int(stage_steps) != stage_steps or stage_steps < 1:
+            raise ValueError(f"ECT needs stage_steps >= 1 (steps per tuning stage), got {stage_steps}")
+        if not q > 1:
+            raise ValueError(f"ECT needs q > 1 (the gap t - r shrinks by q per stage), got {q}")
+        self.stage_steps = int(stage_steps)
+        self.q, self.k, self.b = float(q), float(k), float(b)
+        self.P_mean, self.P_std, self.sigma_data = P_mean, P_std, sigma_data
+        self.stage = 0
+        self.stage_scale = None
+
+    def stage_at(self, step, origin):
+        """The tuning stage s = floor((step - origin) / stage_steps) of run step `step` (origin: the first tuned)."""
+        return (int(step) - int(origin)) // self.stage_steps
+
+    def scale_of(self, stage):
+        """q^-(s+1) of stage s, the word the step front reads."""
+        return self.q ** -(int(stage) + 1)
+
+    def _qs(self, dev):
+        if self.stage_scale is not None:
+            return self.stage_scale
+        return torch.full((1,), self.scale_of(self.stage), dtype=torch.float32, device=dev)
+
+    def _randn(self, shape, device):
+        return torch.randn(shape, device=device)
+
+    def _rand(self, shape, device):
+        return torch.rand(shape, device=device)
+
+    def __call__(self, net, images, labels=None, mask_ratio=0, mae_loss_coef=0, feat=None, augment_pipe=None):
+        if feat is not None or augment_pipe is not None:
+            raise NotImplementedError("feat / augment_pipe are not part of the MaskDiT latent training path")
+        dev = images.device
+        raw = self._net(net, dev)
+        B = images.shape[0]
+        y = images.contiguous().float()
+        t4 = (self._randn([B, 1, 1, 1], dev) * self.P_std + self.P_mean).exp()
+        eps = self._randn(tuple(y.shape), dev)
+        r4 = ect_r(t4, self._qs(dev), self.k, self.b)
+        xt, xr = (y + t4 * eps).contiguous(), (y + r4 * eps).contiguous()
+        sr = torch.where(r4 > 0, r4, t4)
+        return self._finish(raw, y, xt, xr, sr.reshape(B).contiguous(), t4.reshape(B).contiguous(),
+                            r4.reshape(B).contiguous(), labels, mask_ratio, mae_loss_coef)
+
+    def from_moments(self, net, moments, labels=None, mask_ratio=0, mae_loss_coef=0, class_dropout_prob=0.0,
+                     scale_factor=0.18215, eps=None, drop_u=None):
+        """`EDMLoss.from_moments` with the ECT step front (`ops.ect_step_front`): latent, label dropout, t, r, x_t and
+        x_r in one launch, the same draws in the same order, `eps` / `drop_u` as there."""
+        dev = moments.device
+        raw = self._net(net, dev)
+        B, C2, R, _ = moments.shape
+        moments = moments.contiguous().float()
+        if eps is None:
+            eps = self._randn((B, C2 // 2, R, R), dev)
+        if class_dropout_prob > 0 and labels is not None:
+            if drop_u is None:
+                drop_u = self._rand((B, 1), dev).reshape(B)
+            drop_u = drop_u.contiguous()
+            if labels.dtype != torch.float32 or not labels.is_contiguous():
+                labels = labels.contiguous().float()
+        else:
+            drop_u = None
+        rnd_normal = self._randn([B, 1, 1, 1], dev).reshape(B).contiguous()
+        noise = self._randn((B, C2 // 2, R, R), dev).contiguous()
+        y, xt, xr, sr, t, r = ops.ect_step_front(moments, eps, rnd_normal, noise, self._qs(dev), labels, drop_u,
+                                                 float(class_dropout_prob), scale_factor, self.P_mean, self.P_std,
+                                                 self.k, self.b)
+        return self._finish(raw, y, xt, xr, sr, t, r, labels, mask_ratio, mae_loss_coef)
+
+    def _net(self, net, dev):
+        raw = _unwrap(net)
+        if not isinstance(raw, EDMPrecond) or isinstance(raw, FlowPrecond):
+            raise TypeError("maskdit_b200.Losses['ect'] tunes a maskdit_b200.EDMPrecond network"
+                            + (" (consistency tuning of a FlowPrecond is not supported)"
+                               if isinstance(raw, FlowPrecond) else ""))
+        if raw.logvar_channels:
+            raise ValueError("Losses['ect'] does not train a learned loss weighting: build the network with "
+                             "logvar_channels=0")
+        raw._ready(dev)
+        return raw
+
+    def _finish(self, raw, y, xt, xr, sr, t, r, labels, mask_ratio, mae_loss_coef):
+        dev, B = y.device, y.shape[0]
+        _, _, lab = raw._norm_inputs(y, t, labels)
+        md = None
+        if mask_ratio > 0:
+            assert raw.training, "masked loss needs net.train()"
+            L = raw.model.num_patches
+            md = ops.mask_indices(self._rand((B, L), dev), int(L * (1 - mask_ratio)))
+        coef = float(mae_loss_coef) if (mask_ratio > 0 and mae_loss_coef > 0) else 0.0
+        c = 0.00054 * math.sqrt(y[0].numel())
+        if torch.is_grad_enabled():
+            loss = _FusedECTLossFn.apply(raw._anchor, raw, xt, xr, sr, y, t, r, lab, md, coef, c)
+        else:
+            Fr, _ = raw._engine.forward(xr, sr, lab, md, save=False)
+            Ft, _ = raw._engine.forward(xt, t, lab, md, save=False)
+            loss, _, _ = ops.ect_loss(Ft, Fr, xt, xr, y, t, r, md["mask"] if md else None, None, raw.sigma_data, c,
+                                      coef, raw.model.patch_size, want_dF=False)
+        self.last_mask_dict = md
+        self.last_edm_loss = loss
+        return loss
+
+
+Losses = {"edm": EDMLoss, "flow": FlowLoss, "ect": ECTLoss}

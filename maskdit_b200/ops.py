@@ -263,6 +263,39 @@ def flow_loss(F, xt, y, eps, t, mask, gl, mae_coef, p, want_xhat=False, want_dF=
     return loss, xh, dF
 
 
+def ect_step_front(moments, eps, rnd_normal, noise_unit, qs, labels=None, drop_u=None, drop_prob=0.0,
+                   scale_factor=0.18215, P_mean=-1.1, P_std=2.0, k=8.0, b=1.0):
+    """`step_front` for Easy Consistency Tuning: moments -> latent x, label dropout, t = exp(P_mean + P_std rnd_normal),
+    r = t max(0, 1 - qs (1 + k sigmoid(-b t))), x_t = x + t noise_unit, x_r = x + r noise_unit: one launch.  `qs` is
+    one fp32 word on the device holding q^-(s+1).  Returns (x, x_t, x_r, sigma of the target forward, t, r)."""
+    _c(moments, f32), _c(eps, f32), _c(rnd_normal, f32), _c(noise_unit, f32), _c(qs, f32), _c(labels, f32), \
+        _c(drop_u, f32)
+    B, C2, R, _ = moments.shape
+    C = C2 // 2
+    y = torch.empty(B, C, R, R, dtype=f32, device=moments.device)
+    xt, xr = torch.empty_like(y), torch.empty_like(y)
+    sr, t, r = (torch.empty(B, dtype=f32, device=moments.device) for _ in range(3))
+    nc = labels.shape[1] if labels is not None else 0
+    check(lib().mdt_ect_step_front(ptr(moments), ptr(eps), ptr(rnd_normal), ptr(noise_unit), ptr(drop_u), drop_prob,
+                                   scale_factor, P_mean, P_std, ptr(qs), float(k), float(b), ptr(y), ptr(xt), ptr(xr),
+                                   ptr(sr), ptr(t), ptr(r), ptr(labels) if drop_u is not None else 0, B, C, R, nc,
+                                   stream_ptr()), "mdt_ect_step_front")
+    return y, xt, xr, sr, t, r
+
+
+def ect_loss(Ft, Fr, xt, xr, y, t, r, mask, gl, sigma_data, c, mae_coef, p, want_D=False, want_dF=True):
+    """Consistency loss of the student output Ft against the target output Fr (mdt_ect_loss).  Returns (loss [B],
+    D_t or None, dF bf16 or None)."""
+    B, C, R, _ = xt.shape
+    loss = torch.empty(B, dtype=f32, device=xt.device)
+    D = torch.empty_like(xt) if want_D else None
+    dF = torch.empty(Ft.shape, dtype=bf16, device=xt.device) if want_dF else None
+    check(lib().mdt_ect_loss(ptr(Ft), ptr(Fr), ptr(xt), ptr(xr), ptr(y), ptr(t), ptr(r), ptr(mask), ptr(gl),
+                             float(sigma_data), float(c), float(mae_coef), ptr(loss), ptr(D), ptr(dF), B, C, R, p,
+                             stream_ptr()), "mdt_ect_loss")
+    return loss, D, dF
+
+
 def flow_cfg_out(F, B, C, R, p, cfg_scale=None):
     """The velocity [B, C, R, R]: unpatchify(F), or with `cfg_scale` the CFG combine Fu + s (Fc - Fu) of F's two
     halves (cond rows first)."""

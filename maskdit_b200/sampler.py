@@ -5,7 +5,8 @@ consumed once per step even when S_churn = 0).  With a `maskdit_b200.EDMPrecond`
 eval-mode engine pass at batch 2B with the classifier-free-guidance combine fused into the output kernel, and the
 fp64 Euler/Heun state updates are single fused kernels.  Both samplers can instead guide with a second network
 (`guide_net`, `guidance`: autoguidance) and apply either guidance only inside a noise-level interval
-(`guidance_interval`); see `_denoiser`.  `flow_sampler` integrates a rectified-flow network's velocity instead.
+(`guidance_interval`); see `_denoiser`.  `flow_sampler` integrates a rectified-flow network's velocity instead, and
+`consistency_sampler` samples a consistency-tuned network in one evaluation per noise level.
 """
 from __future__ import annotations
 
@@ -84,6 +85,40 @@ def edm_sampler(net, latents, class_labels=None, cfg_scale=None, feat=None, rand
             den = denoise(x32, t_next).float().contiguous()
             ops.heun_update(1, x_hat, den, d_cur, x_next, x32, t_hat, t_next)      # 2nd-order correction (:61-64)
     return x_next
+
+
+def consistency_sigmas(sigmas, sigma_max=float("inf")):
+    """The noise levels of `consistency_sampler`: each clamped to `sigma_max` as `edm_sampler` clamps its largest, then
+    required positive, finite and strictly decreasing.  Returns a list of floats."""
+    out = [min(float(s), float(sigma_max)) for s in sigmas]
+    if not out:
+        raise ValueError("consistency sampling needs at least one noise level")
+    if not all(np.isfinite(s) and s > 0 for s in out):
+        raise ValueError(f"consistency sampling needs positive, finite noise levels, got {out}")
+    if any(a <= b for a, b in zip(out, out[1:])):
+        raise ValueError(f"consistency sampling needs strictly decreasing noise levels, got {out}")
+    return out
+
+
+@torch.no_grad()
+def consistency_sampler(net, latents, class_labels=None, cfg_scale=None, randn_like=torch.randn_like, sigmas=(80.0,),
+                        guide_net=None, guidance=None, guidance_interval=None):
+    """Few-step sampler of a consistency-tuned network (`Losses['ect']`, DESIGN §5), one network evaluation per noise
+    level: x = sigma_0 z, D = f(x, sigma_0); then for each following sigma_i, x = D + sigma_i eps_i (one `randn_like`
+    per re-noising) and D = f(x, sigma_i).  Returns the last D (fp64).  Every evaluation is `edm_sampler`'s, so
+    `cfg_scale`, `guide_net` / `guidance` and `guidance_interval` apply as there; the state is fp64 and every update is
+    one `mdt_lincomb_f64` launch that also writes the next fp32 network input."""
+    denoise = _denoiser(net, class_labels, cfg_scale, None, guide_net, guidance, guidance_interval)
+    sig = consistency_sigmas(sigmas, net.sigma_max)
+    x = latents.to(torch.float64).contiguous().clone()
+    xin = torch.empty(latents.shape, dtype=torch.float32, device=latents.device)
+    ops.lincomb_f64(sig[0], x, out=x, out_f32=xin)                                                # sigma_0 z
+    D = denoise(xin, sig[0]).float().contiguous()
+    for s in sig[1:]:
+        noise = randn_like(x).contiguous()
+        ops.lincomb_f64(s, noise, 0.0, None, 1.0, D, out=x, out_f32=xin)                         # D + sigma_i eps_i
+        D = denoise(xin, s).float().contiguous()
+    return D.double()
 
 
 def flow_grid(num_steps):

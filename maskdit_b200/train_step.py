@@ -17,7 +17,7 @@ import torch
 import torch.distributed as dist
 
 from . import ops, phema
-from .loss import EDMLoss
+from .loss import ECTLoss, EDMLoss
 from .maskdit import EDMPrecond
 
 
@@ -111,6 +111,11 @@ class GradComm:
 class TrainStep:
     phema_emas = ()   # no post-hoc EMA profiles unless the constructor is given widths
     edm_loss = None   # the last step's reference per-sample loss (see `step`)
+    # consistency tuning (loss_fn an ECTLoss): the stage's device word q^-(s+1) that the step front reads (allocated by
+    # the first tuned step), the run step of the first tuned step, and the last step's stage
+    _ect_qs = None
+    ect_origin = None
+    ect_stage = None
 
     def __init__(self, net: EDMPrecond, ema: EDMPrecond | None = None, lr=1e-4, betas=(0.9, 0.999), eps=1e-8,
                  weight_decay=0.0, ema_decay=0.9999, loss_fn: EDMLoss | None = None, process_group=None,
@@ -264,6 +269,9 @@ class TrainStep:
         `max_grad_norm`).  Reading its value synchronises; the step itself never does."""
         return self._gn[0] if self.max_grad_norm is not None else None
 
+    def _tunes(self):
+        return isinstance(getattr(self, "loss_fn", None), ECTLoss)
+
     def applied_steps(self) -> int:
         """Adam's step count: the steps whose update was applied (a host read of the device counter under
         `skip_nonfinite`, i.e. one synchronisation; `step_count` otherwise)."""
@@ -279,7 +287,8 @@ class TrainStep:
         param_group (apex layout).  Tensors are copies on the current device.  The step count is Adam's
         (`applied_steps()`): under `skip_nonfinite` it leaves out the skipped steps.
         With power-function EMA profiles, `phema` holds their widths, exponents, origin, step count and flat buffers
-        (host copies: the device keeps no second copy of them)."""
+        (host copies: the device keeps no second copy of them).  Under consistency tuning, `ect` holds the tuning
+        origin, so a resumed run continues the stage."""
         state, n_all = {}, 0
         adam_step = self.applied_steps()
         for i, (k, p) in enumerate(self.net.named_parameters()):
@@ -293,6 +302,8 @@ class TrainStep:
         sd = {"state": state,
               "param_groups": [{"lr": self.lr, "betas": self.betas, "eps": self.eps, "weight_decay": self.wd,
                                 "step": adam_step, "params": list(range(n_all))}]}
+        if self._tunes():
+            sd["ect"] = {"origin": self.ect_origin, "stage_steps": self.loss_fn.stage_steps}
         if self.phema_emas:
             sd["phema"] = {"sigma_rels": list(self.phema_sigma_rels), "gammas": list(self.phema_gammas),
                            "origin": self.phema_origin, "steps": self.phema_steps,
@@ -339,6 +350,8 @@ class TrainStep:
             group["weight_decay"]
         if self.phema_emas:
             self._load_phema(sd.get("phema"))
+        if self._tunes():   # a state without it (an EDM run's) starts tuning at the next step
+            self.ect_origin = (sd.get("ect") or {}).get("origin")
 
     def _load_phema(self, ph):
         """Continue the stored profiles, or (a state without them, e.g. a reference checkpoint) start new ones whose
@@ -504,6 +517,8 @@ class TrainStep:
         flat buffer anyway, so the rounds simply run back to back and 1/rounds is folded into the optimizer kernel.
         `moments=True`: `images` are VAE moments [B,2C,R,R] straight from the dataset; the latent sampling, the label
         dropout (`class_dropout_prob`) and the noise injection run as the fused step-front kernel (EDMLoss.from_moments).
+        With an `ECTLoss` the step runs at tuning stage s = floor((run step - ect_origin) / stage_steps), the run step
+        being `step_count + lr_step_offset` before the call and `ect_origin` the run step of the first tuned step.
         Under `torch.use_deterministic_algorithms(True)` the library's deterministic mode is on for the step
         (`mdt_set_deterministic`): the gradients, and so the weights, moments and EMA, repeat bit for bit."""
         st = self.st
@@ -536,6 +551,15 @@ class TrainStep:
                 self.phema_origin = self.step_count - 1 + self.lr_step_offset
             self.phema_steps += 1
             self._phema_c = [phema.one_minus_beta(g, self.phema_steps) for g in self.phema_gammas]
+        if self._tunes():   # the stage word changes on the device, so a replayed graph reads it too
+            if self._ect_qs is None:
+                self._ect_qs = torch.zeros(1, dtype=torch.float32, device=st.w32.device)
+            self.loss_fn.stage_scale = self._ect_qs
+            run = self.step_count - 1 + self.lr_step_offset
+            if self.ect_origin is None:
+                self.ect_origin = run
+            self.ect_stage = self.loss_fn.stage_at(run, self.ect_origin)
+            self._ect_qs.fill_(self.loss_fn.scale_of(self.ect_stage))
         guard = self._flag is not None
         if guard:
             self._flag.zero_()

@@ -27,6 +27,11 @@ the validation line adds the EMA's u at the validation levels.
 Gradient-norm clipping (not in the reference): `--max_grad_norm 1.0` clips the global gradient norm as
 torch.nn.utils.clip_grad_norm_ does, `--max_grad_norm inf` only measures it; either way the log line reports the
 window's mean and maximum norm.
+Consistency tuning (not in the reference): `train.objective: ect` with a `train.ect:` block (`stage_steps`, optional `q`,
+`k`, `b`, `P_mean`, `P_std`) tunes an EDM network into a one- or two-step generator (`Losses['ect']`); start it from a
+trained checkpoint with `--ckpt_path pre.pt --use_strict_load False` (weights and EMA, a fresh optimizer).  `Train Loss`
+is then the consistency loss and the log line appends the tuning stage; the `Val Loss` line stays the EDM denoising loss,
+which does not measure a tuned network's sample quality.
 """
 import argparse
 import copy
@@ -36,8 +41,8 @@ import time
 import torch
 import torch.distributed as dist
 
-from maskdit_b200.config import build_net, load_config, mask_ratio_schedule, parse_float_none, parse_int_list
-from maskdit_b200.loss import Losses
+from maskdit_b200.config import build_loss, build_net, load_config, mask_ratio_schedule, parse_float_none, \
+    parse_int_list
 from maskdit_b200.train_step import TrainStep, check_max_grad_norm
 
 
@@ -64,10 +69,11 @@ def skip_nonfinite(args):
     return not args.no_amp
 
 
-def log_line(step, loss, steps_per_sec, skipped=None, grad_norm=None, weighted=None):
+def log_line(step, loss, steps_per_sec, skipped=None, grad_norm=None, weighted=None, ect_stage=None):
     """The training log line (the reference's format, train.py:247); `skipped` (a count), `grad_norm` (the
-    window's mean and max) and `weighted` (the mean objective of a learned loss weighting) are appended only when
-    given.  `loss` is always the reference's loss, so it compares across runs with and without the weighting."""
+    window's mean and max), `weighted` (the mean objective of a learned loss weighting) and `ect_stage` (the
+    consistency-tuning stage of the last step) are appended only when given.  `loss` is the reference's loss, so it
+    compares across runs with and without the weighting (under consistency tuning, the consistency loss)."""
     line = f"(step={step:07d}) Train Loss: {loss:.4f}, Train Steps/Sec: {steps_per_sec:.2f}"
     if skipped is not None:
         line += f", Skipped Steps: {skipped}"
@@ -75,6 +81,8 @@ def log_line(step, loss, steps_per_sec, skipped=None, grad_norm=None, weighted=N
         line += f", Grad Norm: {grad_norm[0]:.4g} (max {grad_norm[1]:.4g})"
     if weighted is not None:
         line += f", Weighted Loss: {weighted:.4f}"
+    if ect_stage is not None:
+        line += f", ECT stage: {ect_stage}"
     return line
 
 
@@ -148,6 +156,10 @@ def held_out_set(args, cfg):
 def main():
     args, _ = build_parser().parse_known_args()
     cfg = load_config(args.config)
+    try:
+        loss_fn = build_loss(cfg)
+    except ValueError as e:
+        raise SystemExit(f"{args.config}: {e}")
 
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
     local = int(os.environ.get("LOCAL_RANK", 0))
@@ -176,7 +188,7 @@ def main():
         ema.load_state_dict({k.replace("_orig_mod.", ""): v for k, v in sd["ema"].items()}, strict=strict)
         step0 = int(os.path.basename(ck)[:-3]) if os.path.basename(ck)[:-3].isdigit() else 0
     ts = TrainStep(net, ema, lr=cfg.train.lr, lr_rampup_kimg=cfg.train.lr_rampup_kimg, global_batch=global_batch,
-                   loss_fn=Losses[cfg.model.precond](), reference_lr_schedule=True,
+                   loss_fn=loss_fn, reference_lr_schedule=True,
                    skip_nonfinite=skip_nonfinite(args), phema_sigma_rels=args.phema_sigma_rel,
                    max_grad_norm=args.max_grad_norm)
     if ck and strict and "opt" in sd:                      # train.py:150: optimizer state only under strict loading
@@ -262,7 +274,7 @@ def main():
                 # every rank computes the same norm from the same summed gradient
                 gnorm = (float(gn_sum) / log_steps, float(gn_max)) if gn_sum is not None else None
                 print(log_line(step, float(avg), log_steps / (time.time() - t0), skipped, gnorm,
-                               float(wavg) if wavg is not None else None), flush=True)
+                               float(wavg) if wavg is not None else None, ts.ect_stage), flush=True)
             running, weighted, log_steps, t0 = 0.0, 0.0, 0, time.time()
             gn_sum = gn_max = None
         if held is not None and step % args.val_every == 0:
