@@ -18,8 +18,11 @@ applies CFG or the guide only at evaluations with LO < sigma <= HI.  A rectified
 samples with `flow_sampler` (Heun on a uniform t grid, `--num_steps`, `--cfg_scale`, `--guidance_interval` on t) and
 refuses the ablation switches, `--S_churn` and autoguidance.  `--consistency_sigmas S0 [S1 ...]` samples a
 consistency-tuned EDM network (train.py with `train.objective: ect`) with `consistency_sampler`, one evaluation per
-noise level, and refuses the ablation switches, `--S_churn` and flow configs.  Class-unconditional configs sample with all-zero
-label rows as the reference does (sample.py:261-264).
+noise level, and refuses the ablation switches, `--S_churn` and flow configs.  `--dpm_order {1,2,3}` samples an EDM or a
+flow config with `dpm_solver_sampler` (multistep DPM-Solver++: DDIM, 2M or 3M) in `--num_steps` network evaluations,
+with `--cfg_scale`, autoguidance (EDM) and `--guidance_interval` as above, and refuses the ablation switches, `--S_churn`
+and `--consistency_sigmas`.  Class-unconditional configs sample with all-zero label rows as the reference does
+(sample.py:261-264).
 """
 import argparse
 import os
@@ -30,8 +33,8 @@ import torch
 from maskdit_b200.config import build_net, load_config, parse_float_none, parse_int_list
 from maskdit_b200.maskdit import eval_state_dict
 from maskdit_b200 import ops
-from maskdit_b200.sampler import (ablation_sampler, consistency_sampler, consistency_sigmas, edm_sampler, flow_sampler,
-                                  rank_seed_batches, write_png)
+from maskdit_b200.sampler import (ablation_sampler, consistency_sampler, consistency_sigmas, dpm_solver_sampler,
+                                  edm_sampler, flow_sampler, rank_seed_batches, write_png)
 
 
 class StackedRandomGenerator:
@@ -87,6 +90,9 @@ def build_parser():
     ap.add_argument("--consistency_sigmas", type=float, nargs="+", default=None, metavar="SIGMA",
                     help="sample a consistency-tuned network (train.objective: ect) at these strictly decreasing noise "
                          "levels, one network evaluation each (e.g. 80, or 80 0.8)")
+    ap.add_argument("--dpm_order", type=int, choices=[1, 2, 3], default=None,
+                    help="sample with multistep DPM-Solver++ of this order (1 DDIM, 2 2M, 3 3M) in --num_steps network "
+                         "evaluations, EDM or flow configs")
     return ap
 
 
@@ -123,6 +129,16 @@ def parse_args(argv=None):
             consistency_sigmas(args.consistency_sigmas)
         except ValueError as e:
             ap.error(f"--consistency_sigmas: {e}")
+    if args.dpm_order is not None:
+        bad = [f"--{k}" for k in ("solver", "discretization", "schedule", "scaling") if getattr(args, k)]
+        if args.S_churn:
+            bad.append("--S_churn")
+        if args.consistency_sigmas is not None:
+            bad.append("--consistency_sigmas")
+        if bad:
+            ap.error(f"--dpm_order samples with dpm_solver_sampler: {', '.join(bad)} do not apply to it")
+        if args.num_steps < 1:
+            ap.error(f"--dpm_order needs --num_steps >= 1, got {args.num_steps}")
     return args
 
 
@@ -207,6 +223,9 @@ def main(argv=None):
             if args.consistency_sigmas is not None:
                 z = consistency_sampler(net, latents.float(), labels.float(), cfg_scale=args.cfg_scale,
                                         randn_like=rnd.randn_like, sigmas=args.consistency_sigmas, **gkw).float()
+            elif args.dpm_order is not None:
+                z = dpm_solver_sampler(net, latents.float(), labels.float(), cfg_scale=args.cfg_scale,
+                                       num_steps=args.num_steps, order=args.dpm_order, **gkw).float()
             elif flow:
                 z = flow_sampler(net, latents.float(), labels.float(), cfg_scale=args.cfg_scale,
                                  num_steps=args.num_steps, **gkw).float()

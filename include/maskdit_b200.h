@@ -307,6 +307,17 @@ int mdt_heun_update(int mode, const double* x_hat, const float* denoised, double
 int mdt_lincomb_f64(double a, const double* x, double b, const double* y, double c, const float* z, double* out,
                     float* out_f32, double f32_scale, long long n, void* stream);
 
+/* One multistep DPM-Solver++ step in fp64 (dpm_solver_sampler, DESIGN §5), one launch per network evaluation:
+ *   D = F (kind MDT_DPM_DATA: F is the data prediction) or D = x - t*F (MDT_DPM_VELOCITY: F is a flow network's
+ *   velocity; x is the state at flow time t) ;  d_out = D ;  x = a*x + b0*D + b1*h1 + b2*h2 (in place) ;
+ *   x_f32 = float(x).  Each product and sum is rounded separately, in that order.  h2 / h1 may be NULL (term
+ *   omitted; h2 only with h1), x_f32 may be NULL.  MDT_ERR_ARG for a NULL F / x / d_out, n <= 0, an unknown kind or a
+ *   non-finite scalar.                                                                                            */
+#define MDT_DPM_DATA 0
+#define MDT_DPM_VELOCITY 1
+int mdt_dpm_update(const float* F, int kind, double t, double* x, double* d_out, const double* h1, const double* h2,
+                   double a, double b0, double b1, double b2, float* x_f32, long long n, void* stream);
+
 /* Sampler tail (sample.py:287): img [B,C,H,W] f32 in [-1,1] -> uint8 [B,H,W,C] = clamp((img + 1) * 127.5, 0, 255).  */
 int mdt_to_uint8_nhwc(const float* img, unsigned char* out, int B, int C, int H, int W, void* stream);
 

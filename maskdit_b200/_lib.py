@@ -101,6 +101,7 @@ _SIGS = {
     "mdt_guided_precond_out": [_P, _I, _P, _I, _P, _P, _F, _F, _P, _I, _I, _I, _P],
     "mdt_heun_update": [_I, _P, _P, _P, _P, _P, _D, _D, _LL, _P],
     "mdt_lincomb_f64": [_D, _P, _D, _P, _D, _P, _P, _P, _D, _LL, _P],
+    "mdt_dpm_update": [_P, _I, _D, _P, _P, _P, _P, _D, _D, _D, _D, _P, _LL, _P],
     "mdt_to_uint8_nhwc": [_P, _P, _I, _I, _I, _I, _P],
     # step driver (csrc/driver.cu)
     "mdt_model_create": [POINTER(ModelCfg), POINTER(c_void_p)],

@@ -477,6 +477,26 @@ __global__ void lincomb_f64_kernel(double a, const double* __restrict__ x, doubl
   if (out_f32) out_f32[i] = static_cast<float>(v * f32_scale);
 }
 
+// One multistep DPM-Solver++ step (dpm_solver_sampler, DESIGN §5): the data prediction D_i of this evaluation (F itself,
+// or x - t F for a flow network's velocity), then x' = a x + b0 D_i + b1 H1 + b2 H2 with host-computed fp64 scalars.
+// Every product and sum is rounded on its own, in that order (no contraction), so the result is the op-by-op fp64 value.
+__global__ void dpm_update_kernel(const float* __restrict__ F, int velocity, double t, double* __restrict__ x,
+                                  double* __restrict__ d_out, const double* __restrict__ h1,
+                                  const double* __restrict__ h2, double a, double b0, double b1, double b2,
+                                  float* __restrict__ x_f32, long long n) {
+  const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  if (i >= n) return;
+  const double xi = x[i];
+  const double f = static_cast<double>(F[i]);
+  const double d = velocity ? __dsub_rn(xi, __dmul_rn(t, f)) : f;
+  d_out[i] = d;
+  double v = __dadd_rn(__dmul_rn(a, xi), __dmul_rn(b0, d));
+  if (h1) v = __dadd_rn(v, __dmul_rn(b1, h1[i]));
+  if (h2) v = __dadd_rn(v, __dmul_rn(b2, h2[i]));
+  x[i] = v;
+  if (x_f32) x_f32[i] = static_cast<float>(v);
+}
+
 __global__ void to_uint8_nhwc_kernel(const float* __restrict__ img, unsigned char* __restrict__ out, int B, int C,
                                      int H, int W) {
   const long long n = static_cast<long long>(B) * C * H * W;
@@ -1062,6 +1082,16 @@ int mdt_lincomb_f64(double a, const double* x, double b, const double* y, double
   if (!x || (!out && !out_f32) || n <= 0) return MDT_ERR_ARG;
   lincomb_f64_kernel<<<static_cast<int>((n + 255) / 256), 256, 0, S(stream)>>>(a, x, b, y, c, z, out, out_f32,
                                                                                f32_scale, n);
+  return launch_status();
+}
+
+int mdt_dpm_update(const float* F, int kind, double t, double* x, double* d_out, const double* h1, const double* h2,
+                   double a, double b0, double b1, double b2, float* x_f32, long long n, void* stream) {
+  if (!F || !x || !d_out || n <= 0 || (kind != MDT_DPM_DATA && kind != MDT_DPM_VELOCITY) ||
+      (h2 && !h1) || !isfinite(a) || !isfinite(b0) || !isfinite(b1) || !isfinite(b2) || !isfinite(t))
+    return MDT_ERR_ARG;
+  dpm_update_kernel<<<static_cast<int>((n + 255) / 256), 256, 0, S(stream)>>>(
+      F, kind == MDT_DPM_VELOCITY, t, x, d_out, h1, h2, a, b0, b1, b2, x_f32, n);
   return launch_status();
 }
 

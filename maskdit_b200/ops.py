@@ -353,6 +353,20 @@ def lincomb_f64(a, x, b=0.0, y=None, c=0.0, z=None, out=None, out_f32=None, f32_
     return out, out_f32
 
 
+def dpm_update(F, x, d_out, a, b0, h1=None, b1=0.0, h2=None, b2=0.0, velocity=False, t=0.0, out_f32=None):
+    """One DPM-Solver++ step in place: D = F, or x - t F when `velocity` (a flow network's v^); d_out = D;
+    x = a x + b0 D + b1 h1 + b2 h2 (terms with a None operand omitted); out_f32 = float(x)."""
+    _c(F, f32), _c(x, torch.float64), _c(d_out, torch.float64), _c(h1, torch.float64), _c(h2, torch.float64)
+    _c(out_f32, f32)
+    for o in (F, d_out, h1, h2, out_f32):
+        if o is not None and o.numel() != x.numel():
+            raise L.MdtError(f"dpm_update operands must match the state's {x.numel()} elements, got {o.numel()}")
+    check(lib().mdt_dpm_update(ptr(F), 1 if velocity else 0, float(t), ptr(x), ptr(d_out), ptr(h1), ptr(h2), float(a),
+                               float(b0), float(b1), float(b2), ptr(out_f32), x.numel(), stream_ptr()),
+          "mdt_dpm_update")
+    return x, out_f32
+
+
 def to_uint8_nhwc(img):
     """[B,C,H,W] f32 in [-1,1] -> uint8 [B,H,W,C] (sample.py:287)."""
     _c(img, f32)

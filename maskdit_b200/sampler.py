@@ -5,10 +5,13 @@ consumed once per step even when S_churn = 0).  With a `maskdit_b200.EDMPrecond`
 eval-mode engine pass at batch 2B with the classifier-free-guidance combine fused into the output kernel, and the
 fp64 Euler/Heun state updates are single fused kernels.  Both samplers can instead guide with a second network
 (`guide_net`, `guidance`: autoguidance) and apply either guidance only inside a noise-level interval
-(`guidance_interval`); see `_denoiser`.  `flow_sampler` integrates a rectified-flow network's velocity instead, and
-`consistency_sampler` samples a consistency-tuned network in one evaluation per noise level.
+(`guidance_interval`); see `_denoiser`.  `flow_sampler` integrates a rectified-flow network's velocity instead,
+`consistency_sampler` samples a consistency-tuned network in one evaluation per noise level, and `dpm_solver_sampler`
+(multistep DPM-Solver++) samples an EDM or a flow network in one evaluation per noise level.
 """
 from __future__ import annotations
+
+import math
 
 import numpy as np
 import torch
@@ -155,6 +158,109 @@ def flow_sampler(net, latents, class_labels=None, cfg_scale=None, num_steps=50, 
         v2 = denoise(xin, t_next).float().contiguous()
         ops.lincomb_f64(1.0, x, 0.0, None, 0.5 * h, v2, out=x, out_f32=xin)             # ... + h/2 v'
     return x
+
+
+def _lambda(alpha, sigma):
+    """log(alpha / sigma), with the limits -inf at alpha = 0 (flow time t = 1) and +inf at sigma = 0."""
+    if alpha == 0:
+        return -math.inf
+    if sigma == 0:
+        return math.inf
+    return math.log(alpha / sigma)
+
+
+def dpm_solver_coefficients(alpha, sigma, order):
+    """The steps of multistep DPM-Solver++ (DESIGN §5) on the levels x = alpha_i x0 + sigma_i eps, i = 0..N (sigma_N = 0),
+    expanded to x' = a x + b0 D_i + b1 D_{i-1} + b2 D_{i-2}: one (k, a, b0, b1, b2) per step i = 0..N-1, in fp64.
+    k = min(order, i + 1, N - i) is the step's order (the terms k does not use have coefficient 0).  The step into
+    sigma = 0 is x' = alpha_N D; a history term whose lambda gap is infinite (flow time t = 1) drops out (its ratio r
+    is infinite)."""
+    if order not in (1, 2, 3):
+        raise ValueError(f"order must be 1, 2 or 3, got {order}")
+    alpha, sigma = [float(v) for v in alpha], [float(v) for v in sigma]
+    N = len(sigma) - 1
+    lam = [_lambda(a, s) for a, s in zip(alpha, sigma)]
+    out = []
+    for i in range(N):
+        a1 = alpha[i + 1]
+        if sigma[i + 1] == 0:
+            out.append((1, 0.0, a1, 0.0, 0.0))
+            continue
+        h = lam[i + 1] - lam[i]
+        E = math.expm1(-h)
+        a, b0, b1, b2 = sigma[i + 1] / sigma[i], -a1 * E, 0.0, 0.0
+        k = min(order, i + 1, N - i)
+        if k == 2:
+            r0 = (lam[i] - lam[i - 1]) / h
+            # - a1 E / 2 * (D_i - D_{i-1}) / r0
+            c = -0.5 * a1 * E / r0
+            b0, b1 = b0 + c, -c
+        elif k == 3:
+            r0 = (lam[i] - lam[i - 1]) / h
+            r1 = (lam[i - 1] - lam[i - 2]) / h
+            c1 = a1 * (E / h + 1)                       # weight of D1
+            c2 = -a1 * ((E + h) / (h * h) - 0.5)        # weight of D2
+            # D1 = (1 + r0/(r0+r1)) D1_0 - r0/(r0+r1) D1_1,  D2 = (D1_0 - D1_1)/(r0+r1),  D1_j = difference / r_j
+            w0 = c1 * (1 + r0 / (r0 + r1)) + c2 / (r0 + r1)
+            w1 = -c1 * r0 / (r0 + r1) - c2 / (r0 + r1)
+            b0, b1, b2 = b0 + w0 / r0, -w0 / r0 + w1 / r1, -w1 / r1
+        out.append((k, a, b0, b1, b2))
+    return out
+
+
+def dpm_solver_levels(net, num_steps, sigma_min=0.002, sigma_max=80, rho=7):
+    """(flow, levels): the N = num_steps noise levels of `dpm_solver_sampler` followed by 0.  EDM: `edm_sampler`'s
+    Karras grid, clamped to the network's sigma range (a single level is sigma_max); flow (`FlowPrecond`):
+    `flow_grid(N)`."""
+    if num_steps < 1:
+        raise ValueError(f"num_steps must be at least 1, got {num_steps}")
+    from .maskdit import FlowPrecond
+    if isinstance(net, FlowPrecond):
+        return True, flow_grid(num_steps)
+    sigma_min = max(sigma_min, net.sigma_min)
+    sigma_max = min(sigma_max, net.sigma_max)
+    if num_steps == 1:
+        return False, np.array([float(sigma_max), 0.0])
+    i = np.arange(num_steps, dtype=np.float64)
+    t = (sigma_max ** (1 / rho) + i / (num_steps - 1) * (sigma_min ** (1 / rho) - sigma_max ** (1 / rho))) ** rho
+    return False, np.concatenate([t, [0.0]])
+
+
+def _dpm_solve(denoise, x, levels, flow, order):
+    """Multistep DPM-Solver++ from the fp64 state `x` at levels[0] through `levels` (the last one 0).  denoise(x32,
+    level) is the network output at the fp32 input x32: D (EDM) or the velocity v^ (flow, D = x - t v^ from the fp64
+    state).  One network evaluation and one `mdt_dpm_update` launch per positive level; x is updated in place."""
+    levels = np.asarray(levels, dtype=np.float64)
+    alpha, sigma = (1.0 - levels, levels) if flow else (np.ones_like(levels), levels)
+    steps = dpm_solver_coefficients(alpha, sigma, order)
+    hist = [torch.empty_like(x) for _ in range(min(order, len(steps)))]
+    xin = x.float().contiguous()
+    for i, (k, a, b0, b1, b2) in enumerate(steps):
+        lv = float(levels[i])
+        F = denoise(xin, lv).float().contiguous()
+        slot = lambda j: hist[(i - j) % len(hist)]  # noqa: E731  D_{i-j}
+        last = i == len(steps) - 1
+        ops.dpm_update(F, x, slot(0), a, b0, slot(1) if k >= 2 else None, b1, slot(2) if k >= 3 else None, b2,
+                       velocity=flow, t=lv, out_f32=None if last else xin)
+    return x
+
+
+@torch.no_grad()
+def dpm_solver_sampler(net, latents, class_labels=None, cfg_scale=None, num_steps=10, order=3, sigma_min=0.002,
+                       sigma_max=80, rho=7, guide_net=None, guidance=None, guidance_interval=None):
+    """Multistep DPM-Solver++ (Lu et al., 2022; DESIGN §5), a training-free ODE sampler of an EDM (`EDMPrecond`) or a
+    rectified-flow (`FlowPrecond`) network in `num_steps` network evaluations, one per level of
+    `dpm_solver_levels`: order 1 is DDIM, 2 and 3 are 2M and 3M.  The state is fp64, every step is one `mdt_dpm_update`
+    launch, and the returned fp64 value is D at the last positive level.  Each evaluation is `edm_sampler`'s, so
+    `cfg_scale`, `guide_net` / `guidance` (EDM only: a flow network refuses a guide) and `guidance_interval` apply as
+    there; for a flow network the interval is decided on t."""
+    if order not in (1, 2, 3):
+        raise ValueError(f"order must be 1, 2 or 3, got {order}")
+    flow, levels = dpm_solver_levels(net, num_steps, sigma_min, sigma_max, rho)
+    denoise = _denoiser(net, class_labels, cfg_scale, None, guide_net, guidance, guidance_interval)
+    x = latents.to(torch.float64).contiguous().clone()
+    ops.lincomb_f64(float(levels[0]), x, out=x)                                                  # sigma_0 z
+    return _dpm_solve(denoise, x, levels, flow, order)
 
 
 class _Schedules:
