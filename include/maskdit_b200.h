@@ -536,6 +536,33 @@ int mdt_nccl_comm_create(const void* id128, int rank, int world, int max_ctas, v
 int mdt_nccl_comm_destroy(void* comm);
 int mdt_allreduce_grads(void* comm, void* grad, long long n, int bf16, void* stream);
 
+/* Sharded optimizer state (ZeRO stage 1: the all-reduce split into its reduce-scatter and all-gather halves).  Both
+ * collectives run in place on `buf`, which holds world * count_per_rank elements; rank r's share is
+ * buf + r * count_per_rank.
+ *   mdt_reduce_scatter_grads: rank r's share becomes the SUM over the ranks of that share (fp32, or bf16 when
+ *   bf16 != 0); the rest of `buf` is left undefined.
+ *   mdt_allgather: every rank's share is copied to the same place on every rank.  dtype MDT_DTYPE_F32, _BF16 or _F64.
+ * MDT_ERR_ARG for a NULL pointer, count_per_rank <= 0 or another dtype; MDT_ERR_DRIVER when the process's NCCL lacks
+ * ncclReduceScatter / ncclAllGather / ncclCommUserRank.                                                             */
+#define MDT_DTYPE_F32 0
+#define MDT_DTYPE_BF16 1
+#define MDT_DTYPE_F64 2
+int mdt_reduce_scatter_grads(void* comm, void* buf, long long count_per_rank, int bf16, void* stream);
+int mdt_allgather(void* comm, void* buf, long long count_per_rank, int dtype, void* stream);
+
+/* The fp32-read set of the handle's training step: the [lo, hi) element ranges of the trainable region that some
+ * launch of mdt_forward / mdt_backward or of the training losses reads from `w32` rather than the bf16 shadow `w16`
+ * (the patch embedder, every bias of a GEMM epilogue, the adaLN biases, the mask token, the learned weighting's w).
+ * Sorted, disjoint, merged where adjacent, each hi rounded up to the 64-element tensor boundary.  Writes at most `cap`
+ * pairs to lohi (may be NULL with cap 0) and returns the number of ranges, or a negative status.  A sharded optimizer
+ * all-gathers these ranges of w32 after its update; every other master element may be stale on a rank between steps. */
+int mdt_model_fp32_read_ranges(const mdt_model* m, long long* lohi, int cap);
+
+/* dst[seg[3i+1] + j] = src[seg[3i] + j] for j < seg[3i+2], for each of the nseg segments (a device table of int64
+ * triples {src offset, dst offset, count}, in fp32 elements).  Segments must not overlap in dst.  The sharded
+ * optimizer packs and unpacks the fp32-read set with it.                                                          */
+int mdt_copy_segments_f32(const float* src, float* dst, const long long* seg, int nseg, void* stream);
+
 /* ============================================================================================================
  * SD-VAE: decode, the sampler tail (sample.py:275 `vae.decode(z)`; autoencoder.py:306-453), and encode, the latent
  * extraction (extract_latent.py:66; autoencoder.py:212-303,431-442).  Activations are pixel-major

@@ -118,6 +118,10 @@ _SIGS = {
     "mdt_nccl_comm_create": [_P, _I, _I, _I, POINTER(c_void_p)],
     "mdt_nccl_comm_destroy": [_P],
     "mdt_allreduce_grads": [_P, _P, _LL, _I, _P],
+    "mdt_reduce_scatter_grads": [_P, _P, _LL, _I, _P],
+    "mdt_allgather": [_P, _P, _LL, _I, _P],
+    "mdt_model_fp32_read_ranges": [_P, POINTER(c_longlong), _I],
+    "mdt_copy_segments_f32": [_P, _P, _P, _I, _P],
     "mdt_vae_post_quant": [_P, _P, _P, _F, _P, _I, _I, _I, _P],
     "mdt_vae_gn_stats": [_P, _P, _P, _I, _I, _I, _P],
     "mdt_vae_im2col": [_P, _P, _P, _P, _I, _I, _I, _P, _I, _I, _I, _I, _I, _P],

@@ -20,7 +20,9 @@
 #include <dlfcn.h>
 #include <string.h>
 
+#include <algorithm>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "common.cuh"
@@ -525,6 +527,31 @@ int mdt_model_param_info(const mdt_model* m, int i, char* name, int name_cap, lo
 
 int mdt_model_mod_width(const mdt_model* m) { return m ? m->NA : -1; }
 
+int mdt_model_fp32_read_ranges(const mdt_model* m, long long* lohi, int cap) {
+  if (!m || cap < 0 || (cap > 0 && !lohi)) return MDT_ERR_ARG;
+  // every W32() / w32 + offset read of mdt_forward and mdt_backward, and the loss kernels' logvar w
+  std::vector<const Tensor*> ts = {&m->xw, &m->xb, &m->t0b, &m->t2b, &m->flb};
+  for (auto* blocks : {&m->enc, &m->dec})
+    for (const BlockP& b : *blocks) ts.insert(ts.end(), {&b.qkv_b, &b.proj_b, &b.fc1_b, &b.fc2_b});
+  if (m->has_dec) ts.push_back(&m->dlb);
+  if (m->cfg.has_mask_token) ts.push_back(&m->mask_token);
+  if (m->logvar_channels > 0) ts.push_back(&m->lv_w);
+  std::vector<std::pair<i64, i64>> r;
+  for (const Tensor* t : ts) r.emplace_back(t->off, t->off + round_up(t->numel));
+  r.emplace_back(m->ada_b_off, m->ada_b_off + round_up(m->ada_b.back().off + m->ada_b.back().numel - m->ada_b_off));
+  std::sort(r.begin(), r.end());
+  std::vector<std::pair<i64, i64>> merged;
+  for (const auto& x : r) {
+    if (!merged.empty() && x.first <= merged.back().second)
+      merged.back().second = std::max(merged.back().second, x.second);
+    else
+      merged.push_back(x);
+  }
+  for (size_t i = 0; i < merged.size() && static_cast<int>(i) < cap; ++i)
+    lohi[2 * i] = merged[i].first, lohi[2 * i + 1] = merged[i].second;
+  return static_cast<int>(merged.size());
+}
+
 int mdt_model_set_recompute(mdt_model* m, int r) {
   if (!m || r < 0 || r > static_cast<int>(m->enc.size() + m->dec.size())) return MDT_ERR_ARG;
   m->recompute = r;
@@ -804,6 +831,10 @@ struct NcclApi {
   int (*GetVersion)(int*) = nullptr;
   int (*CommDestroy)(void*) = nullptr;
   int (*AllReduce)(const void*, void*, size_t, int, int, void*, cudaStream_t) = nullptr;
+  // the sharded optimizer's halves of the all-reduce (optional: only mdt_reduce_scatter_grads / mdt_allgather need them)
+  int (*ReduceScatter)(const void*, void*, size_t, int, int, void*, cudaStream_t) = nullptr;
+  int (*AllGather)(const void*, void*, size_t, int, void*, cudaStream_t) = nullptr;
+  int (*CommUserRank)(void*, int*) = nullptr;
   bool ok = false;
 };
 NcclApi& nccl() {
@@ -822,6 +853,9 @@ NcclApi& nccl() {
       api.GetVersion = reinterpret_cast<decltype(api.GetVersion)>(dlsym(h, "ncclGetVersion"));
       api.CommDestroy = reinterpret_cast<decltype(api.CommDestroy)>(dlsym(h, "ncclCommDestroy"));
       api.AllReduce = reinterpret_cast<decltype(api.AllReduce)>(dlsym(h, "ncclAllReduce"));
+      api.ReduceScatter = reinterpret_cast<decltype(api.ReduceScatter)>(dlsym(h, "ncclReduceScatter"));
+      api.AllGather = reinterpret_cast<decltype(api.AllGather)>(dlsym(h, "ncclAllGather"));
+      api.CommUserRank = reinterpret_cast<decltype(api.CommUserRank)>(dlsym(h, "ncclCommUserRank"));
       api.ok = api.GetUniqueId && api.CommInitRank && api.CommDestroy && api.AllReduce;
     }
   }
@@ -870,6 +904,39 @@ int mdt_allreduce_grads(void* comm, void* grad, long long n, int bf16, void* str
   if (!nccl().ok) return MDT_ERR_DRIVER;
   // ncclDataType_t: ncclFloat32 = 7, ncclBfloat16 = 9 ; ncclRedOp_t: ncclSum = 0
   return nccl().AllReduce(grad, grad, static_cast<size_t>(n), bf16 ? 9 : 7, 0, comm, static_cast<cudaStream_t>(stream)) == 0
+             ? MDT_OK
+             : MDT_ERR_CUDA;
+}
+
+int mdt_reduce_scatter_grads(void* comm, void* buf, long long count_per_rank, int bf16, void* stream) {
+  if (!comm || !buf || count_per_rank <= 0) return MDT_ERR_ARG;
+  if (!nccl().ok || !nccl().ReduceScatter || !nccl().CommUserRank) return MDT_ERR_DRIVER;
+  int rank = 0;
+  if (nccl().CommUserRank(comm, &rank) != 0) return MDT_ERR_CUDA;
+  const size_t esz = bf16 ? 2 : 4;
+  char* recv = static_cast<char*>(buf) + static_cast<size_t>(rank) * static_cast<size_t>(count_per_rank) * esz;
+  return nccl().ReduceScatter(buf, recv, static_cast<size_t>(count_per_rank), bf16 ? 9 : 7, 0, comm,
+                              static_cast<cudaStream_t>(stream)) == 0
+             ? MDT_OK
+             : MDT_ERR_CUDA;
+}
+
+int mdt_allgather(void* comm, void* buf, long long count_per_rank, int dtype, void* stream) {
+  if (!comm || !buf || count_per_rank <= 0) return MDT_ERR_ARG;
+  // ncclDataType_t: ncclFloat32 = 7, ncclFloat64 = 8, ncclBfloat16 = 9
+  int nd = 0;
+  size_t esz = 0;
+  switch (dtype) {
+    case MDT_DTYPE_F32: nd = 7, esz = 4; break;
+    case MDT_DTYPE_BF16: nd = 9, esz = 2; break;
+    case MDT_DTYPE_F64: nd = 8, esz = 8; break;
+    default: return MDT_ERR_ARG;
+  }
+  if (!nccl().ok || !nccl().AllGather || !nccl().CommUserRank) return MDT_ERR_DRIVER;
+  int rank = 0;
+  if (nccl().CommUserRank(comm, &rank) != 0) return MDT_ERR_CUDA;
+  const char* send = static_cast<char*>(buf) + static_cast<size_t>(rank) * static_cast<size_t>(count_per_rank) * esz;
+  return nccl().AllGather(send, buf, static_cast<size_t>(count_per_rank), nd, comm, static_cast<cudaStream_t>(stream)) == 0
              ? MDT_OK
              : MDT_ERR_CUDA;
 }

@@ -1309,6 +1309,24 @@ int mdt_power_ema(const float* w, float* const* ema, const float* one_minus_beta
   return launch_status();
 }
 
+// One block row per segment (blockIdx.y), the row's blocks striding over its elements: the sharded optimizer's
+// pack / unpack of the fp32-read set (a few hundred segments, a few MB).
+__global__ void copy_segments_kernel(const float* __restrict__ src, float* __restrict__ dst,
+                                     const long long* __restrict__ seg) {
+  const long long so = seg[3 * blockIdx.y], d = seg[3 * blockIdx.y + 1], n = seg[3 * blockIdx.y + 2];
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.x) * blockDim.x)
+    dst[d + i] = src[so + i];
+}
+
+int mdt_copy_segments_f32(const float* src, float* dst, const long long* seg, int nseg, void* stream) {
+  if (nseg < 0 || nseg > 65535) return MDT_ERR_ARG;
+  if (nseg == 0) return MDT_OK;
+  if (!src || !dst || !seg) return MDT_ERR_ARG;
+  copy_segments_kernel<<<dim3(8, nseg), 256, 0, S(stream)>>>(src, dst, seg);
+  return launch_status();
+}
+
 int mdt_step_front(const float* moments, const float* eps, const float* rnd_normal, const float* noise_unit,
                    const float* drop_u, float drop_prob, float scale_factor, float P_mean, float P_std, float* y,
                    float* yn, float* sigma, float* labels, int B, int C, int R, int num_classes, void* stream) {

@@ -405,6 +405,15 @@ class CEngine:
         """Elements of the trainable region, or of the whole blob (`mdt_model_param_count`)."""
         return self._L.mdt_model_param_count(self._h, int(trainable_only))
 
+    def fp32_read_ranges(self):
+        """[(lo, hi)] of the trainable region that the training step reads from the fp32 masters
+        (`mdt_model_fp32_read_ranges`)."""
+        k = self._L.mdt_model_fp32_read_ranges(self._h, None, 0)
+        ops.check(min(k, 0), "mdt_model_fp32_read_ranges", 0)
+        buf = (ctypes.c_longlong * (2 * max(k, 1)))()
+        ops.check(min(self._L.mdt_model_fp32_read_ranges(self._h, buf, k), 0), "mdt_model_fp32_read_ranges", 0)
+        return [(buf[2 * i], buf[2 * i + 1]) for i in range(k)]
+
     @property
     def num_blocks(self):
         return self.cfg.depth + self.cfg.dec_depth

@@ -474,3 +474,11 @@ def power_ema(w, emas, coeffs):
     check(lib().mdt_power_ema(ptr(w), (ctypes.c_void_p * max(k, 1))(*[e.data_ptr() for e in emas]),
                               (ctypes.c_float * max(k, 1))(*[float(c) for c in coeffs]), k, w.numel(), stream_ptr()),
           "mdt_power_ema")
+
+
+def copy_segments_f32(src, dst, seg):
+    """dst[d:d + c] = src[s:s + c] for every row {s, d, c} of the int64 device table `seg` [k, 3] (fp32 elements of the
+    flat tensors src and dst; the rows must not overlap in dst)."""
+    _c(src, f32), _c(dst, f32), _c(seg, torch.int64)
+    check(lib().mdt_copy_segments_f32(ptr(src), ptr(dst), ptr(seg), seg.shape[0], stream_ptr()),
+          "mdt_copy_segments_f32")

@@ -20,6 +20,8 @@ from . import ops, phema
 from .loss import ECTLoss, EDMLoss
 from .maskdit import EDMPrecond
 
+_GATHER_DTYPES = {torch.float32: 0, torch.bfloat16: 1, torch.float64: 2}   # MDT_DTYPE_F32 / _BF16 / _F64
+
 
 class DataParallelB200:
     """What the reference's loss expects from the DDP wrapper: `.module`, `.training`, callable (loss.py:41,47,52).
@@ -78,6 +80,33 @@ def ar_chunk_bounds(n, k):
     return [(lo, min(n, lo + step)) for lo in range(0, n, step)]
 
 
+SHARD_ALIGN = 64   # elements: 256 B of fp32, the optimizer kernels' float4 and alignment rules
+
+
+def shard_piece(count, world):
+    """Elements per rank of an exchange chunk of `count` elements under `TrainStep(shard_optimizer=True)`: count / world
+    rounded up to a multiple of SHARD_ALIGN."""
+    return -(-(-(-count // world)) // SHARD_ALIGN) * SHARD_ALIGN
+
+
+def owned_ranges(n, world, chunks):
+    """Per rank, the [lo, hi) element ranges of a flat buffer of n elements whose optimizer state the rank owns under
+    `TrainStep(shard_optimizer=True)`: one range per exchange chunk (`ar_chunk_bounds(n, chunks)`), rank r owning piece r
+    of the chunk's split into `world` pieces of `shard_piece(chunk, world)` elements.  So each chunk's reduce-scatter
+    and all-gather are one call with equal counts.  The pieces of the last ranks may run past the chunk's end: the
+    exchange buffer pads them, and their ranges here are clamped to the chunk (shorter, or empty with lo == hi)."""
+    for name, v in (("n", n), ("world", world), ("chunks", chunks)):
+        if isinstance(v, bool) or not isinstance(v, int) or v < 1:
+            raise ValueError(f"owned_ranges: {name} must be an int >= 1, got {v!r}")
+    out = [[] for _ in range(world)]
+    for lo, hi in ar_chunk_bounds(n, chunks):
+        p = shard_piece(hi - lo, world)
+        for r in range(world):
+            a = min(hi, lo + r * p)
+            out[r].append((a, min(hi, a + p)))
+    return out
+
+
 class GradComm:
     """The step's gradient exchange behind the C ABI (`mdt_nccl_*`, `mdt_allreduce_grads`, csrc/driver.cu): an NCCL
     communicator of our own, created from a unique id that rank 0 draws and `torch.distributed` merely ships to the
@@ -102,6 +131,19 @@ class GradComm:
         ops.check(ops.lib().mdt_allreduce_grads(self._comm, t.data_ptr(), t.numel(), int(t.dtype == torch.bfloat16),
                                                 ops.stream_ptr()), "mdt_allreduce_grads", 0)
 
+    def reduce_scatter(self, t, count):
+        """In-place SUM of t (world * count elements) whose share `count` elements at rank * count is this rank's."""
+        assert t.is_cuda and t.is_contiguous() and t.dtype in (torch.float32, torch.bfloat16)
+        assert t.numel() == count * self.world
+        ops.check(ops.lib().mdt_reduce_scatter_grads(self._comm, t.data_ptr(), count, int(t.dtype == torch.bfloat16),
+                                                     ops.stream_ptr()), "mdt_reduce_scatter_grads", 0)
+
+    def all_gather(self, t, count):
+        """In place: every rank's `count` elements at rank * count of t (world * count elements) to every rank."""
+        assert t.is_cuda and t.is_contiguous() and t.dtype in _GATHER_DTYPES and t.numel() == count * self.world
+        ops.check(ops.lib().mdt_allgather(self._comm, t.data_ptr(), count, _GATHER_DTYPES[t.dtype], ops.stream_ptr()),
+                  "mdt_allgather", 0)
+
     def close(self):
         if self._comm:
             ops.lib().mdt_nccl_comm_destroy(self._comm)
@@ -110,6 +152,7 @@ class GradComm:
 
 class TrainStep:
     phema_emas = ()   # no post-hoc EMA profiles unless the constructor is given widths
+    _sh = None        # the sharded layout (shard_optimizer at world > 1)
     edm_loss = None   # the last step's reference per-sample loss (see `step`)
     # consistency tuning (loss_fn an ECTLoss): the stage's device word q^-(s+1) that the step front reads (allocated by
     # the first tuned step), the run step of the first tuned step, and the last step's stage
@@ -121,7 +164,7 @@ class TrainStep:
                  weight_decay=0.0, ema_decay=0.9999, loss_fn: EDMLoss | None = None, process_group=None,
                  lr_rampup_kimg=0.0, global_batch=None, device=None, overlap=False, graph=None,
                  reference_lr_schedule=False, collective=None, grad_dtype=None, skip_nonfinite=False,
-                 recompute_blocks=None, phema_sigma_rels=(), max_grad_norm=None):
+                 recompute_blocks=None, phema_sigma_rels=(), max_grad_norm=None, shard_optimizer=False):
         """max_grad_norm: gradient-norm clipping, torch.nn.utils.clip_grad_norm_'s formula on the device.  None
         (default): off, nothing is allocated or launched.  A float c > 0: every step measures
         norm = grad_scale * ||g||_2 over the trainable region, g being the gradient the optimizer reads (the fp32 flat
@@ -176,6 +219,17 @@ class TrainStep:
           overlap     only False is accepted: the exchange overlapped with the backward was removed (a C caller can
                       still overlap through `mdt_backward`'s `on_ready` callback).  `self.overlap` stays readable
                       and is always False, so code that inspects a TrainStep's configuration keeps working.
+          shard_optimizer  False (default): every rank keeps the whole optimizer state.  True (ZeRO stage 1, needs
+                      collective 'mdt'): the all-reduce is split into its two halves.  Each exchange chunk is
+                      reduce-scattered, each rank runs AdamW, the EMA and the post-hoc EMA profiles on its own piece of
+                      every chunk (`owned_ranges`), then the bf16 shadow is all-gathered, and once per step the ranges
+                      the step reads from the fp32 masters (`CEngine.fp32_read_ranges`).  m, v and the profiles are
+                      allocated at 1/world of the trainable region; the weights, the shadow, the gradient and the EMA
+                      keep their full buffers.  The update is elementwise, so the weights are the replicated step's bit
+                      for bit (the clipping norm may differ by fp64 reassociation).  A rank's fp32 masters outside its
+                      pieces and that set are stale between steps: `materialize()` gathers them and the EMA, and
+                      `state_dict()` / `phema_snapshot()` become collectives that return the replicated layout.
+                      At world 1 the flag changes nothing.
         Environment overrides: MDT_COLLECTIVE, MDT_GRAD_AR, MDT_AR_CHUNKS."""
         if overlap:
             raise ValueError("overlap=True: the gradient exchange overlapped with the backward was removed; the "
@@ -203,8 +257,6 @@ class TrainStep:
         if recompute_blocks is not None:
             self._engine.recompute_blocks = int(recompute_blocks)
         n = self.st.n_train
-        self.m = torch.zeros(n, dtype=torch.float32, device=dev)
-        self.v = torch.zeros(n, dtype=torch.float32, device=dev)
         self.ema_st = None
         if ema is not None:
             self.ema_st = ema.prepare(dev)
@@ -217,12 +269,18 @@ class TrainStep:
             ("mdt" if self.world > 1 and dist.get_backend(process_group) == "nccl" else "torch")
         self.grad_dtype = env.get("MDT_GRAD_AR") or grad_dtype or "bf16"
         assert self.collective in ("mdt", "torch") and self.grad_dtype in ("fp32", "bf16")
+        self.shard_optimizer = bool(shard_optimizer)
+        sharded = self.shard_optimizer and self.world > 1
+        if sharded and self.collective != "mdt":
+            raise ValueError("shard_optimizer=True needs collective='mdt' (the library's own NCCL communicator): the "
+                             "torch.distributed exchange has no reduce-scatter / all-gather path")
+        self.rank = dist.get_rank(process_group) if self.world > 1 else 0
         self.comm = None
         self.g16 = None
         if self.world > 1:
             if self.collective == "mdt":
                 self.comm = GradComm(process_group)
-            if self.grad_dtype == "bf16":
+            if self.grad_dtype == "bf16" and not sharded:
                 self.g16 = torch.empty(n, dtype=torch.bfloat16, device=dev)
         self.graph = (os.environ.get("MDT_TRAIN_GRAPH", "0") == "1") if graph is None else bool(graph)
         self._graphs = {}
@@ -247,10 +305,169 @@ class TrainStep:
         if len(self.phema_sigma_rels) > 4:   # mdt_power_ema advances up to 4 profiles from one read of the weights
             raise ValueError(f"{len(self.phema_sigma_rels)} post-hoc EMA profiles: at most 4")
         self.phema_gammas = tuple(phema.sigma_rel_to_gamma(s) for s in self.phema_sigma_rels)
-        self.phema_emas = [torch.zeros(n, dtype=torch.float32, device=dev) for _ in self.phema_sigma_rels]
+        self._sh = None   # the sharded layout (`_shard_setup`), None when every rank keeps the whole state
+        if sharded:
+            self._shard_setup()
+        else:
+            self.m = torch.zeros(n, dtype=torch.float32, device=dev)
+            self.v = torch.zeros(n, dtype=torch.float32, device=dev)
+            self.phema_emas = [torch.zeros(n, dtype=torch.float32, device=dev) for _ in self.phema_sigma_rels]
         self.phema_origin = None   # run step before the profiles' first update (None: set by the next step)
         self.phema_steps = 0       # updates since the origin (the profiles' t after the last step)
         self._phema_c = None
+
+    # -- sharded optimizer state (shard_optimizer=True) ---------------------------------------------------------------
+    def _shard_setup(self):
+        """Lay out and allocate the sharded state for (world, rank, ar_chunks): per chunk k of `ar_chunk_bounds`, the
+        piece p_k = `shard_piece`, this rank's owned range, the chunk's place in the padded exchange buffer (world * p_k
+        elements) and in the local state (p_k elements: m, v and the profiles); then the fp32-read set's pack tables."""
+        n, W, r, dev = self.st.n_train, self.world, self.rank, self.st.w32.device
+        bounds = ar_chunk_bounds(n, self.ar_chunks)
+        owned = owned_ranges(n, W, self.ar_chunks)
+        pieces = [shard_piece(hi - lo, W) for lo, hi in bounds]
+        xoff, loff = [0], [0]
+        for p in pieces:
+            xoff.append(xoff[-1] + W * p)
+            loff.append(loff[-1] + p)
+        self._sh = sh = type("ShardLayout", (), {})()
+        sh.bounds, sh.pieces, sh.owned, sh.own, sh.xoff, sh.loff = bounds, pieces, owned, owned[r], xoff, loff
+        self.m = self.v = None
+        self.phema_emas = []
+        self.m = torch.zeros(loff[-1], dtype=torch.float32, device=dev)
+        self.v = torch.zeros(loff[-1], dtype=torch.float32, device=dev)
+        self.phema_emas = [torch.zeros(loff[-1], dtype=torch.float32, device=dev) for _ in self.phema_sigma_rels]
+        # the exchange buffer: chunk k at xoff[k], its padding (world * p_k - chunk elements) zero and never read
+        self.g16 = None
+        self.xbuf = torch.zeros(xoff[-1], dtype=torch.bfloat16 if self.grad_dtype == "bf16" else torch.float32,
+                                device=dev)
+        if self.max_grad_norm is not None:   # one fp64 sum of squares per (chunk, rank)
+            self._gn_slots = torch.zeros(len(bounds) * W, dtype=torch.float64, device=dev)
+        # fp32-read set: each rank packs its owned part of the set into its slot of `_rset`, one all-gather, and every
+        # rank unpacks the other ranks' slots into w32
+        read = self._engine.fp32_read_ranges()
+        segs, sizes = [], []
+        for rr in range(W):
+            mine, o = [], 0
+            for a, b in owned[rr]:
+                for lo, hi in read:
+                    lo, hi = max(a, lo), min(b, hi)
+                    if lo < hi:
+                        mine.append((lo, o, hi - lo))
+                        o += hi - lo
+            segs.append(mine)
+            sizes.append(o)
+        P = max(SHARD_ALIGN, -(-max(sizes) // SHARD_ALIGN) * SHARD_ALIGN)
+        sh.read, sh.read_segs, sh.rset_piece = read, segs, P
+        self._rset = torch.zeros(W * P, dtype=torch.float32, device=dev)
+        pack = [(g, r * P + o, c) for g, o, c in segs[r]]
+        unpack = [(rr * P + o, g, c) for rr in range(W) if rr != r for g, o, c in segs[rr]]
+        sh.pack = torch.tensor(pack, dtype=torch.int64).reshape(-1, 3).to(dev)
+        sh.unpack = torch.tensor(unpack, dtype=torch.int64).reshape(-1, 3).to(dev)
+
+    def _xchunk(self, k):
+        sh = self._sh
+        return self.xbuf[sh.xoff[k]:sh.xoff[k + 1]]
+
+    def _fill_x(self, k):
+        """Chunk k of the local fp32 gradient into its exchange slot (bf16: cast, under the guard with the check)."""
+        lo, hi = self._sh.bounds[k]
+        x = self._xchunk(k)
+        if x.dtype == torch.bfloat16:
+            if self._flag is not None:
+                ops.cast_bf16_check(self.st.grad[lo:hi], self._flag, out=x[:hi - lo])
+            else:
+                ops.cast_bf16(self.st.grad[lo:hi], out=x[:hi - lo])
+        else:
+            x[:hi - lo].copy_(self.st.grad[lo:hi])
+            if x.numel() > hi - lo:   # the slot doubled as the shadow's staging last step
+                x[hi - lo:].zero_()
+        return x
+
+    def _own_grad(self, k):
+        """This rank's summed gradient of chunk k (its owned range's elements) in the exchange buffer."""
+        sh = self._sh
+        a, b = sh.own[k]
+        o = sh.xoff[k] + self.rank * sh.pieces[k]
+        return self.xbuf[o:o + b - a]
+
+    def _step_piece(self, k):
+        sh = self._sh
+        a, b = sh.own[k]
+        if b > a:
+            self._step_range(a, b, self._own_grad(k), sh.loff[k])
+
+    def _gather_w16(self, k):
+        """All-gather chunk k of the bf16 shadow: in place, or (a padded chunk, whose last pieces would run past it)
+        staged through the chunk's exchange slot, which the optimizer has read by now."""
+        sh, st, W, r = self._sh, self.st, self.world, self.rank
+        lo, hi = sh.bounds[k]
+        p = sh.pieces[k]
+        if W * p == hi - lo:
+            self.comm.all_gather(st.w16[lo:hi], p)
+            return
+        a, b = sh.own[k]
+        stage = self._xchunk(k).view(torch.bfloat16)[:W * p]
+        stage[r * p:r * p + b - a].copy_(st.w16[a:b])
+        self.comm.all_gather(stage, p)
+        st.w16[lo:hi].copy_(stage[:hi - lo])
+
+    def _gather_chunk(self, k, piece, out):
+        """out (chunk k's hi - lo elements, host or device) = chunk k assembled from every rank's `piece` (its owned
+        range's values): one all-gather through a chunk-sized device temporary."""
+        sh = self._sh
+        lo, hi = sh.bounds[k]
+        p = sh.pieces[k]
+        tmp = torch.zeros(self.world * p, dtype=piece.dtype, device=self.st.w32.device)
+        tmp[self.rank * p:self.rank * p + piece.numel()].copy_(piece)
+        self.comm.all_gather(tmp, p)
+        out.copy_(tmp[:hi - lo])
+
+    def _full(self, local):
+        """A host fp32 tensor of the trainable region holding the replicated layout of the local state `local`
+        (a collective under sharding; a host copy otherwise)."""
+        if self._sh is None:
+            return local.to("cpu", copy=True)
+        sh = self._sh
+        out = torch.empty(self.st.n_train, dtype=torch.float32)
+        for k, ((lo, hi), (a, b)) in enumerate(zip(sh.bounds, sh.own)):
+            self._gather_chunk(k, local[sh.loff[k]:sh.loff[k] + b - a], out[lo:hi])
+        return out
+
+    def _keep(self, local, lo, src):
+        """Store the replicated-layout values src, which start at element lo, into the local state: all of them, or
+        under sharding the part inside this rank's pieces."""
+        if self._sh is None:
+            local[lo:lo + src.numel()].copy_(src)
+            return
+        sh = self._sh
+        for k, (a, b) in enumerate(sh.own):
+            x, y = max(a, lo), min(b, lo + src.numel())
+            if x < y:
+                o = sh.loff[k] + x - a
+                local[o:o + y - x].copy_(src[x - lo:y - lo])
+
+    def materialize(self, ema=True, params=True):
+        """Under sharding, a collective that every rank calls: all-gather the fp32 masters of the EMA network
+        (`ema`) and of the trained network (`params`) into their full buffers, so that host reads (state dicts,
+        validation, sampling) see current values.  The bf16 shadow is current already and is not recast.  Does nothing
+        without sharding."""
+        if self._sh is None:
+            return
+        sh = self._sh
+        flats = ([self.st.w32] if params else []) + ([self.ema_st.w32] if ema and self.ema_st is not None else [])
+        with torch.no_grad():
+            for w in flats:
+                for k, ((lo, hi), (a, b)) in enumerate(zip(sh.bounds, sh.own)):
+                    self._gather_chunk(k, w[a:b], w[lo:hi])
+        if params:   # the writes went through views of the parameters' storage: the shadow already holds these values
+            self.st.mark_shadow_fresh(self.net._params())
+        if ema and self.ema_st is not None:
+            self.ema_st._versions = None
+
+    @property
+    def sharded(self) -> bool:
+        """Whether the optimizer state is sharded across the ranks (`shard_optimizer` at world > 1)."""
+        return self._sh is not None
 
     @property
     def recompute_blocks(self) -> int:
@@ -288,17 +505,20 @@ class TrainStep:
         (`applied_steps()`): under `skip_nonfinite` it leaves out the skipped steps.
         With power-function EMA profiles, `phema` holds their widths, exponents, origin, step count and flat buffers
         (host copies: the device keeps no second copy of them).  Under consistency tuning, `ect` holds the tuning
-        origin, so a resumed run continues the stage."""
+        origin, so a resumed run continues the stage.
+        Under `shard_optimizer` this is a collective that every rank calls.  It returns the replicated layout and
+        values, gathered chunk by chunk into host tensors (no full-size device temporary)."""
         state, n_all = {}, 0
         adam_step = self.applied_steps()
+        m, v = (self.m, self.v) if self._sh is None else (self._full(self.m), self._full(self.v))
         for i, (k, p) in enumerate(self.net.named_parameters()):
             n_all = i + 1
             if not p.requires_grad:
                 continue
             lo, _, shape = self.st.offsets[k]
             n = p.numel()
-            state[i] = {"step": torch.tensor(float(adam_step)), "exp_avg": self.m[lo:lo + n].view(shape).clone(),
-                        "exp_avg_sq": self.v[lo:lo + n].view(shape).clone()}
+            state[i] = {"step": torch.tensor(float(adam_step)), "exp_avg": m[lo:lo + n].view(shape).clone(),
+                        "exp_avg_sq": v[lo:lo + n].view(shape).clone()}
         sd = {"state": state,
               "param_groups": [{"lr": self.lr, "betas": self.betas, "eps": self.eps, "weight_decay": self.wd,
                                 "step": adam_step, "params": list(range(n_all))}]}
@@ -307,13 +527,15 @@ class TrainStep:
         if self.phema_emas:
             sd["phema"] = {"sigma_rels": list(self.phema_sigma_rels), "gammas": list(self.phema_gammas),
                            "origin": self.phema_origin, "steps": self.phema_steps,
-                           "emas": [e.to("cpu", copy=True) for e in self.phema_emas]}
+                           "emas": [self._full(e) for e in self.phema_emas]}
         return sd
 
     def load_state_dict(self, sd):
         """Accepts (a) this class's own layout, (b) `torch.optim.AdamW(model.parameters()).state_dict()`, (c) apex
         FusedAdam's (same indexing, `step` only in the param_group) and (d) round-1 checkpoints of this repo (compact
-        indices over the trainable parameters + `param_names`)."""
+        indices over the trainable parameters + `param_names`).  Under `shard_optimizer` a rank keeps the part of
+        the (full-layout) state inside its pieces, so states move between world sizes and between sharded and
+        replicated runs."""
         state = {int(k): v for k, v in sd["state"].items()}
         group = sd["param_groups"][0]
         named = list(self.net.named_parameters())
@@ -336,9 +558,8 @@ class TrainStep:
             lo, _, shape = self.st.offsets[k]
             if tuple(e["exp_avg"].shape) != tuple(shape):
                 raise ValueError(f"optimizer state of {k}: shape {tuple(e['exp_avg'].shape)} != {tuple(shape)}")
-            n = e["exp_avg"].numel()
-            self.m[lo:lo + n].copy_(e["exp_avg"].reshape(-1))
-            self.v[lo:lo + n].copy_(e["exp_avg_sq"].reshape(-1))
+            self._keep(self.m, lo, e["exp_avg"].reshape(-1).to(self.m.device))
+            self._keep(self.v, lo, e["exp_avg_sq"].reshape(-1).to(self.v.device))
             if "step" in e:
                 step = e["step"]
         if step is None:
@@ -365,17 +586,19 @@ class TrainStep:
             raise ValueError(f"the state holds post-hoc EMA profiles of sigma_rel {list(ph['sigma_rels'])}, this "
                              f"TrainStep keeps {list(self.phema_sigma_rels)}")
         for e, src in zip(self.phema_emas, ph["emas"]):
-            if src.numel() != e.numel():
-                raise ValueError(f"post-hoc EMA profile of {src.numel()} elements, the model trains {e.numel()}")
-            e.copy_(src.reshape(-1))
+            if src.numel() != self.st.n_train:
+                raise ValueError(f"post-hoc EMA profile of {src.numel()} elements, the model trains "
+                                 f"{self.st.n_train}")
+            self._keep(e, 0, src.reshape(-1).to(e.device))
         self.phema_origin, self.phema_steps = int(ph["origin"]), int(ph["steps"])
 
     # -- power-function EMA profiles (post-hoc EMA) ----------------------------------------------------------------
     def phema_state_dicts(self):
-        """The profiles as model state dicts with the module's keys (host copies; frozen tensors from the weights)."""
+        """The profiles as model state dicts with the module's keys (host copies; frozen tensors from the weights).  A
+        collective under sharding."""
         out = []
         for e in self.phema_emas:
-            flat = e.to("cpu", copy=True)   # one host storage per profile; the trainable tensors are views into it
+            flat = self._full(e)   # one host storage per profile; the trainable tensors are views into it
             sd = {}
             for k, v in self.net.state_dict().items():
                 o, cnt, shape = self.st.offsets.get(k, (None, None, None))
@@ -388,7 +611,8 @@ class TrainStep:
 
     def phema_snapshot(self):
         """What post-hoc EMA reconstruction reads: {step, origin, profiles: [{sigma_rel, gamma, ema}]}, where step is
-        the run step of the last update and each ema a state dict."""
+        the run step of the last update and each ema a state dict.  A collective under sharding, with the replicated
+        run's layout and values."""
         if self.phema_origin is None:
             raise ValueError("the post-hoc EMA profiles have not been updated yet")
         return {"step": self.phema_origin + self.phema_steps, "origin": self.phema_origin,
@@ -405,6 +629,11 @@ class TrainStep:
     def describe_collective(self):
         if self.world == 1:
             return "none (1 GPU)"
+        if self._sh is not None:
+            return (f"sharded optimizer state (rank {self.rank} of {self.world}): {self.grad_dtype} reduce-scatter of "
+                    f"the flat gradient buffer in {len(self._sh.bounds)} chunks on a side stream, the optimizer on "
+                    f"this rank's piece of each chunk, then an all-gather of the bf16 shadow and one of the fp32-read "
+                    f"set, own NCCL communicator behind the C ABI (mdt_reduce_scatter_grads, mdt_allgather)")
         how = "own NCCL communicator behind the C ABI (mdt_allreduce_grads)" if self.comm else "torch.distributed"
         when = f"after the backward in {self.ar_chunks} chunks on a side stream, pipelined with the optimizer pass" \
             if self.ar_chunks > 1 else "one flat call after the backward"
@@ -439,24 +668,85 @@ class TrainStep:
         ops.grad_clip_coef(self._gn_slots[:k], self._grad_scale, self.max_grad_norm, self._gn[:1], self._gn[1:],
                            flag=self._flag if self._clips() else None)
 
-    def _step_range(self, lo, hi):
+    def _step_range(self, lo, hi, g=None, s=None):
+        """The optimizer pass over weights [lo, hi): gradient `g` (default: the range of the summed buffer), moments
+        and profiles from element `s` of the local state (default lo: the whole state is local)."""
         st, n = self.st, hi - lo
         if n <= 0:
             return
-        g = self.g16[lo:hi] if (self.g16 is not None and self.world > 1) else st.grad[lo:hi]
+        if g is None:
+            g = self.g16[lo:hi] if (self.g16 is not None and self.world > 1) else st.grad[lo:hi]
+        s = lo if s is None else s
+        m, v = self.m[s:s + n], self.v[s:s + n]
         ema = self.ema_st.w32[lo:hi] if self.ema_st is not None else None
         # a finite clipping bound: the optimizer reads the coefficient (c = inf keeps the plain kernels)
         coef = self._gn[1:] if self._clips() else None
         if self._flag is not None:   # Adam's step number comes from the device counter, the skip from the flag
-            ops.adamw_ema_guarded(st.w32[lo:hi], g, self.m[lo:hi], self.v[lo:hi], ema, st.w16[lo:hi], n, self._lr_now,
+            ops.adamw_ema_guarded(st.w32[lo:hi], g, m, v, ema, st.w16[lo:hi], n, self._lr_now,
                                   self._flag, self._counts, self.betas[0], self.betas[1], self.eps, self.wd,
                                   self.ema_decay, self._grad_scale, coef=coef)
         else:
-            ops.adamw_ema(st.w32[lo:hi], g, self.m[lo:hi], self.v[lo:hi], ema, st.w16[lo:hi], n, self._lr_now,
+            ops.adamw_ema(st.w32[lo:hi], g, m, v, ema, st.w16[lo:hi], n, self._lr_now,
                           self.step_count, self.betas[0], self.betas[1], self.eps, self.wd, self.ema_decay,
                           self._grad_scale, coef=coef)
         if self.phema_emas:   # the profiles follow the range's new (or, skipped, unchanged) weights on the same stream
-            ops.power_ema(st.w32[lo:hi], [e[lo:hi] for e in self.phema_emas], self._phema_c)
+            ops.power_ema(st.w32[lo:hi], [e[s:s + n] for e in self.phema_emas], self._phema_c)
+
+    def _sharded_exchange_step(self, guard, measure):
+        """Reduce-scatter -> optimizer on the owned pieces -> all-gather, chunk by chunk.  Every collective runs on the
+        exchange stream in the same order on every rank; the optimizer pass of chunk k runs on the main stream while
+        chunk k+1 is on the wire, and the shadow of chunk k is gathered while chunk k+1 is stepped."""
+        st, sh, W, r = self.st, self._sh, self.world, self.rank
+        main = torch.cuda.current_stream()
+        if self.side is None:
+            self.side = torch.cuda.Stream(device=st.grad.device)
+        self.side.wait_stream(main)
+        evs = []
+        with torch.cuda.stream(self.side):
+            cast_first = guard and self.xbuf.dtype == torch.bfloat16
+            if guard:   # chunk 0's optimizer pass needs the decision: check every local chunk first
+                if cast_first:
+                    for k in range(len(sh.bounds)):
+                        self._fill_x(k)
+                else:
+                    ops.nonfinite_check(st.grad[:st.n_train], self._flag)
+                self._all_reduce(self._flag)
+            for k in range(len(sh.bounds)):
+                x = self._xchunk(k) if cast_first else self._fill_x(k)
+                self.comm.reduce_scatter(x, sh.pieces[k])
+                ev = torch.cuda.Event()
+                ev.record(self.side)
+                evs.append(ev)
+                if measure:   # this rank's sum of squares of the chunk, then every rank's, in (chunk, rank) order
+                    slot = self._gn_slots[k * W + r:k * W + r + 1]
+                    g = self._own_grad(k)
+                    if g.numel():
+                        ops.grad_sumsq(g, slot, self._gn_scratch)
+                    else:
+                        slot.zero_()
+                    self.comm.all_gather(self._gn_slots[k * W:(k + 1) * W], 1)
+            if measure:
+                self._grad_norm_coef(len(sh.bounds) * W)
+        if self._clips():   # clipping needs the global norm: every chunk's pass waits for the coefficient
+            main.wait_stream(self.side)
+            evs = [None] * len(sh.bounds)
+        stepped = []
+        for k, ev in enumerate(evs):
+            if ev is not None:
+                main.wait_event(ev)
+            self._step_piece(k)
+            done = torch.cuda.Event()
+            done.record(main)
+            stepped.append(done)
+        with torch.cuda.stream(self.side):
+            for k, done in enumerate(stepped):
+                self.side.wait_event(done)
+                self._gather_w16(k)
+            # the masters the step reads in fp32, from every rank's pieces
+            ops.copy_segments_f32(st.w32, self._rset, sh.pack)
+            self.comm.all_gather(self._rset, sh.rset_piece)
+            ops.copy_segments_f32(self._rset, st.w32, sh.unpack)
+        main.wait_stream(self.side)
 
     def _fwd_bwd_graphed(self, images, labels, mask_ratio, mae_loss_coef, loss_call, moments=False):
         """Gradient zeroing + loss forward + engine backward (~770 launches, 70 ms of host time) replayed from a CUDA
@@ -599,6 +889,8 @@ class TrainStep:
             elif guard:
                 ops.nonfinite_check(st.grad[:n], self._flag)
             self._step_range(0, n)
+        elif self._sh is not None:
+            self._sharded_exchange_step(guard, measure)
         else:
             # pipeline the exposed all-reduce against the optimizer pass: chunk k is stepped while k+1 is on the wire
             if self.side is None:

@@ -125,6 +125,10 @@ def build_parser():
     ap.add_argument("--max_grad_norm", type=parse_max_grad_norm, default=None,
                     help="clip the global gradient norm to this bound (torch's clip_grad_norm_; 'inf' only measures) "
                          "and log its mean and max over each logging window")
+    ap.add_argument("--shard_optimizer", action="store_true",
+                    help="keep AdamW's moments and the post-hoc EMA profiles sharded across the data-parallel ranks "
+                         "(each rank updates 1/world of the weights and the EMA, then the shadow is all-gathered); "
+                         "checkpoints and snapshots keep the replicated format")
     ap.add_argument("--val_every", type=int, default=0,
                     help="every N steps, print the held-out denoising loss of the EMA (0: off)")
     ap.add_argument("--val_count", type=int, default=1000,
@@ -190,7 +194,7 @@ def main():
     ts = TrainStep(net, ema, lr=cfg.train.lr, lr_rampup_kimg=cfg.train.lr_rampup_kimg, global_batch=global_batch,
                    loss_fn=loss_fn, reference_lr_schedule=True,
                    skip_nonfinite=skip_nonfinite(args), phema_sigma_rels=args.phema_sigma_rel,
-                   max_grad_norm=args.max_grad_norm)
+                   max_grad_norm=args.max_grad_norm, shard_optimizer=args.shard_optimizer)
     if ck and strict and "opt" in sd:                      # train.py:150: optimizer state only under strict loading
         ts.load_state_dict(sd["opt"])
     ts.lr_step_offset = step0 - ts.step_count              # lr follows the run's step counter (train.py:223)
@@ -279,26 +283,32 @@ def main():
             gn_sum = gn_max = None
         if held is not None and step % args.val_every == 0:
             from maskdit_b200.validate import validate
+            ts.materialize(params=False)   # sharded: the EMA's masters from every rank (a no-op otherwise)
             # eager, fixed draws from their own generators: the training step's RNG stream and memory plan are untouched
             res = validate(ema, held, levels=args.val_levels, batch=micro_batch)
             if rank == 0:
                 u = ema.logvar(res["sigma"]).tolist() if ema.logvar_channels else None
                 print(val_line(step, res, u), flush=True)
         if step % cfg.log.ckpt_every == 0 and step > step0:
+            # sharded: every rank gathers the masters, the EMA and the optimizer state (collectives); rank 0 writes
+            ts.materialize()
+            opt = ts.state_dict() if rank == 0 or ts.sharded else None
             if rank == 0:
                 d = os.path.join(args.results_dir, "checkpoints")
                 os.makedirs(d, exist_ok=True)
-                torch.save({"model": net.state_dict(), "ema": ema.state_dict(), "opt": ts.state_dict(), "args": args},
+                torch.save({"model": net.state_dict(), "ema": ema.state_dict(), "opt": opt, "args": args},
                            os.path.join(d, f"{step:07d}.pt"))
             if world > 1:
                 dist.barrier()
-        if args.phema_every and step % args.phema_every == 0 and step > step0 and rank == 0:
-            # every rank holds the same profiles; rank 0 writes them
-            d = os.path.join(args.results_dir, "phema")
-            os.makedirs(d, exist_ok=True)
-            path = os.path.join(d, f"phema-{step:07d}.pt")
-            torch.save(ts.phema_snapshot(), path)
-            print(f"(step={step:07d}) Post-hoc EMA snapshot (origin {ts.phema_origin}): {path}", flush=True)
+        if args.phema_every and step % args.phema_every == 0 and step > step0:
+            # rank 0 writes the profiles; sharded, every rank takes part in gathering them
+            snap = ts.phema_snapshot() if rank == 0 or ts.sharded else None
+            if rank == 0:
+                d = os.path.join(args.results_dir, "phema")
+                os.makedirs(d, exist_ok=True)
+                path = os.path.join(d, f"phema-{step:07d}.pt")
+                torch.save(snap, path)
+                print(f"(step={step:07d}) Post-hoc EMA snapshot (origin {ts.phema_origin}): {path}", flush=True)
     if world > 1:
         dist.destroy_process_group()
 
