@@ -22,7 +22,9 @@ noise level, and refuses the ablation switches, `--S_churn` and flow configs.  `
 flow config with `dpm_solver_sampler` (multistep DPM-Solver++: DDIM, 2M or 3M) in `--num_steps` network evaluations,
 with `--cfg_scale`, autoguidance (EDM) and `--guidance_interval` as above, and refuses the ablation switches, `--S_churn`
 and `--consistency_sigmas`.  Class-unconditional configs sample with all-zero label rows as the reference does
-(sample.py:261-264).
+(sample.py:261-264).  A network trained with model guidance (train.py with `train.objective: mg`) outputs the guided
+denoiser itself: every sampler above samples it guided without `--cfg_scale`, at one network pass per evaluation, and
+`--cfg_scale` on top compounds the two guidances.
 """
 import argparse
 import os

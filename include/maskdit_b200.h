@@ -274,6 +274,29 @@ int mdt_ect_loss(const float* Ft, const float* Fr, const float* xt, const float*
                  const float* r, const float* mask, const float* gl, float sigma_data, float c, float mae_coef,
                  float* loss, float* D_t, void* dF_bf16, int B, int C, int R, int p, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Model guidance (MG; the definition is DESIGN §5): the conditional network learns the guided denoiser.
+ * mdt_mg_loss: F [B,L,p*p*C] the student's output (conditional, gradient-carrying) ; Fu the no-gradient output of the
+ *   same weights on the same xin, sigma and kept tokens with the null (all-zero) label row ; labels [B,num_classes] the
+ *   student's label rows (a row is kept when any entry is non-zero).  Per row: w_b = w when the label row is kept and
+ *   lo < sigma[b] <= hi, else 0 ; target = y + w_b c_out (F - Fu), and where w_b = 0 exactly y (a select: Fu of such a
+ *   row is never read into the result).  loss[b] is mdt_edm_loss's loss with y replaced by the target in the
+ *   denoising term (the MAE term unchanged) ; dF_bf16 (optional, needs gl) = d(sum_b gl[b] loss[b]) / dF with the
+ *   target held constant ; edm_loss (optional) [B] = mdt_edm_loss's loss against y, bit for bit ; Dx as mdt_edm_loss.
+ *   With w_b = 0 on every row, loss and dF_bf16 are mdt_edm_loss's bits.  0 <= w < 1 (w = 1 - 1/s for the
+ *   CFG-equivalent scale s), lo < hi.  The pd rules are mdt_edm_loss's.
+ * mdt_flow_mg_loss: the same on velocities for mdt_flow_loss: target v' = (eps - y) + w_b (F - Fu), the interval on t,
+ *   edm_loss = mdt_flow_loss's loss bit for bit, x_hat as there.
+ * ------------------------------------------------------------------------------------------------------------ */
+int mdt_mg_loss(const float* F, const float* Fu, const float* xin, const float* y, const float* sigma,
+                const float* labels, int num_classes, const float* mask, const float* gl, float sigma_data,
+                float mae_coef, float w, float lo, float hi, float* loss, float* edm_loss, float* Dx, void* dF_bf16,
+                int B, int C, int R, int p, void* stream);
+int mdt_flow_mg_loss(const float* F, const float* Fu, const float* xt, const float* y, const float* eps,
+                     const float* t, const float* labels, int num_classes, const float* mask, const float* gl,
+                     float mae_coef, float w, float lo, float hi, float* loss, float* edm_loss, float* x_hat,
+                     void* dF_bf16, int B, int C, int R, int p, void* stream);
+
 /* D only (sampler / generic autograd path): Dx = c_skip*xin + c_out*unpatchify(F); and its backward
  * dF_bf16 = c_out * patchify(gD).                                                                            */
 int mdt_edm_precond_out(const float* F, const float* xin, const float* sigma, float sigma_data, float* Dx, int B,

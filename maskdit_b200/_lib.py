@@ -95,6 +95,8 @@ _SIGS = {
     "mdt_ect_step_front": [_P, _P, _P, _P, _P, _F, _F, _F, _F, _P, _F, _F, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I,
                            _P],
     "mdt_ect_loss": [_P, _P, _P, _P, _P, _P, _P, _P, _P, _F, _F, _F, _P, _P, _P, _I, _I, _I, _I, _P],
+    "mdt_mg_loss": [_P, _P, _P, _P, _P, _P, _I, _P, _P, _F, _F, _F, _F, _F, _P, _P, _P, _P, _I, _I, _I, _I, _P],
+    "mdt_flow_mg_loss": [_P, _P, _P, _P, _P, _P, _P, _I, _P, _P, _F, _F, _F, _F, _P, _P, _P, _P, _I, _I, _I, _I, _P],
     "mdt_edm_precond_out": [_P, _P, _P, _F, _P, _I, _I, _I, _I, _P],
     "mdt_edm_precond_out_bwd": [_P, _P, _F, _P, _I, _I, _I, _I, _P],
     "mdt_cfg_precond_out": [_P, _P, _P, _F, _F, _P, _I, _I, _I, _I, _P],

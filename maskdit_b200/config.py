@@ -87,31 +87,63 @@ def build_net(cfg: Node, **extra):
 
 
 ECT_KEYS = ("stage_steps", "q", "k", "b", "P_mean", "P_std")
+MG_KEYS = ("scale", "interval")
+OBJECTIVE_BLOCKS = ("ect", "mg")
 
 
 def build_loss(cfg: Node):
     """The training loss of a config: `Losses[model.precond]()` as train.py:137 builds it, or, with
     `train.objective: ect`, Easy Consistency Tuning (`Losses['ect']`) of an EDM network with the `train.ect` block's
-    `stage_steps` (required), `q`, `k`, `b`, `P_mean` and `P_std`.  An absent `train.objective` is the precond's own
-    objective.  Raises ValueError for a combination that cannot train."""
+    `stage_steps` (required), `q`, `k`, `b`, `P_mean` and `P_std`, or, with `train.objective: mg`, model guidance
+    (`Losses['mg']`) of a class-conditional EDM or flow network with the `train.mg` block's `scale` (required, >= 1,
+    the CFG-equivalent scale) and `interval: [lo, hi]` (the noise levels, or flow times, that are guided; default
+    all).  An absent `train.objective` is the precond's own objective.  Raises ValueError for a combination that cannot
+    train."""
     from .loss import Losses
     m, tr = cfg.model, cfg.get("train") or Node()
     obj = tr.get("objective", None)
-    block = tr.get("ect", None)
+    given = [k for k in OBJECTIVE_BLOCKS if tr.get(k, None) is not None]
+    for k in given:
+        if obj != k:
+            what = "consistency tuning" if k == "ect" else "model guidance"
+            raise ValueError(f"train.{k} configures {what}: set train.objective: {k}")
     if obj in (None, m.precond):
-        if block is not None:
-            raise ValueError("train.ect configures consistency tuning: set train.objective: ect")
         return Losses[m.precond]()
-    if obj != "ect":
-        raise ValueError(f"unknown train.objective {obj!r} (the precond's own, or 'ect')")
+    if obj not in OBJECTIVE_BLOCKS:
+        raise ValueError(f"unknown train.objective {obj!r} (the precond's own, 'ect' or 'mg')")
+    if int(m.get("logvar_channels", 0) or 0):
+        raise ValueError(f"train.objective: {obj} does not train a learned loss weighting: drop model.logvar_channels")
+    if obj == "mg":
+        return _build_mg(m, tr.get("mg", None))
     if m.precond != "edm":
         raise ValueError(f"train.objective: ect tunes an EDM network, not model.precond: {m.precond}")
-    if int(m.get("logvar_channels", 0) or 0):
-        raise ValueError("train.objective: ect does not train a learned loss weighting: drop model.logvar_channels")
-    block = dict(block or {})
+    block = dict(tr.get("ect", None) or {})
     unknown = sorted(set(block) - set(ECT_KEYS))
     if unknown:
         raise ValueError(f"unknown train.ect keys {unknown} (known: {list(ECT_KEYS)})")
     if block.get("stage_steps") is None:
         raise ValueError("train.objective: ect needs train.ect.stage_steps (steps per tuning stage)")
     return Losses["ect"](**block)
+
+
+def _build_mg(m, block):
+    from .loss import Losses
+    if m.precond not in ("edm", "flow"):
+        raise ValueError(f"train.objective: mg trains an EDM or flow network, not model.precond: {m.precond}")
+    if not int(m.get("num_classes", 0) or 0):
+        raise ValueError("train.objective: mg guides a class-conditional network: model.num_classes is 0")
+    if not float(m.get("class_dropout_prob", 0) or 0) > 0:
+        raise ValueError("train.objective: mg needs model.class_dropout_prob > 0: the null-label output it guides "
+                         "against is only trained on the dropped labels")
+    block = dict(block or {})
+    unknown = sorted(set(block) - set(MG_KEYS))
+    if unknown:
+        raise ValueError(f"unknown train.mg keys {unknown} (known: {list(MG_KEYS)})")
+    if block.get("scale") is None:
+        raise ValueError("train.objective: mg needs train.mg.scale (the CFG-equivalent scale, >= 1)")
+    interval = block.get("interval")
+    if interval is not None:
+        if not isinstance(interval, (list, tuple)) or len(interval) != 2:
+            raise ValueError(f"train.mg.interval must be [lo, hi], got {interval!r}")
+        interval = (float(interval[0]), float(interval[1]))
+    return Losses["mg"](scale=float(block["scale"]), interval=interval)

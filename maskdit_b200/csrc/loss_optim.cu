@@ -353,6 +353,244 @@ ect_loss_kernel(const float* __restrict__ Ft, const float* __restrict__ Fr, cons
   }
 }
 
+// ---- Model guidance (DESIGN §5) -----------------------------------------------------------------------------------------
+// F is the student's output (gradient-carrying, conditional) and Fu the no-gradient output of the same weights on the
+// same input and kept tokens with the null (all-zero) label row.  Row b is guided with w_b = w when its label row is
+// non-zero and lo < level_b <= hi, else w_b = 0.  Its target is the plain target plus w_b c_out (F - Fu) (EDM) or
+// w_b (F - Fu) (flow); where w_b = 0 it is the plain target itself, a select that never reads Fu.
+struct MgArgs {
+  const float* Fu;      // [B, L, pd]
+  const float* labels;  // [B, nc]
+  int nc;
+  float w, lo, hi;
+  float* edm_loss;      // [B] optional: the plain loss against the unguided target
+};
+
+// w_b of sample b, in every thread of the block.
+MDT_DEVINL float mg_weight(const MgArgs& mg, int b, float level) {
+  int nz = 0;
+  for (int k = threadIdx.x; k < mg.nc; k += blockDim.x) nz |= mg.labels[static_cast<size_t>(b) * mg.nc + k] != 0.f;
+  const bool kept = __syncthreads_or(nz) != 0;
+  return (kept && level > mg.lo && level <= mg.hi) ? mg.w : 0.f;
+}
+
+// edm_loss_kernel<kReg, false> with the guided target.  The plain sums (`edm_loss`) are formed with the same operations
+// in the same order, and a row with w_b = 0 takes the plain error, so there `loss` and dF are edm_loss_kernel's bits.
+template <bool kReg>
+__global__ void __launch_bounds__(256)
+mg_loss_kernel(const float* __restrict__ F, const float* __restrict__ xin, const float* __restrict__ y,
+               const float* __restrict__ sigma, const float* __restrict__ mask, const float* __restrict__ gl,
+               float sd, float mae_coef, float* __restrict__ loss, float* __restrict__ Dx,
+               __nv_bfloat16* __restrict__ dF, PatchGeom gm, MgArgs mg) {
+  __shared__ float s_buf[32];
+  const int b = blockIdx.x;
+  const float sg = sigma[b];
+  const float den = sg * sg + sd * sd;
+  const float c_skip = sd * sd / den, c_out = sg * sd * rsqrtf(den);
+  const float w = den / ((sg * sd) * (sg * sd));
+  const float glb = gl ? gl[b] : 0.f;
+  const float wb = mg_weight(mg, b, sg);
+  const bool guided = wb != 0.f;
+  float n_mask = 0.f;
+  if (mask) {
+    float cnt = 0.f;
+    for (int l = threadIdx.x; l < gm.L; l += blockDim.x) cnt += mask[static_cast<size_t>(b) * gm.L + l];
+    n_mask = block_sum(cnt, s_buf);
+  }
+  const float n_keep = static_cast<float>(gm.L) - n_mask;
+  float acc = 0.f, acc_g = 0.f;   // the plain and the guided sums
+  for (int l = threadIdx.x; l < gm.L; l += blockDim.x) {
+    const float* f = F + (static_cast<size_t>(b) * gm.L + l) * gm.pd;
+    const float* fu = mg.Fu + (static_cast<size_t>(b) * gm.L + l) * gm.pd;
+    float dv[kReg ? kMaxPD : 1], xv[kReg ? kMaxPD : 1];
+    auto xat = [&](int j) -> float {
+      if constexpr (kReg) return xv[j];
+      else return xin[gm.pix(b, l, j)];
+    };
+    auto dat = [&](int j) -> float {
+      if constexpr (kReg) return dv[j];
+      else return c_skip * xin[gm.pix(b, l, j)] + c_out * f[j];
+    };
+    auto tat = [&](int j) -> float {   // the target of element j
+      const float yv = y[gm.pix(b, l, j)];
+      if (!guided) return yv;
+      return yv + wb * (c_out * (f[j] - fu[j]));
+    };
+    float se = 0.f, sx = 0.f, sq = 0.f;
+    for (int j = 0; j < gm.pd; ++j) {
+      const size_t px = gm.pix(b, l, j);
+      const float xi = xin[px];
+      const float d = c_skip * xi + c_out * f[j];
+      if (Dx) Dx[px] = d;
+      const float e = d - y[px];
+      if constexpr (kReg) dv[j] = d, xv[j] = xi;
+      se += e * e, sx += xi;
+      if (guided) {
+        const float eg = d - tat(j);
+        sq += eg * eg;
+      }
+    }
+    if (!guided) sq = se;
+    const float inv_pd = 1.f / gm.pd;
+    if (!mask) {
+      acc += w * se;  // mean over all elements of the sample, applied below
+      acc_g += w * sq;
+      if (dF) {
+        const float k = glb * w * 2.f * c_out / (static_cast<float>(gm.L) * gm.pd);
+        for (int j = 0; j < gm.pd; ++j)
+          dF[(static_cast<size_t>(b) * gm.L + l) * gm.pd + j] = __float2bfloat16_rn(k * (dat(j) - tat(j)));
+      }
+    } else {
+      const float mk = mask[static_cast<size_t>(b) * gm.L + l];
+      float contrib = (1.f - mk) * w * se * inv_pd / n_keep;
+      float contrib_g = guided ? (1.f - mk) * w * sq * inv_pd / n_keep : contrib;
+      float k_edm = glb * (1.f - mk) / n_keep * w * 2.f * inv_pd * c_out;
+      float k_mae = 0.f, mu = 0.f, rstd = 0.f;
+      if (mae_coef > 0.f && mk != 0.f) {
+        // MaskDiT's MAE term, unchanged: target = per-patch normalised noisy input, unbiased variance
+        mu = sx * inv_pd;
+        float var = 0.f;
+        for (int j = 0; j < gm.pd; ++j) var += (xat(j) - mu) * (xat(j) - mu);
+        var /= static_cast<float>(gm.pd - 1);
+        rstd = rsqrtf(var + 1e-6f);
+        float sm = 0.f;
+        for (int j = 0; j < gm.pd; ++j) {
+          const float e = dat(j) - (xat(j) - mu) * rstd;
+          sm += e * e;
+        }
+        const float m = mae_coef * mk * sm * inv_pd / n_mask;
+        contrib += m;
+        contrib_g += m;
+        k_mae = glb * mae_coef * mk / n_mask * 2.f * inv_pd * c_out;
+      }
+      acc += contrib;
+      acc_g += contrib_g;
+      if (dF) {
+        for (int j = 0; j < gm.pd; ++j) {
+          const float dj = dat(j);
+          float gval = k_edm * (dj - tat(j));
+          if (k_mae != 0.f) gval += k_mae * (dj - (xat(j) - mu) * rstd);
+          dF[(static_cast<size_t>(b) * gm.L + l) * gm.pd + j] = __float2bfloat16_rn(gval);
+        }
+      }
+    }
+  }
+  const float tot = block_sum(acc_g, s_buf);
+  if (threadIdx.x == 0) loss[b] = mask ? tot : tot / (static_cast<float>(gm.L) * gm.pd);
+  if (mg.edm_loss) {
+    const float tp = block_sum(acc, s_buf);
+    if (threadIdx.x == 0) mg.edm_loss[b] = mask ? tp : tp / (static_cast<float>(gm.L) * gm.pd);
+  }
+}
+
+// flow_loss_kernel<kReg> with the guided velocity target v' = (eps - x) + w_b (F - Fu), the interval on t; the same bit
+// rules as mg_loss_kernel.
+template <bool kReg>
+__global__ void __launch_bounds__(256)
+flow_mg_loss_kernel(const float* __restrict__ F, const float* __restrict__ xt, const float* __restrict__ y,
+                    const float* __restrict__ eps, const float* __restrict__ tt, const float* __restrict__ mask,
+                    const float* __restrict__ gl, float mae_coef, float* __restrict__ loss, float* __restrict__ Dx,
+                    __nv_bfloat16* __restrict__ dF, PatchGeom gm, MgArgs mg) {
+  __shared__ float s_buf[32];
+  const int b = blockIdx.x;
+  const float tb = tt[b];
+  const float glb = gl ? gl[b] : 0.f;
+  const float wb = mg_weight(mg, b, tb);
+  const bool guided = wb != 0.f;
+  float n_mask = 0.f;
+  if (mask) {
+    float cnt = 0.f;
+    for (int l = threadIdx.x; l < gm.L; l += blockDim.x) cnt += mask[static_cast<size_t>(b) * gm.L + l];
+    n_mask = block_sum(cnt, s_buf);
+  }
+  const float n_keep = static_cast<float>(gm.L) - n_mask;
+  float acc = 0.f, acc_g = 0.f;
+  for (int l = threadIdx.x; l < gm.L; l += blockDim.x) {
+    const float* f = F + (static_cast<size_t>(b) * gm.L + l) * gm.pd;
+    const float* fu = mg.Fu + (static_cast<size_t>(b) * gm.L + l) * gm.pd;
+    float ev[kReg ? kMaxPD : 1], xv[kReg ? kMaxPD : 1];
+    auto xat = [&](int j) -> float {
+      if constexpr (kReg) return xv[j];
+      else return xt[gm.pix(b, l, j)];
+    };
+    auto eat = [&](int j) -> float {   // v^ - v
+      if constexpr (kReg) return ev[j];
+      else {
+        const size_t px = gm.pix(b, l, j);
+        return f[j] - (eps[px] - y[px]);
+      }
+    };
+    auto gat = [&](int j) -> float {   // v^ - v'
+      if (!guided) return eat(j);
+      const size_t px = gm.pix(b, l, j);
+      return f[j] - ((eps[px] - y[px]) + wb * (f[j] - fu[j]));
+    };
+    auto dat = [&](int j) -> float { return __fmaf_rn(-tb, f[j], xat(j)); };   // x^ = x_t - t v^
+    float se = 0.f, sx = 0.f, sq = 0.f;
+    for (int j = 0; j < gm.pd; ++j) {
+      const size_t px = gm.pix(b, l, j);
+      const float xi = xt[px];
+      const float e = f[j] - (eps[px] - y[px]);
+      if (Dx) Dx[px] = __fmaf_rn(-tb, f[j], xi);
+      if constexpr (kReg) ev[j] = e, xv[j] = xi;
+      se += e * e, sx += xi;
+      if (guided) {
+        const float eg = gat(j);
+        sq += eg * eg;
+      }
+    }
+    if (!guided) sq = se;
+    const float inv_pd = 1.f / gm.pd;
+    if (!mask) {
+      acc += se;  // mean over all elements of the sample, applied below
+      acc_g += sq;
+      if (dF) {
+        const float k = glb * 2.f / (static_cast<float>(gm.L) * gm.pd);
+        for (int j = 0; j < gm.pd; ++j)
+          dF[(static_cast<size_t>(b) * gm.L + l) * gm.pd + j] = __float2bfloat16_rn(k * gat(j));
+      }
+    } else {
+      const float mk = mask[static_cast<size_t>(b) * gm.L + l];
+      float contrib = (1.f - mk) * se * inv_pd / n_keep;
+      float contrib_g = guided ? (1.f - mk) * sq * inv_pd / n_keep : contrib;
+      const float k_v = glb * (1.f - mk) / n_keep * 2.f * inv_pd;
+      float k_mae = 0.f, mu = 0.f, rstd = 0.f;
+      if (mae_coef > 0.f && mk != 0.f) {
+        // MaskDiT's MAE term with D replaced by x^, unchanged: target = per-patch normalised x_t, unbiased variance
+        mu = sx * inv_pd;
+        float var = 0.f;
+        for (int j = 0; j < gm.pd; ++j) var += (xat(j) - mu) * (xat(j) - mu);
+        var /= static_cast<float>(gm.pd - 1);
+        rstd = rsqrtf(var + 1e-6f);
+        float sm = 0.f;
+        for (int j = 0; j < gm.pd; ++j) {
+          const float e = dat(j) - (xat(j) - mu) * rstd;
+          sm += e * e;
+        }
+        const float m = mae_coef * mk * sm * inv_pd / n_mask;
+        contrib += m;
+        contrib_g += m;
+        k_mae = -tb * glb * mae_coef * mk / n_mask * 2.f * inv_pd;   // d x^ / d v^ = -t
+      }
+      acc += contrib;
+      acc_g += contrib_g;
+      if (dF) {
+        for (int j = 0; j < gm.pd; ++j) {
+          float gval = k_v * gat(j);
+          if (k_mae != 0.f) gval += k_mae * (dat(j) - (xat(j) - mu) * rstd);
+          dF[(static_cast<size_t>(b) * gm.L + l) * gm.pd + j] = __float2bfloat16_rn(gval);
+        }
+      }
+    }
+  }
+  const float tot = block_sum(acc_g, s_buf);
+  if (threadIdx.x == 0) loss[b] = mask ? tot : tot / (static_cast<float>(gm.L) * gm.pd);
+  if (mg.edm_loss) {
+    const float tp = block_sum(acc, s_buf);
+    if (threadIdx.x == 0) mg.edm_loss[b] = mask ? tp : tp / (static_cast<float>(gm.L) * gm.pd);
+  }
+}
+
 // u(sigma_b) alone, one block of 256 threads per sample: the loss kernel's arithmetic, so the same bits.
 __global__ void __launch_bounds__(256) logvar_kernel(const float* __restrict__ sigma, LogvarArgs lv) {
   __shared__ float s_buf[32];
@@ -1396,4 +1634,41 @@ int mdt_ect_loss(const float* Ft, const float* Fr, const float* xt, const float*
   return launch_status();
 }
 
+static bool mg_args_ok(const float* Fu, const float* labels, int num_classes, float w, float lo, float hi) {
+  return Fu && labels && num_classes >= 1 && w >= 0.f && w < 1.f && lo < hi;
+}
+
+int mdt_mg_loss(const float* F, const float* Fu, const float* xin, const float* y, const float* sigma,
+                const float* labels, int num_classes, const float* mask, const float* gl, float sigma_data,
+                float mae_coef, float w, float lo, float hi, float* loss, float* edm_loss, float* Dx, void* dF_bf16,
+                int B, int C, int R, int p, void* stream) {
+  if (!F || !xin || !y || !sigma || !loss || B <= 0 || !mg_args_ok(Fu, labels, num_classes, w, lo, hi))
+    return MDT_ERR_ARG;
+  if (dF_bf16 && !gl) return MDT_ERR_ARG;
+  PatchGeom gm;
+  if (int rc = make_geom(&gm, C, R, p)) return rc;
+  auto kern = gm.pd <= kMaxPD ? mg_loss_kernel<true> : mg_loss_kernel<false>;
+  kern<<<B, 256, 0, S(stream)>>>(F, xin, y, sigma, mask, gl, sigma_data, mae_coef, loss, Dx,
+                                 static_cast<__nv_bfloat16*>(dF_bf16), gm,
+                                 MgArgs{Fu, labels, num_classes, w, lo, hi, edm_loss});
+  return launch_status();
+}
+
+int mdt_flow_mg_loss(const float* F, const float* Fu, const float* xt, const float* y, const float* eps,
+                     const float* t, const float* labels, int num_classes, const float* mask, const float* gl,
+                     float mae_coef, float w, float lo, float hi, float* loss, float* edm_loss, float* x_hat,
+                     void* dF_bf16, int B, int C, int R, int p, void* stream) {
+  if (!F || !xt || !y || !eps || !t || !loss || B <= 0 || !mg_args_ok(Fu, labels, num_classes, w, lo, hi))
+    return MDT_ERR_ARG;
+  if (dF_bf16 && !gl) return MDT_ERR_ARG;
+  PatchGeom gm;
+  if (int rc = make_geom(&gm, C, R, p)) return rc;
+  auto kern = gm.pd <= kMaxPD ? flow_mg_loss_kernel<true> : flow_mg_loss_kernel<false>;
+  kern<<<B, 256, 0, S(stream)>>>(F, xt, y, eps, t, mask, gl, mae_coef, loss, x_hat,
+                                 static_cast<__nv_bfloat16*>(dF_bf16), gm,
+                                 MgArgs{Fu, labels, num_classes, w, lo, hi, edm_loss});
+  return launch_status();
+}
+
 }  // extern "C"
+

@@ -427,4 +427,124 @@ class ECTLoss:
         return loss
 
 
-Losses = {"edm": EDMLoss, "flow": FlowLoss, "ect": ECTLoss}
+def mg_weight(scale):
+    """Model guidance's w = 1 - 1/s of the CFG-equivalent scale s >= 1 (DESIGN §5)."""
+    s = float(scale)
+    if not s >= 1 or math.isinf(s):
+        raise ValueError(f"model guidance needs a finite scale s >= 1 (the CFG-equivalent scale), got {scale}")
+    return 1.0 - 1.0 / s
+
+
+class _FusedMGLossFn(torch.autograd.Function):
+    """Returns (objective, plain loss); the plain loss carries no gradient.  `eps` is None for EDM, the noise for
+    flow."""
+
+    @staticmethod
+    def forward(ctx, anchor, net, mg, xin, y, eps, sigma, labels, mask_dict, mae_coef):
+        # the null-label forward first: the student's saving forward must be the handle's last, its backward reads
+        # that workspace
+        Fu, _ = net._engine.forward(xin, sigma, torch.zeros_like(labels), mask_dict, save=False)
+        Fc, saved = net._engine.forward(xin, sigma, labels, mask_dict, save=True)
+        mask = mask_dict["mask"] if mask_dict is not None else None
+        loss, plain, _ = mg._kernel(net, Fc, Fu, xin, y, eps, sigma, labels, mask, None, mae_coef)
+        ctx.net, ctx.mg, ctx.saved = net, mg, saved
+        ctx.args = (Fc, Fu, xin, y, eps, sigma, labels, mask, mae_coef)
+        ctx.mark_non_differentiable(plain)
+        return loss, plain
+
+    @staticmethod
+    def backward(ctx, gl, _):
+        _, _, dF = ctx.mg._kernel(ctx.net, *ctx.args[:8], gl.contiguous().float(), ctx.args[8])
+        ctx.net._run_backward(ctx.saved, dF.view(-1, dF.shape[-1]))
+        ctx.saved = ctx.args = None
+        return (torch.zeros(1, device=gl.device),) + (None,) * 9
+
+
+class MGLoss:
+    """Model guidance (MG; Tang et al. 2025, in this repository's own definition, DESIGN §5) of a class-conditional
+    `EDMPrecond` or `FlowPrecond`: the network learns to output the guided denoiser, so it samples guided without
+    CFG's second pass.  The draws and the step front are those of `EDMLoss` / `FlowLoss` for the network given (MG
+    draws nothing more).  The student D_c carries the gradient; D_u is a no-gradient forward of the same weights on the
+    same input, noise level and kept tokens with the null (all-zero) label row.  Row b's target is
+    y + w_b sg(D_c - D_u), w_b = w = 1 - 1/scale where its label was kept and lo < sigma_b <= hi (flow: t), else 0;
+    the objective is MaskDiT's loss with that target in the denoising term (flow: v' = (eps - y) + w_b (F_c - F_u)).
+    The call returns the per-sample objective; `last_edm_loss` holds the plain loss against y (for the training log)
+    and `last_objective` the objective."""
+
+    def __init__(self, scale, interval=None, P_mean=None, P_std=None, sigma_data=0.5):
+        self.scale = float(scale)
+        self.w = mg_weight(scale)
+        lo, hi = (0.0, math.inf) if interval is None else (float(interval[0]), float(interval[1]))
+        if not lo < hi:
+            raise ValueError(f"model guidance needs an interval lo < hi, got [{lo}, {hi}]")
+        self.lo, self.hi = lo, hi
+        self.P_mean, self.P_std, self.sigma_data = P_mean, P_std, sigma_data
+
+    def _randn(self, shape, device):
+        return torch.randn(shape, device=device)
+
+    def _rand(self, shape, device):
+        return torch.rand(shape, device=device)
+
+    def _front(self, net):
+        """An `EDMLoss` or `FlowLoss` for `net` that draws through this object's hooks and finishes with MG."""
+        flow = isinstance(_unwrap(net), FlowPrecond)
+        kw = {k: v for k, v in (("P_mean", self.P_mean), ("P_std", self.P_std)) if v is not None}
+        front = FlowLoss(**kw) if flow else EDMLoss(sigma_data=self.sigma_data, **kw)
+        front._randn, front._rand = self._randn, self._rand
+        front._finish = self._finish_flow if flow else self._finish_edm
+        return front
+
+    def __call__(self, net, images, labels=None, mask_ratio=0, mae_loss_coef=0, feat=None, augment_pipe=None):
+        return self._front(net)(net, images, labels, mask_ratio, mae_loss_coef, feat, augment_pipe)
+
+    def from_moments(self, net, moments, labels=None, mask_ratio=0, mae_loss_coef=0, class_dropout_prob=0.0,
+                     scale_factor=0.18215, eps=None, drop_u=None):
+        """`EDMLoss.from_moments` / `FlowLoss.from_moments` of the network given, finished with MG."""
+        return self._front(net).from_moments(net, moments, labels, mask_ratio, mae_loss_coef, class_dropout_prob,
+                                             scale_factor, eps, drop_u)
+
+    def _kernel(self, raw, F, Fu, xin, y, eps, sigma, lab, mask, gl, coef):
+        p, want = raw.model.patch_size, gl is not None
+        if eps is None:
+            loss, plain, _, dF = ops.mg_loss(F, Fu, xin, y, sigma, lab, mask, gl, raw.sigma_data, coef, self.w,
+                                             self.lo, self.hi, p, want_dF=want)
+        else:
+            loss, plain, _, dF = ops.flow_mg_loss(F, Fu, xin, y, eps, sigma, lab, mask, gl, coef, self.w, self.lo,
+                                                  self.hi, p, want_dF=want)
+        return loss, plain, dF
+
+    def _finish_edm(self, raw, y, yn, sigma, labels, mask_ratio, mae_loss_coef):
+        return self._finish(raw, yn, y, None, sigma, labels, mask_ratio, mae_loss_coef)
+
+    def _finish_flow(self, raw, x, xt, eps, t, labels, mask_ratio, mae_loss_coef):
+        return self._finish(raw, xt, x, eps, t, labels, mask_ratio, mae_loss_coef)
+
+    def _finish(self, raw, xin, y, eps, sigma, labels, mask_ratio, mae_loss_coef):
+        if not raw.num_classes:
+            raise ValueError("Losses['mg'] guides a class-conditional network: this one has num_classes=0")
+        if raw.logvar_channels:
+            raise ValueError("Losses['mg'] does not train a learned loss weighting: build the network with "
+                             "logvar_channels=0")
+        dev, B = y.device, y.shape[0]
+        _, _, lab = raw._norm_inputs(y, sigma, labels)
+        md = None
+        if mask_ratio > 0:
+            assert raw.training, "masked loss needs net.train()"
+            L = raw.model.num_patches
+            md = ops.mask_indices(self._rand((B, L), dev), int(L * (1 - mask_ratio)))
+        coef = float(mae_loss_coef) if (mask_ratio > 0 and mae_loss_coef > 0) else 0.0
+        if torch.is_grad_enabled():
+            loss, plain = _FusedMGLossFn.apply(raw._anchor, raw, self, xin, y, eps, sigma, lab, md, coef)
+        else:
+            Fu, _ = raw._engine.forward(xin, sigma, torch.zeros_like(lab), md, save=False)
+            Fc, _ = raw._engine.forward(xin, sigma, lab, md, save=False)
+            loss, plain, _ = self._kernel(raw, Fc, Fu, xin, y, eps, sigma, lab, md["mask"] if md else None, None,
+                                          coef)
+        self.last_mask_dict = md
+        self.last_edm_loss = plain
+        self.last_objective = loss
+        return loss
+
+
+Losses = {"edm": EDMLoss, "flow": FlowLoss, "ect": ECTLoss, "mg": MGLoss}

@@ -296,6 +296,32 @@ def ect_loss(Ft, Fr, xt, xr, y, t, r, mask, gl, sigma_data, c, mae_coef, p, want
     return loss, D, dF
 
 
+def mg_loss(F, Fu, xin, y, sigma, labels, mask, gl, sigma_data, mae_coef, w, lo, hi, p, want_D=False, want_dF=True):
+    """Model-guidance loss of the student output F against the guided target built with the null-label output Fu
+    (mdt_mg_loss).  Returns (loss [B], the plain EDM loss [B], D or None, dF bf16 or None)."""
+    B, C, R, _ = xin.shape
+    loss, edm = torch.empty(B, dtype=f32, device=xin.device), torch.empty(B, dtype=f32, device=xin.device)
+    D = torch.empty_like(xin) if want_D else None
+    dF = torch.empty(F.shape, dtype=bf16, device=xin.device) if want_dF else None
+    check(lib().mdt_mg_loss(ptr(F), ptr(Fu), ptr(xin), ptr(y), ptr(sigma), ptr(labels), labels.shape[1], ptr(mask),
+                            ptr(gl), float(sigma_data), float(mae_coef), float(w), float(lo), float(hi), ptr(loss),
+                            ptr(edm), ptr(D), ptr(dF), B, C, R, p, stream_ptr()), "mdt_mg_loss")
+    return loss, edm, D, dF
+
+
+def flow_mg_loss(F, Fu, xt, y, eps, t, labels, mask, gl, mae_coef, w, lo, hi, p, want_xhat=False, want_dF=True):
+    """`mg_loss` on velocities (mdt_flow_mg_loss).  Returns (loss [B], the plain flow loss [B], x_hat or None, dF bf16
+    or None)."""
+    B, C, R, _ = xt.shape
+    loss, plain = torch.empty(B, dtype=f32, device=xt.device), torch.empty(B, dtype=f32, device=xt.device)
+    xh = torch.empty_like(xt) if want_xhat else None
+    dF = torch.empty(F.shape, dtype=bf16, device=xt.device) if want_dF else None
+    check(lib().mdt_flow_mg_loss(ptr(F), ptr(Fu), ptr(xt), ptr(y), ptr(eps), ptr(t), ptr(labels), labels.shape[1],
+                                 ptr(mask), ptr(gl), float(mae_coef), float(w), float(lo), float(hi), ptr(loss),
+                                 ptr(plain), ptr(xh), ptr(dF), B, C, R, p, stream_ptr()), "mdt_flow_mg_loss")
+    return loss, plain, xh, dF
+
+
 def flow_cfg_out(F, B, C, R, p, cfg_scale=None):
     """The velocity [B, C, R, R]: unpatchify(F), or with `cfg_scale` the CFG combine Fu + s (Fc - Fu) of F's two
     halves (cond rows first)."""

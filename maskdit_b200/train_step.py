@@ -17,7 +17,7 @@ import torch
 import torch.distributed as dist
 
 from . import ops, phema
-from .loss import ECTLoss, EDMLoss
+from .loss import ECTLoss, EDMLoss, MGLoss
 from .maskdit import EDMPrecond
 
 _GATHER_DTYPES = {torch.float32: 0, torch.bfloat16: 1, torch.float64: 2}   # MDT_DTYPE_F32 / _BF16 / _F64
@@ -790,9 +790,14 @@ class TrainStep:
         loss = out.clone()
         return loss, (out_edm.clone() if out_edm is not None else loss)
 
+    def _splits_loss(self):
+        """Whether the objective the gradient follows differs from the plain loss: a learned loss weighting, or model
+        guidance."""
+        return bool(self.net.logvar_channels) or isinstance(self.loss_fn, MGLoss)
+
     def _last_edm_loss(self):
-        """The reference loss of the last loss call when the network learns its loss weighting, else None."""
-        return self.loss_fn.last_edm_loss.detach() if self.net.logvar_channels else None
+        """The plain loss of the last loss call when the objective differs from it (`_splits_loss`), else None."""
+        return self.loss_fn.last_edm_loss.detach() if self._splits_loss() else None
 
     def step(self, images, labels, mask_ratio=0.5, mae_loss_coef=0.1, grad_accum=1, moments=False,
              class_dropout_prob=0.0):
@@ -807,6 +812,8 @@ class TrainStep:
         flat buffer anyway, so the rounds simply run back to back and 1/rounds is folded into the optimizer kernel.
         `moments=True`: `images` are VAE moments [B,2C,R,R] straight from the dataset; the latent sampling, the label
         dropout (`class_dropout_prob`) and the noise injection run as the fused step-front kernel (EDMLoss.from_moments).
+        With an `MGLoss` (model guidance) the returned tensor is the MG objective and `edm_loss` the plain EDM or flow
+        loss against the unguided target.
         With an `ECTLoss` the step runs at tuning stage s = floor((run step - ect_origin) / stage_steps), the run step
         being `step_count + lr_step_offset` before the call and `ect_origin` the run step of the first tuned step.
         Under `torch.use_deterministic_algorithms(True)` the library's deterministic mode is on for the step
@@ -867,7 +874,7 @@ class TrainStep:
                 losses.append(lr_.detach())
                 edm.append(self._last_edm_loss())
             loss = torch.cat(losses)
-            edm_loss = torch.cat(edm) if self.net.logvar_channels else loss
+            edm_loss = torch.cat(edm) if self._splits_loss() else loss
         elif self.graph and ops.L.GEMM_PROFILE is None:
             loss, edm_loss = self._fwd_bwd_graphed(images, labels, mask_ratio, mae_loss_coef, loss_call, moments)
         else:

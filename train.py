@@ -32,6 +32,13 @@ Consistency tuning (not in the reference): `train.objective: ect` with a `train.
 trained checkpoint with `--ckpt_path pre.pt --use_strict_load False` (weights and EMA, a fresh optimizer).  `Train Loss`
 is then the consistency loss and the log line appends the tuning stage; the `Val Loss` line stays the EDM denoising loss,
 which does not measure a tuned network's sample quality.
+Model guidance (not in the reference): `train.objective: mg` with a `train.mg:` block (`scale`, the CFG-equivalent
+scale s >= 1, and optional `interval: [lo, hi]`) trains a class-conditional EDM or flow network to output the guided
+denoiser (`Losses['mg']`, DESIGN §5), so it samples guided at one network pass per step without `--cfg_scale`.  It
+needs `model.class_dropout_prob > 0`, and fine-tunes from a trained checkpoint with `--ckpt_path pre.pt
+--use_strict_load False` as consistency tuning does.  `Train Loss` stays the plain EDM / flow loss, so it compares with
+a run without MG, and the log line appends `MG Loss`, the mean objective.  The `Val Loss` of an MG network is expected
+to be higher than without MG, because it learns guided outputs: it is not a quality measure for MG.
 """
 import argparse
 import copy
@@ -43,6 +50,7 @@ import torch.distributed as dist
 
 from maskdit_b200.config import build_loss, build_net, load_config, mask_ratio_schedule, parse_float_none, \
     parse_int_list
+from maskdit_b200.loss import MGLoss
 from maskdit_b200.train_step import TrainStep, check_max_grad_norm
 
 
@@ -69,11 +77,12 @@ def skip_nonfinite(args):
     return not args.no_amp
 
 
-def log_line(step, loss, steps_per_sec, skipped=None, grad_norm=None, weighted=None, ect_stage=None):
+def log_line(step, loss, steps_per_sec, skipped=None, grad_norm=None, weighted=None, ect_stage=None, mg=None):
     """The training log line (the reference's format, train.py:247); `skipped` (a count), `grad_norm` (the
-    window's mean and max), `weighted` (the mean objective of a learned loss weighting) and `ect_stage` (the
-    consistency-tuning stage of the last step) are appended only when given.  `loss` is the reference's loss, so it
-    compares across runs with and without the weighting (under consistency tuning, the consistency loss)."""
+    window's mean and max), `weighted` (the mean objective of a learned loss weighting), `ect_stage` (the
+    consistency-tuning stage of the last step) and `mg` (the mean model-guidance objective) are appended only when
+    given.  `loss` is the reference's loss, so it compares across runs with and without the weighting or model guidance
+    (under consistency tuning, the consistency loss)."""
     line = f"(step={step:07d}) Train Loss: {loss:.4f}, Train Steps/Sec: {steps_per_sec:.2f}"
     if skipped is not None:
         line += f", Skipped Steps: {skipped}"
@@ -83,6 +92,8 @@ def log_line(step, loss, steps_per_sec, skipped=None, grad_norm=None, weighted=N
         line += f", Weighted Loss: {weighted:.4f}"
     if ect_stage is not None:
         line += f", ECT stage: {ect_stage}"
+    if mg is not None:
+        line += f", MG Loss: {mg:.4f}"
     return line
 
 
@@ -236,6 +247,8 @@ def main():
             print(f"Validation: {len(held)} held-out items x {args.val_levels} noise levels every {args.val_every} "
                   f"steps", flush=True)
     log_every = cfg.log.log_every
+    guided = isinstance(loss_fn, MGLoss)
+    split = bool(net.logvar_channels) or guided   # the objective differs from the reference's loss
     running, weighted, log_steps, t0, step = 0.0, 0.0, 0, time.time(), step0
     gn_sum = gn_max = None   # the window's gradient norms, accumulated on the device like `running`
     recompute_shown = 0
@@ -246,8 +259,8 @@ def main():
         # moments -> latent (train.py:206), label dropout (:209), noise injection (loss.py:35-39): fused step front
         loss = ts.step(moments, labels, ratio, cfg.model.mae_loss_coef, grad_accum=rounds, moments=True,
                        class_dropout_prob=drop)
-        running = running + ts.edm_loss.mean()   # the reference's loss; the objective differs with a weighting
-        if net.logvar_channels:
+        running = running + ts.edm_loss.mean()   # the reference's loss; the objective differs with a weighting or MG
+        if split:
             weighted = weighted + loss.mean()
         if ts.grad_norm is not None:
             gn = ts.grad_norm
@@ -264,7 +277,7 @@ def main():
             break
         if step % log_every == 0:
             avg = running / log_steps
-            wavg = weighted / log_steps if net.logvar_channels else None
+            wavg = weighted / log_steps if split else None
             if world > 1:
                 dist.all_reduce(avg)
                 avg = avg / world
@@ -278,7 +291,8 @@ def main():
                 # every rank computes the same norm from the same summed gradient
                 gnorm = (float(gn_sum) / log_steps, float(gn_max)) if gn_sum is not None else None
                 print(log_line(step, float(avg), log_steps / (time.time() - t0), skipped, gnorm,
-                               float(wavg) if wavg is not None else None, ts.ect_stage), flush=True)
+                               float(wavg) if wavg is not None and not guided else None, ts.ect_stage,
+                               float(wavg) if guided else None), flush=True)
             running, weighted, log_steps, t0 = 0.0, 0.0, 0, time.time()
             gn_sum = gn_max = None
         if held is not None and step % args.val_every == 0:
